@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - ResNet50 pipeline-partitioned inference throughput on N B200s (BASELINE.json metric).
+"""bench.py - ResNet50 pipeline-partitioned inference throughput on N H100s (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W            # N = 1
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
@@ -64,10 +64,13 @@ def parse_args():
     ap.add_argument("--cpu-seconds", type=float, default=10.0)
     ap.add_argument("--batch1-roofline", action="store_true",
                     help="also time every op on a single-image microbatch (the un-coalesced launch)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (the last stage's per-image "
+                         "outputs, float32) to DIR/<name>.npy; inputs are seeded, so two builds compare output for output")
     return ap.parse_args()
 
 
-# engine defaults (measured on B200, profiles/README.md round 2): G queue items per launch, lanes per stage
+# engine defaults: G queue items per launch, lanes per stage
 DEFAULT_COALESCE = {"resnet50": 32, "resnet152": 16, "vgg16": 8}
 DEFAULT_DEPTH = 4
 
@@ -83,7 +86,8 @@ def load_peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 tensor rate - bounds, never reached
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ----------------------------------------------------------------------------------------------- clocks
@@ -162,13 +166,13 @@ def cpu_reference_run(model, n_stages, x, steps, warmup, seconds=None):
         t0 = time.perf_counter()
         n = 0
         while True:
-            stages[0].predict(x)
+            y = stages[0].predict(x)
             n += 1
             el = time.perf_counter() - t0
-            if (seconds is not None and el >= seconds) or (seconds is None and (n >= steps or el > 90.0)):
+            if (seconds is not None and el >= seconds) or (seconds is None and n >= steps):
                 break
         dt = time.perf_counter() - t0
-        return n / dt, dt / n * 1e3, cores, n
+        return n / dt, dt / n * 1e3, cores, n, y
     torch.set_num_threads(max(1, cores // n_stages))   # N stage threads share the host cores
     qs = [queue.Queue(8) for _ in range(n_stages + 1)]
     stop = threading.Event()
@@ -203,16 +207,15 @@ def cpu_reference_run(model, n_stages, x, steps, warmup, seconds=None):
         qs[-1].get()
     t0 = time.perf_counter()
     done = 0
+    y = None
     for _ in range(steps):
-        qs[-1].get()
+        y = qs[-1].get()
         done += 1
-        if time.perf_counter() - t0 > 90.0:      # bounded sample: stop counting after 90 s
-            break
     dt = time.perf_counter() - t0
     stop.set()
     for t in ths:
         t.join()
-    return done / dt, dt / done * 1e3, cores, done
+    return done / dt, dt / done * 1e3, cores, done, y
 
 
 def run_reference(args):
@@ -223,8 +226,12 @@ def run_reference(args):
     model = build_model(args.model)
     from defer_b200 import applications
     x = applications.synthetic_input(args.batch)
-    steps = min(args.steps, 400)
-    val, ms, cores, n = cpu_reference_run(model, args.gpus, x, steps, max(3, min(args.warmup, 10)))
+    val, ms, cores, n, y = cpu_reference_run(model, args.gpus, x, args.steps, max(3, min(args.warmup, 10)))
+    if args.dump_outputs:
+        # the reference path's output for the last timed queue item (same seeded input as the GPU arm)
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / "probs.npy", np.ascontiguousarray(y, np.float32))
     val *= args.batch
     sample = f"{n} predict calls of {args.model} batch {args.batch}, {args.gpus} stage(s), torch CPU (oneDNN) port"
     line = {"impl": "reference", "metric": "inferences_per_sec", "value": val, "unit": "inferences/s",
@@ -249,7 +256,7 @@ def workload_config(args):
                   "design; the per-kernel roofline numbers are taken with a 256 MB L2 flush between launches"}
 
 
-# ----------------------------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------------------------- GPU arm
 def run_b200(args):
     from defer_b200 import _cabi
     _cabi.load()                      # before torch initialises CUDA (sets CUDA_DEVICE_MAX_CONNECTIONS)
@@ -268,6 +275,8 @@ def run_b200(args):
         if world == 1 and args.gpus > 1:
             raise SystemExit(f"--gpus {args.gpus} needs torchrun with --nproc-per-node {args.gpus}")
         args.gpus = world
+    if args.dump_outputs and world > 1:
+        raise SystemExit("--dump-outputs needs a single-process run (the last stage's results stay on the last rank)")
     n_stages = args.gpus
     G = args.coalesce or DEFAULT_COALESCE[args.model]
     K, W, B = args.steps, max(args.warmup, 3), args.batch
@@ -404,21 +413,28 @@ def run_b200(args):
         r.mark_after(m1, 1)
     barrier_sync()
 
+    dumped = {}
+
     def direct_pass(n, start):
         """Issue n microbatches back to back, limited only by back-pressure (at most max_inflight in flight)."""
         if ctx is None:
             last_st = my_stages[-1]
             inflight = 0
             out = np.empty(last_st.out_shape, np.float32)
+
+            def collect(s):
+                last_st.result(s, out)
+                if s == m1:                      # the last timed step
+                    dumped["probs"] = out.copy()
             for s in range(start, start + n):
                 if inflight == depth:
-                    last_st.result(s - depth, out)
+                    collect(s - depth)
                     inflight -= 1
                 for r in my_stages:
                     r.step(s)
                 inflight += 1
             for s in range(start + n - inflight, start + n):
-                last_st.result(s, out)
+                collect(s)
             return
         # one process per GPU: rank 0 steps stage 0 and publishes `submitted`; node loops follow
         if rank == 0:
@@ -519,20 +535,6 @@ def run_b200(args):
     if rank == 0 and not args.no_roofline and ctx is None:
         rows = op_table(my_stages[0])
         roofline = roofline_of(rows, EB)
-        # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture (per launch, like `achieved`):
-        # well above the algorithmic bytes would mean wasted re-reads
-        tpath = ROOT / "profiles" / "ncu_traffic.json"
-        if tpath.exists():
-            try:
-                tr = json.loads(tpath.read_text())
-                key = f"{args.model}_{args.dtype}_b{EB}"
-                if key in tr:
-                    roofline["traffic"] = tr[key]["traffic_bytes_per_launch"]
-                    roofline["traffic_note"] = ("dram__bytes_read.sum + dram__bytes_write.sum per launch, mean of the launches in "
-                                                + tr[key]["source"] + "; algorithmic bytes per launch (mean over the step) = "
-                                                f"{roofline['alg_bytes_per_step'] / roofline['launches_per_step']:.0f}")
-            except Exception:   # a malformed side file must not take the bench line down
-                pass
         # the same algorithmic bytes over the TIMED REGION (all lanes overlapping): what the pipeline sustains, as
         # opposed to one launch timed alone behind an L2 flush
         try:
@@ -560,13 +562,19 @@ def run_b200(args):
                 one.close()
     cpu_baseline = None
     if rank == 0 and not args.no_cpu and n_stages == 1:
-        val, msc, cores, n = cpu_reference_run(model, 1, np.array(x1), 0, 3, seconds=args.cpu_seconds)
+        val, msc, cores, n, _ = cpu_reference_run(model, 1, np.array(x1), 0, 3, seconds=args.cpu_seconds)
         cpu_baseline = {"value": val * B, "unit": "inferences/s", "cores": cores, "kind": "port",
                         "sample": f"{n} predict calls in {args.cpu_seconds:.0f} s of {args.model} batch {B} "
                                   "(oracle/torch_cpu.py, oneDNN, all host threads; test/local_infer.py protocol)",
                         "host_cpus": os.cpu_count()}
 
     # =========================================================================== shut down + report
+    if args.dump_outputs and rank == 0:
+        # probabilities of the G images of the last timed microbatch, as the last stage returned them
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        for name, arr in dumped.items():
+            np.save(out_dir / f"{name}.npy", np.ascontiguousarray(arr, np.float32))
     if rank == 0:
         defer.close()
     if ctx is not None:

@@ -1,6 +1,6 @@
-"""defer_b200 - Blackwell-native pipeline-partitioned inference with the DEFER API.
+"""defer_b200 - Hopper-native (H100) pipeline-partitioned inference with the DEFER API.
 
-Public surface mirrors the reference (``/root/reference/src``): ``DEFER`` (dispatcher), ``Node``,
+Public surface mirrors the reference (``src``): ``DEFER`` (dispatcher), ``Node``,
 ``NodeState``, ``dag_util.construct_model``; model builders stand in for ``keras.applications``.
 """
 from . import keras_like, applications, dag_util  # noqa: F401

@@ -1,7 +1,7 @@
 """ResNet50 / ResNet152 / VGG16 builders with Keras layer names and Keras arithmetic.
 
 The reference imports these from ``tensorflow.python.keras.applications``
-(``/root/reference/test/test.py:3,14``, ``test/local_infer.py:3,8``).  Graphs follow
+(``test/test.py:3,14``, ``test/local_infer.py:3,8``).  Graphs follow
 ``keras_applications`` 1.0.8 (restated, not vendored - see SURVEY.md 8c):
 
 * ``ResNet50``: old-style ``resnet50.py`` - stride on the first 1x1 conv and on the projection

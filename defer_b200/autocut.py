@@ -1,6 +1,6 @@
 """Balanced cut selection - the caller side of ``DEFER._partition`` (SURVEY.md 8f, rank 1).
 
-The reference takes the cut list by hand (``/root/reference/test/test.py:15-18``); pipeline throughput is
+The reference takes the cut list by hand (``test/test.py:15-18``); pipeline throughput is
 1 / max(stage time), so a poorly balanced list wastes GPUs (with the reference's own 8-stage list the
 first stage - stem + 3 residual blocks - is ~2x the median stage).  ``balanced_cuts`` picks the cut layers
 that minimise the slowest stage:
@@ -21,7 +21,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .planner import Plan, plan_stage
 
-HBM_GBS = 6572.0          # MEASURED_PEAKS.json on this pool's B200s
+HBM_GBS = 3350.0          # H100 SXM data-sheet HBM3 bandwidth
 LAUNCH_US = 2.0           # per-launch cost with several microbatches in flight (device launch rate)
 
 

@@ -1,6 +1,4 @@
 // api_kernels.cu - per-kernel C-ABI entry points (raw device pointers) for parity tests and ncu.
-#include <stdlib.h>
-
 #include <vector>
 
 #include "common.cuh"
@@ -19,154 +17,34 @@ int defer_k_conv(int fmt, int backend, const void* x, int x_is_f32, const float*
   int ho = (h + pad_t + pad_b - kh) / sh + 1, wo = (w + pad_l + pad_r - kw) / sw + 1;
   DEFER_CHECK(ho >= 1 && wo >= 1, "k_conv: empty output");
   if (residual) flags |= DEFER_FLAG_RESIDUAL;
-  if (backend >= 4 && backend <= 7) {
-    // streaming persistent kernel (conv_stream_kernel): 4 = 64-wide N tiles, 5 = 128-wide, 6 / 7 = the same with the
-    // per-thread (peer-memory capable) epilogue that a stage's last conv uses when its output is the next GPU's slot
-    DEFER_CHECK(fmt != DEFER_FMT_F32 && !x_is_f32, "k_conv: tcgen05 backend needs BF16X2/BF16 activations");
+  if (backend >= 2 && backend <= 7) {
+    // 2: one tile per CTA (conv_umma_kernel) | 3: persistent grid, 64-wide N tiles | 4 / 5: streaming persistent kernel
+    // with 64- / 128-wide N tiles | 6 / 7: the same, planned for an output in a peer GPU's slot
+    DEFER_CHECK(fmt != DEFER_FMT_F32 && !x_is_f32, "k_conv: wgmma backend needs BF16X2/BF16 activations");
     DEFER_CHECK(umma_conv_supported(fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l),
-                "k_conv: shape not supported by the tcgen05 kernel");
+                "k_conv: shape not supported by the wgmma kernel");
     UmmaConvPlan plan;
     UmmaConvLaneArgs args;
     void* dev_op = nullptr;
-    const int want_bn = (backend & 1) ? 128 : 64;
+    const int stream_bn = backend >= 4 ? ((backend & 1) ? 128 : 64) : 0;
     int rc = umma_conv_prepare(&plan, fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l, flags, w_hwio, scale, shift,
-                               /*mega=*/false, /*stream_bn=*/want_bn);
+                               /*mega=*/backend == 3, stream_bn);
     args.direct_out = backend >= 6;
     if (rc == DEFER_OK) rc = umma_conv_bind(plan, &args, x, residual, y);
-    long long* trace = nullptr;
-    const char* trace_path = getenv("DEFER_UMMA_TRACE");
-    if (rc == DEFER_OK && trace_path) {
-      cudaMalloc((void**)&trace, 8 * 64 * sizeof(long long));
-      cudaMemset(trace, 0, 8 * 64 * sizeof(long long));
-      args.trace = trace;
-    }
-    std::vector<unsigned char> host(umma_mega_op_bytes());
-    if (rc == DEFER_OK) rc = umma_mega_fill(host.data(), plan, args);
-    if (rc == DEFER_OK && cudaMalloc(&dev_op, host.size()) != cudaSuccess) rc = DEFER_ERR_CUDA;
-    if (rc == DEFER_OK) cudaMemcpy(dev_op, host.data(), host.size(), cudaMemcpyHostToDevice);
     const int n_tiles = plan.tiles_n * plan.tiles_h * plan.tiles_w * (cout / plan.bn);
-    if (rc == DEFER_OK && trace) {   // warm-up so the traced launch sees warm descriptor / instruction caches
-      rc = launch_conv_stream(plan.nplanes, plan.bn, dev_op, n_tiles, plan.k_blocks, st);
-      cudaStreamSynchronize(st);
-      cudaMemset(trace, 0, 8 * 64 * sizeof(long long));
+    if (backend == 2) {
+      if (rc == DEFER_OK) rc = launch_conv_umma(plan, args, st);
+    } else {
+      std::vector<unsigned char> host(umma_mega_op_bytes());
+      if (rc == DEFER_OK) rc = umma_mega_fill(host.data(), plan, args);
+      if (rc == DEFER_OK && cudaMalloc(&dev_op, host.size()) != cudaSuccess) rc = DEFER_ERR_CUDA;
+      if (rc == DEFER_OK) cudaMemcpy(dev_op, host.data(), host.size(), cudaMemcpyHostToDevice);
+      if (rc == DEFER_OK)
+        rc = backend == 3 ? launch_conv_persistent(plan.nplanes, dev_op, n_tiles, st)
+                          : launch_conv_stream(plan.nplanes, plan.bn, dev_op, n_tiles, plan.k_blocks, st);
     }
-    if (rc == DEFER_OK) rc = launch_conv_stream(plan.nplanes, plan.bn, dev_op, n_tiles, plan.k_blocks, st);
     cudaError_t e = cudaStreamSynchronize(st);
-    if (trace) {
-      long long hb[8 * 64];
-      cudaMemcpy(hb, trace, sizeof hb, cudaMemcpyDeviceToHost);
-      FILE* f = fopen(trace_path, "a");
-      if (f) {
-        fprintf(f, "# stream conv backend=%d n=%d hw=%dx%d cin=%d cout=%d k=%d s=%d bn=%d tiles=%d k_blocks=%d (ns since the first stamp)\n", backend,
-                n, h, w, cin, cout, kh, sh, plan.bn, n_tiles, plan.k_blocks);
-        for (int i = 0; i < 8; ++i) {
-          if (!hb[i * 64]) continue;
-          fprintf(f, "tile %d:", i);
-          for (int j = 0; j < 64; ++j)
-            if (hb[i * 64 + j]) fprintf(f, " %d=%lld", j, hb[i * 64 + j] - hb[0]);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-      cudaFree(trace);
-    }
     if (dev_op) cudaFree(dev_op);
-    umma_conv_unbind(&args);
-    umma_conv_release(plan);
-    if (rc != DEFER_OK) return rc;
-    DEFER_CUDA(e);
-    return DEFER_OK;
-  }
-  if (backend == 3) {
-    // persistent-grid tcgen05 kernel (the mode the stage runtime picks for ops with many tiles)
-    DEFER_CHECK(fmt != DEFER_FMT_F32 && !x_is_f32, "k_conv: tcgen05 backend needs BF16X2/BF16 activations");
-    DEFER_CHECK(umma_conv_supported(fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l),
-                "k_conv: shape not supported by the tcgen05 kernel");
-    UmmaConvPlan plan;
-    UmmaConvLaneArgs args;
-    void* dev_op = nullptr;
-    long long* trace = nullptr;
-    const char* trace_path = getenv("DEFER_UMMA_TRACE");
-    int rc = umma_conv_prepare(&plan, fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l, flags, w_hwio, scale, shift,
-                               /*mega=*/true);
-    if (rc == DEFER_OK) rc = umma_conv_bind(plan, &args, x, residual, y);
-    if (rc == DEFER_OK && trace_path) {
-      cudaMalloc((void**)&trace, 24 * 8 * sizeof(long long));
-      cudaMemset(trace, 0, 24 * 8 * sizeof(long long));
-      args.trace = trace;
-    }
-    std::vector<unsigned char> host(umma_mega_op_bytes());
-    if (rc == DEFER_OK) rc = umma_mega_fill(host.data(), plan, args);
-    if (rc == DEFER_OK && cudaMalloc(&dev_op, host.size()) != cudaSuccess) rc = DEFER_ERR_CUDA;
-    if (rc == DEFER_OK) cudaMemcpy(dev_op, host.data(), host.size(), cudaMemcpyHostToDevice);
-    const int n_tiles = plan.tiles_n * plan.tiles_h * plan.tiles_w * (cout / 64);
-    if (rc == DEFER_OK && trace) {   // warm-up so the traced launch sees warm descriptor / instruction caches
-      rc = launch_conv_persistent(plan.nplanes, dev_op, n_tiles, st);
-      cudaStreamSynchronize(st);
-      cudaMemset(trace, 0, 24 * 8 * sizeof(long long));
-    }
-    if (rc == DEFER_OK) rc = launch_conv_persistent(plan.nplanes, dev_op, n_tiles, st);
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (trace) {
-      long long hb[24 * 8];
-      cudaMemcpy(hb, trace, sizeof hb, cudaMemcpyDeviceToHost);
-      FILE* f = fopen(trace_path, "a");
-      if (f) {
-        fprintf(f, "# persistent conv n=%d hw=%dx%d cin=%d cout=%d k=%d s=%d tiles=%d\n", n, h, w, cin, cout, kh, sh, n_tiles);
-        for (int i = 0; i < 24; ++i) {
-          if (!hb[i * 8]) continue;
-          fprintf(f, "%d", i);
-          for (int j = 0; j < 8; ++j) fprintf(f, " %lld", hb[i * 8 + j] ? hb[i * 8 + j] - hb[0] : -1);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-      cudaFree(trace);
-    }
-    if (dev_op) cudaFree(dev_op);
-    umma_conv_unbind(&args);
-    umma_conv_release(plan);
-    if (rc != DEFER_OK) return rc;
-    DEFER_CUDA(e);
-    return DEFER_OK;
-  }
-  if (backend == 2) {
-    DEFER_CHECK(fmt != DEFER_FMT_F32 && !x_is_f32, "k_conv: tcgen05 backend needs BF16X2/BF16 activations");
-    DEFER_CHECK(umma_conv_supported(fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l),
-                "k_conv: shape not supported by the tcgen05 kernel");
-    UmmaConvPlan plan;
-    UmmaConvLaneArgs args;
-    int rc = umma_conv_prepare(&plan, fmt, n, h, w, cin, ho, wo, cout, kh, kw, sh, sw, pad_t, pad_l, flags, w_hwio, scale, shift);
-    if (rc == DEFER_OK) rc = umma_conv_bind(plan, &args, x, residual, y);
-    long long* trace = nullptr;
-    int n_ctas = plan.tiles_n * plan.tiles_h * plan.tiles_w * (plan.cout / plan.bn) * plan.splits;
-    const char* trace_path = getenv("DEFER_UMMA_TRACE");
-    if (rc == DEFER_OK && trace_path) {
-      cudaMalloc((void**)&trace, (size_t)n_ctas * 8 * sizeof(long long));
-      cudaMemset(trace, 0, (size_t)n_ctas * 8 * sizeof(long long));
-      args.trace = trace;
-      rc = launch_conv_umma(plan, args, st);   // warm-up launch (descriptor / instruction caches)
-      cudaStreamSynchronize(st);
-    }
-    if (rc == DEFER_OK) rc = launch_conv_umma(plan, args, st);
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (trace) {
-      long long* h = (long long*)malloc((size_t)n_ctas * 8 * sizeof(long long));
-      cudaMemcpy(h, trace, (size_t)n_ctas * 8 * sizeof(long long), cudaMemcpyDeviceToHost);
-      FILE* f = fopen(trace_path, "a");
-      if (f) {
-        fprintf(f, "# conv n=%d h=%d w=%d cin=%d cout=%d k=%d s=%d bn=%d splits=%d stages=%d ctas=%d\n", n, h, w, cin, cout, kh, sh,
-                plan.bn, plan.splits, plan.stages, n_ctas);
-        for (int i = 0; i < n_ctas; ++i) {
-          long long* t = h + 8 * i;
-          fprintf(f, "%d %lld %lld %lld %lld %lld %lld %lld\n", i, t[7], t[1] - t[0], t[2] - t[0], t[3] - t[0], t[4] - t[0],
-                  t[5] - t[0], t[6] - t[0]);
-        }
-        fclose(f);
-      }
-      free(h);
-      cudaFree(trace);
-    }
     umma_conv_unbind(&args);
     umma_conv_release(plan);
     if (rc != DEFER_OK) return rc;

@@ -1,4 +1,4 @@
-// common.cuh - shared helpers for libdefer_b200 (sm_100a only).
+// common.cuh - shared helpers for libdefer_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -42,7 +42,7 @@ const char* get_error();
 // ---------------------------------------------------------------------------------------------
 // Every kernel of the library asks for the same (maximum) shared-memory carve-out.  Lanes run
 // concurrently on one GPU; CTAs of kernels that want different L1/shared splits cannot share an SM, and
-// switching the split drains it.  One uniform configuration lets tiny SIMT kernels and 200 KB tcgen05
+// switching the split drains it.  One uniform configuration lets tiny SIMT kernels and 200 KB wgmma
 // tiles co-reside.  Called once per (kernel, device).
 // ---------------------------------------------------------------------------------------------
 void prefer_max_smem_impl(const void* func);
@@ -153,7 +153,7 @@ struct ConvParams {
 };
 
 int launch_conv_simt(int fmt, bool x_is_f32, const ConvParams& p, cudaStream_t st);
-// tensor-core stem: fp32 image -> [pixels, K_pad] patch matrix in the stage format (then a 1x1 tcgen05 conv)
+// tensor-core stem: fp32 image -> [pixels, K_pad] patch matrix in the stage format (then a 1x1 wgmma conv)
 int launch_stem_im2col(int fmt, const float* x, void* out, int n, int h, int w, int cin, int kh, int kw, int sh, int sw,
                        int pad_t, int pad_l, int ho, int wo, int K_pad, cudaStream_t st);
 int launch_maxpool(int fmt, const void* x, void* y, int n, int h, int w, int c, int ph, int pw, int sh, int sw,

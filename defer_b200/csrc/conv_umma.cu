@@ -1,4 +1,4 @@
-// conv_umma.cu - tcgen05 implicit-GEMM convolution for sm_100a.
+// conv_umma.cu - wgmma implicit-GEMM convolution for sm_90a (Hopper).
 //
 // The contraction of every Conv2D whose C_in is a multiple of 64 (all ResNet / VGG convs but the
 // RGB stem).  GEMM view: M = output pixels, N = C_out, K = taps x C_in.
@@ -8,21 +8,25 @@
 //     TMA zero-fills out-of-bounds elements, which IS the 'same' / ZeroPadding2D border, and its
 //     element strides do stride-2 sub-sampling.  1x1/stride-1 convs use the flat [M, C] view.
 //   * B (weights) is pre-arranged once as [tap][C_out][C_in] bf16 (K-major), a 3-D TMA box.
-//   * Both land in 128B-swizzled shared memory and feed tcgen05.mma (M=128, N=BN, K=16) issued by
-//     one thread; the fp32 accumulator lives in TMEM.
+//   * Both land in 128B-swizzled shared memory (a ring of stages guarded by mbarriers) and feed
+//     wgmma.mma_async m64nBNk16 issued by two consumer warpgroups (rows 0-63 and 64-127 of the tile);
+//     the fp32 accumulator lives in their registers.
 //   * BF16X2 format (fp32 parity path): activations and weights are (hi, lo) bf16 planes and each
-//     K step issues hi*hi + lo*hi + hi*lo  (bf16x3, ~2^-16 relative) into the same accumulator.
-//   * Epilogue (4 warps): tcgen05.ld -> per-channel scale/shift (bias + BN) -> + residual -> relu ->
-//     re-split to bf16 planes -> global stores (plain st.global, so the output may be a peer GPU's
-//     input slot: the hop is fused into the kernel).
-//   * Optional split-K over grid.z for weight-heavy small-M layers (7x7, 14x14 maps at batch 1):
-//     partial tiles go to an fp32 workspace; the last CTA of a tile reduces them in a fixed order.
+//     K = 16 step issues hi*hi + lo*hi + hi*lo (bf16x3, ~2^-16 relative) into the same accumulator.
+//   * Epilogue (the consumer warpgroups, straight from the accumulator registers): per-channel
+//     scale/shift (bias + BN) -> + residual -> relu -> re-split to bf16 planes -> st.global (plain
+//     stores, so the output may be a peer GPU's input slot: the hop is fused into the kernel).
+//   * Split-K for weight-heavy small-M layers (7x7, 14x14 maps at batch 1): either partial tiles in an
+//     fp32 workspace reduced by the last-arriving CTA, or (DEFER_UMMA_CLUSTER=1) the splits of a tile as
+//     one thread-block cluster reducing through distributed shared memory.  Both sum in a fixed order.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM alloc + MMA issuer, warps 2-5 = epilogue.
+// Warp roles (384 threads): warpgroups 0-1 consume (wgmma + epilogue), warpgroup 2 produces (one thread
+// issues the TMA loads; for the fused RGB stem all 128 threads build the A operand from the fp32 image).
+// The same body runs one tile per CTA (conv_umma_kernel) or walks a tile list (conv_stream_kernel:
+// persistent grid, or one cluster walking a run of ops separated by cluster barriers).
 #include <cuda.h>
 #include <string.h>
 
-#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -30,15 +34,21 @@
 
 namespace defer {
 
-static int env_int(const char* name, int dflt);
+static int env_int(const char* name, int dflt) {
+  const char* v = getenv(name);
+  return v ? atoi(v) : dflt;
+}
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M
+constexpr int BM = 128;          // M tile: two wgmma m64 halves
 constexpr int BK = 64;           // K elements per stage (128 B of bf16 = one swizzle atom row)
-constexpr int UMMA_K = 16;
-constexpr int NUM_THREADS = 192;
-constexpr int EPI_THREADS = 128;
+constexpr int CONS_THREADS = 256;
+constexpr int NUM_THREADS = CONS_THREADS + 128;
+constexpr int SMEM_CAP = 227 * 1024 - 256;   // opt-in shared memory per block on H100 (227 KB), less static smem
+constexpr int CTL_BYTES = 256;         // mbarriers
+constexpr int MAX_STAGES = 8;
+constexpr int MEGA_BN = 64;
 
 struct KParams {
   // geometry
@@ -51,10 +61,6 @@ struct KParams {
   int k_blocks;                                   // taps * cblocks
   int splits;
   int cluster;                                    // 1: the `splits` CTAs of a tile form one thread-block cluster (DSMEM reduction)
-  int tma_epi;                                    // 1: staged epilogue - residual tile in by TMA, finished tile out by TMA store
-  int fast;                                       // opt-in (DEFER_UMMA_FAST): bit 0 scale/shift loads off the setup critical path, bit 1 wait only for the bulk store's smem reads
-  int res_stage_bytes;                            // smem reserved for the residual tile (0 without residual / tma_epi)
-  int stages;
   uint32_t flags;
   const float* scale;
   const float* shift;
@@ -63,12 +69,33 @@ struct KParams {
   float* partial;
   unsigned int* counters;
   size_t plane_out;                               // n*ho*wo*cout (elements) - offset of the lo plane
-  int* error_flag;
-  long long* trace;     // optional: 8 clock64 stamps per CTA (debug instrumentation)
-  long long* timeline;  // optional (DEFER_TIMELINE): device-wide log, [0] = cursor, then 8 words per CTA
-  int timeline_cap;
-  int timeline_tag;
-  int pdl;              // launched with programmatic stream serialization: wait for the producer grid before reading
+};
+
+// One op as the kernels read it (kernel parameter or device memory).
+struct alignas(128) MegaOp {
+  CUtensorMap tmx[2];
+  CUtensorMap tmw[2];
+  KParams p;
+  int m_tiles, n_tiles;     // tiles of this op: m fastest
+  // fused stem: the fp32 NHWC image the patch rows are built from, and the real conv geometry
+  const float* stem_x;
+  int stem_h, stem_w, stem_cin, stem_kh, stem_kw, stem_sh, stem_sw, stem_pad_t, stem_pad_l, stem_K;
+};
+
+template <int NPLANES, int BN>
+struct Smem {
+  static constexpr int A_PLANE = BM * 128;   // bytes
+  static constexpr int B_PLANE = BN * 128;
+  static constexpr int STAGE = NPLANES * (A_PLANE + B_PLANE);
+  static constexpr int RED = BM * BN * 4;    // fp32 partial tile of the cluster split-K reduction
+  __host__ __device__ static constexpr int ring(int stages, bool red) {
+    return (red && stages * STAGE < RED) ? RED : stages * STAGE;
+  }
+  // + slack for the manual 1024-B alignment of the dynamic smem base
+  __host__ __device__ static constexpr int total(int stages, bool red) { return ring(stages, red) + CTL_BYTES + 1024; }
+  __host__ __device__ static constexpr int max_stages() {
+    return (SMEM_CAP - CTL_BYTES - 1024) / STAGE > MAX_STAGES ? MAX_STAGES : (SMEM_CAP - CTL_BYTES - 1024) / STAGE;
+  }
 };
 
 // ---------------------------------------------------------------------------------------------- PTX helpers
@@ -77,8 +104,14 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
@@ -96,17 +129,17 @@ __device__ __forceinline__ unsigned long long gtimer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Bounded wait: a protocol bug must surface as an error, never as a hung GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* error_flag, int tag) {
+// Bounded wait: a protocol bug must surface as an error, never as a hung GPU.  No function call on this path (a call
+// inside the main loop would make ptxas serialize every wgmma), so the timeout only records its tag before trapping.
+__device__ int g_conv_wait_timeout_tag;
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag) {
   if (mbar_try_wait(bar, parity)) return;
   unsigned long long t0 = gtimer();
   unsigned spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if ((++spins & 0xfff) == 0 && gtimer() - t0 > 2000000000ull) {
-      if (error_flag) atomicExch(error_flag, 100 + tag);
-      printf("conv_umma: mbarrier wait timeout tag=%d block=(%d,%d,%d) thread=%d\n", tag, blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x);
-      __trap();
+      g_conv_wait_timeout_tag = tag;
+      asm volatile("trap;");
     }
   }
 }
@@ -123,58 +156,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// SWIZZLE_128B, K-major smem matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO(=1)<<16 |
-// SBO(=1024 B >> 4)<<32 | version(=1)<<46 | layout_type(=2, SWIZZLE_128B)<<61
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-
-// ---- TMA store (bulk async group) helpers
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(map)),
-               "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
 // ---- thread-block cluster / distributed shared memory
@@ -203,43 +184,65 @@ __device__ __forceinline__ float4 dsmem_ld4(uint32_t addr) {
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ uint4 lds4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
+__device__ __forceinline__ void cons_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void prod_bar_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
+
+// ---- wgmma
+// SWIZZLE_128B, K-major shared-memory matrix descriptor (sm_90 GMMA): start>>4 | LBO(=16 B, unused for swizzled
+// K-major)>>4 << 16 | SBO(=1024 B: one 8-row swizzle atom)>>4 << 32 | layout SWIZZLE_128B (1) << 62.  The K = 16
+// slices of a 64-wide row start 32 B apart inside the swizzle atom.
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void sts4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+// keeps the compiler from touching accumulator registers across an outstanding wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1),
-// K-major A and B (bits 15, 16 = 0), N>>3 at bit 17, M>>4 at bit 24
+// D[64 x BN] (+)= A[64 x 16] * B[BN x 16]^T, bf16 in, fp32 accumulate, both operands K-major in shared memory
 template <int BN>
-__device__ __forceinline__ constexpr uint32_t make_idesc() {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t a, uint64_t b);
+
+template <>
+__device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1));
 }
 
-template <int NPLANES, int BN>
-struct SmemLayout {
-  static constexpr int A_PLANE = BM * 128;          // bytes
-  static constexpr int B_PLANE = BN * 128;
-  static constexpr int STAGE = NPLANES * (A_PLANE + B_PLANE);
-  static constexpr int MAX_STAGES = (200 * 1024) / STAGE > 8 ? 8 : (200 * 1024) / STAGE;
-  // layout for a run-time ring depth `stages`: [stages x STAGE | barriers 256 B | scale, shift]
-  __host__ __device__ static constexpr int bar_off(int stages) { return stages * STAGE; }
-  __host__ __device__ static constexpr int scale_off(int stages) { return stages * STAGE + 256; }
-  // + slack for the manual 1024-B alignment of the dynamic smem base
-  __host__ __device__ static constexpr int total(int stages) { return stages * STAGE + 256 + 2 * BN * 4 + 1024; }
-};
-
-// rows of one output / residual tile box (what a TMA load of it delivers, OOB rows included)
-__device__ __forceinline__ uint32_t a_rows_out(const KParams& p) {
-  return p.flat ? (uint32_t)BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
+template <>
+__device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
+      "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, "
+      "1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(1));
 }
 
 // accumulator row r of the tile at (n0, h0, w0) -> output pixel (linear NHW index) and whether it exists
@@ -259,1790 +262,348 @@ __device__ __forceinline__ void row_to_pixel(const KParams& p, int r, int n0, in
   }
 }
 
-// ---------------------------------------------------------------------------------------------- the kernel
-// EW = epilogue warps: 4 (192 threads, 2 CTAs/SM) or 8 (320 threads, 1 CTA/SM; warp pairs split the columns)
-// TMEM -> registers for 32 accumulator columns of the fp32-parity scheme with the 2*BN-row B operand: the hi-term block
-// [0, BN) plus the a_hi x b_lo block [BN, 2BN) of the same output columns (see conv_stream_kernel)
-template <int NPLANES, int BN>
-__device__ __forceinline__ void tmem_ld32_acc(uint32_t taddr, uint32_t (&v)[32]) {
-  tmem_ld32(taddr, v);
-  if constexpr (NPLANES == 2) {
-    uint32_t v2[32];
-    tmem_ld32(taddr + BN, v2);
-#pragma unroll
-    for (int q = 0; q < 32; ++q) v[q] = __float_as_uint(__uint_as_float(v[q]) + __uint_as_float(v2[q]));
+// bias/BN, residual, ReLU and the store of two adjacent channels (c, c + 1) of one output pixel
+template <int NPLANES>
+__device__ __forceinline__ void epi_pair(const KParams& p, size_t pix, int c, float v0, float v1) {
+  const float2 sc = p.scale ? __ldg(reinterpret_cast<const float2*>(p.scale + c)) : make_float2(1.f, 1.f);
+  const float2 sf = p.shift ? __ldg(reinterpret_cast<const float2*>(p.shift + c)) : make_float2(0.f, 0.f);
+  v0 = fmaf(v0, sc.x, sf.x);
+  v1 = fmaf(v1, sc.y, sf.y);
+  const size_t o = pix * p.cout + c;
+  if (p.res) {
+    const __nv_bfloat16* r = reinterpret_cast<const __nv_bfloat16*>(p.res) + o;
+    const __nv_bfloat162 h = *reinterpret_cast<const __nv_bfloat162*>(r);
+    v0 += __low2float(h);
+    v1 += __high2float(h);
+    if (NPLANES == 2) {
+      const __nv_bfloat162 l = *reinterpret_cast<const __nv_bfloat162*>(r + p.plane_out);
+      v0 += __low2float(l);
+      v1 += __high2float(l);
+    }
+  }
+  if (p.flags & DEFER_FLAG_RELU) {
+    v0 = fmaxf(v0, 0.f);
+    v1 = fmaxf(v1, 0.f);
+  }
+  uint32_t* y = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o);
+  if (NPLANES == 2) {
+    uint32_t hi, lo;
+    split_bf16x2(v0, v1, hi, lo);
+    y[0] = hi;
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
+  } else {
+    y[0] = pack_bf16x2(v0, v1);
   }
 }
 
-template <int NPLANES, int BN, int EW>
-__global__ void __launch_bounds__(64 + 32 * EW, EW == 4 ? 2 : 1)
-conv_umma_kernel(const __grid_constant__ CUtensorMap tmx0, const __grid_constant__ CUtensorMap tmx1,
-                 const __grid_constant__ CUtensorMap tmw0, const __grid_constant__ CUtensorMap tmw1,
-                 const __grid_constant__ CUtensorMap tmy0, const __grid_constant__ CUtensorMap tmy1,
-                 const __grid_constant__ CUtensorMap tmr0, const __grid_constant__ CUtensorMap tmr1, const KParams p) {
-  using L = SmemLayout<NPLANES, BN>;
+// Fused RGB stem: the producer warpgroup writes one k-block of the A operand (128 patch rows x 64 k, bf16 hi / lo
+// planes) in the SWIZZLE_128B layout TMA would have produced.  In NHWC a patch is kh runs of kw*cin contiguous floats,
+// so k -> (kernel row a, offset jj) and one range check on the flat column index covers the left / right padding.
+template <int NPLANES>
+__device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int m0, int kb, int r) {
+  const KParams& p = op.p;
+  const int m = m0 + r;
+  const int run = op.stem_kw * op.stem_cin, wc = op.stem_w * op.stem_cin;
+  const float* img = nullptr;
+  int ih0 = 0, col0 = 0;
+  if (m < p.m_total) {
+    const int hw = p.ho * p.wo;
+    const int im = m / hw, rem = m - im * hw, oh = rem / p.wo, ow = rem - oh * p.wo;
+    img = op.stem_x + (size_t)im * op.stem_h * wc;
+    ih0 = oh * op.stem_sh - op.stem_pad_t;
+    col0 = (ow * op.stem_sw - op.stem_pad_l) * op.stem_cin;
+  }
+  int k = kb * BK;
+  int a = k / run, jj = k - a * run;
+#pragma unroll 1
+  for (int ch = 0; ch < 8; ++ch) {
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int ih = ih0 + a, col = col0 + jj;
+      v[e] = (img && k < op.stem_K && ih >= 0 && ih < op.stem_h && col >= 0 && col < wc) ? __ldg(img + (size_t)ih * wc + col)
+                                                                                        : 0.f;
+      ++k;
+      if (++jj == run) { jj = 0; ++a; }
+    }
+    const uint32_t off = (uint32_t)r * 128u + ((uint32_t)(ch ^ (r & 7)) << 4);
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (NPLANES == 2) split_bf16x2(v[2 * q], v[2 * q + 1], h[q], l[q]);
+      else h[q] = pack_bf16x2(v[2 * q], v[2 * q + 1]);
+    }
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + off), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3])
+                 : "memory");
+    if (NPLANES == 2)
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + Smem<NPLANES, 64>::A_PLANE + off), "r"(l[0]),
+                   "r"(l[1]), "r"(l[2]), "r"(l[3])
+                   : "memory");
+  }
+}
+
+// ---------------------------------------------------------------------------------------------- the kernel body
+// MODE 0: one (tile, split) per CTA: tile = (blockIdx.x, blockIdx.y), split = blockIdx.z (grid split-K or cluster split-K)
+// MODE 1: persistent grid: CTA b walks tiles b, b + gridDim.x, ... of one op
+// MODE 2: one cluster walks a run of ops; tiles are dealt round-robin to its CTAs, a cluster barrier separates ops
+template <int NPLANES, int BN, int MODE>
+__device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stages, int pdl) {
+  using L = Smem<NPLANES, BN>;
+  constexpr int R = BN / 2;   // accumulator registers per consumer thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  const int STAGES = p.stages;                      // ring depth chosen per launch (smem footprint <-> CTAs per SM)
-  // layout: [operand ring: STAGES x STAGE | residual tile (staged epilogue with residual only) | barriers | scale, shift]
-  const int res_off = STAGES * L::STAGE;
-  const int ctl_off = res_off + p.res_stage_bytes;
-  const uint32_t bar_base = smem_base + ctl_off;
+  const uint32_t ring = smem_u32(smem);
+  const bool red = MODE == 0 && ops[0].p.cluster;
+  const uint32_t bar_base = ring + L::ring(stages, red);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (2 * STAGES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + ctl_off + 8 * (2 * STAGES + 1));
-  const uint32_t res_full_bar = bar_base + 8u * (2 * STAGES + 2);
-  float* s_scale = reinterpret_cast<float*>(smem + ctl_off + 256);
-  float* s_shift = s_scale + BN;
+  auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
   __shared__ int s_is_last;
-  __shared__ long long s_tl[4];   // timeline phases: setup done, first operands landed, accumulator ready, epilogue done
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  long long* trace = p.trace ? p.trace + 8 * ((size_t)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
-  if (trace && threadIdx.x == 0) { trace[0] = clock64(); trace[7] = (long long)gtimer(); }
-  long long tl_t0 = 0;
-  if (p.timeline && threadIdx.x == 0) tl_t0 = (long long)gtimer();
-
-  // ---- tile coordinates
-  const int tile_id = blockIdx.x;
-  int n0 = 0, h0 = 0, w0 = 0;
-  if (p.flat) {
-    w0 = tile_id * BM;
-  } else {
-    int tw = tile_id % p.tiles_w;
-    int t2 = tile_id / p.tiles_w;
-    int th = t2 % p.tiles_h;
-    int tn = t2 / p.tiles_h;
-    n0 = tn * p.tile_n;
-    h0 = th * p.tile_h;
-    w0 = tw * p.tile_w;
-  }
-  const int c_base = blockIdx.y * BN;
-  // split-K range
-  const int split = blockIdx.z;
-  const int kb_begin = (split * p.k_blocks) / p.splits;          // balanced ranges; host guarantees k_blocks >= splits
-  const int kb_end = ((split + 1) * p.k_blocks) / p.splits;
-  const int num_kb = kb_end - kb_begin;
-
-  // ---- one-time setup
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmx0);
-    prefetch_tmap(&tmw0);
-    if (NPLANES == 2) {
-      prefetch_tmap(&tmx1);
-      prefetch_tmap(&tmw1);
-    }
-    for (int s = 0; s < STAGES; ++s) {
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), CONS_THREADS / 32);   // one arrival per consumer warp
     }
-    mbar_init(tmem_full_bar, 1);
-    mbar_init(res_full_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    constexpr uint32_t ncols = (NPLANES == 2 ? 2 : 1) * (BN < 32 ? 32 : BN);
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // per-channel scale / shift of this CTA's BN columns -> shared memory.  Default: before the setup barrier (every warp
-  // waits for the global loads).  DEFER_UMMA_FAST bit 0: the loads are ISSUED before the barrier but CONSUMED after it,
-  // by the epilogue warps only, so the TMA producer starts its first operand fetch ~0.5 us earlier.
-  float pre_sc = 1.f, pre_sf = 0.f;
-  const int pre_i = threadIdx.x - 64;
-  if (warp >= 2) {
-    if (p.fast & 1) {
-      if (pre_i < BN) {          // BN <= 128 = 32 * EW threads at least: one element per thread suffices
-        const int c = c_base + pre_i;
-        if (p.scale && c < p.cout) pre_sc = __ldg(p.scale + c);
-        if (p.shift && c < p.cout) pre_sf = __ldg(p.shift + c);
-      }
-    } else {
-      for (int i = threadIdx.x - 64; i < BN; i += 32 * EW) {
-        int c = c_base + i;
-        s_scale[i] = (p.scale && c < p.cout) ? p.scale[c] : 1.f;
-        s_shift[i] = (p.shift && c < p.cout) ? p.shift[c] : 0.f;
-      }
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp >= 2 && (p.fast & 1)) {
-    if (pre_i < BN) {
-      s_scale[pre_i] = pre_sc;
-      s_shift[pre_i] = pre_sf;
-    }
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");   // epilogue warps only
-  }
-  if (p.pdl) {
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation, scale/shift staging,
-    // descriptor prefetch) overlapped the tail of the previous kernel of this lane; its outputs are visible
-    // only after this wait.  Our own dependents may start their prologue right away.
+  if (pdl) {
+    // programmatic dependent launch: the set-up above overlapped the previous kernel of this lane; its outputs are
+    // visible only after this wait.  Our own dependents may start their prologue right away.
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   }
-  if (trace && threadIdx.x == 0) trace[1] = clock64();   // setup done
-  if (p.timeline && threadIdx.x == 0) s_tl[0] = (long long)gtimer();
 
-  if (warp == 0) {
-    // =================================================================== TMA producer
-    if (lane == 0) {
-      constexpr uint32_t stage_bytes = NPLANES * (L::A_PLANE + L::B_PLANE);
-      // bytes TMA actually delivers: the full boxes (OOB elements are zero-filled and still counted)
-      const uint32_t a_rows = p.flat ? BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
-      const uint32_t tx_bytes = NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE);
-      (void)stage_bytes;
-      if (p.tma_epi && p.res) {
-        // staged epilogue: the residual tile (64-channel boxes, one per plane and 64-column half) does not depend on
-        // the MMAs - fetch it now, it lands while the K loop runs
-        prefetch_tmap(&tmr0);
-        constexpr int HALVES = BN / 64;
-        mbar_expect_tx(res_full_bar, (uint32_t)(NPLANES * HALVES) * a_rows_out(p) * 128u);
-#pragma unroll
-        for (int h = 0; h < HALVES; ++h) {
-          const uint32_t dst = smem_base + res_off + h * (BM * 128);
-          tma_load_4d(dst, &tmr0, res_full_bar, c_base + 64 * h, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-          if (NPLANES == 2)
-            tma_load_4d(dst + HALVES * (BM * 128), &tmr1, res_full_bar, c_base + 64 * h, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-        }
-      }
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1, p.error_flag, 1);
-        const int tap = kb / p.cblocks;
-        const int cb = kb - tap * p.cblocks;
-        const int khi = tap / p.kw;
-        const int kwi = tap - khi * p.kw;
-        const uint32_t a_dst = smem_base + stage * L::STAGE;
-        const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
-        mbar_expect_tx(full_bar(stage), tx_bytes);
-        int cw, ch, cn;
-        if (p.flat) {
-          cw = w0; ch = 0; cn = 0;
-        } else {
-          cw = w0 * p.sw + kwi - p.pad_l;
-          ch = h0 * p.sh + khi - p.pad_t;
-          cn = n0;
-        }
-        tma_load_4d(a_dst, &tmx0, full_bar(stage), cb * BK, cw, ch, cn);
-        tma_load_3d(b_dst, &tmw0, full_bar(stage), cb * BK, c_base, tap);
-        if (NPLANES == 2) {
-          tma_load_4d(a_dst + L::A_PLANE, &tmx1, full_bar(stage), cb * BK, cw, ch, cn);
-          tma_load_3d(b_dst + L::B_PLANE, &tmw1, full_bar(stage), cb * BK, c_base, tap);
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // =================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc<BN>();
-      constexpr uint32_t idesc_wide = make_idesc<(NPLANES == 2 ? 2 * BN : BN)>();
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t accum = 0;
-      for (int i = 0; i < num_kb; ++i) {
-        mbar_wait(full_bar(stage), phase, p.error_flag, 2);
-        if (trace && i == 0) trace[2] = clock64();           // first operands landed
-        if (p.timeline && i == 0) s_tl[1] = (long long)gtimer();
-        tc_fence_after();
-        const uint32_t a_addr = smem_base + stage * L::STAGE;
-        const uint32_t b_addr = a_addr + NPLANES * L::A_PLANE;
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          const uint64_t a_hi = make_sw128_desc(a_addr + k * (UMMA_K * 2));
-          const uint64_t b_hi = make_sw128_desc(b_addr + k * (UMMA_K * 2));   // NPLANES == 2: the 2*BN rows [b_hi | b_lo]
-          if (NPLANES == 2) {
-            // two instructions per K step instead of three (tcgen05.mma costs ~100 cycles whatever N is): the weight
-            // planes are adjacent in shared memory, so a_hi x [b_hi | b_lo] fills columns [0,BN) and [BN,2BN) at once
-            const uint64_t a_lo = make_sw128_desc(a_addr + L::A_PLANE + k * (UMMA_K * 2));
-            umma_bf16(tmem_base, a_hi, b_hi, idesc_wide, accum);
-            umma_bf16(tmem_base, a_lo, b_hi, idesc, 1);
-          } else {
-            umma_bf16(tmem_base, a_hi, b_hi, idesc, accum);
-          }
-          accum = 1;
-        }
-        umma_commit(empty_bar(stage));     // smem slot reusable once these MMAs have read it
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(tmem_full_bar);          // accumulator complete
-      if (trace) trace[3] = clock64();                     // all MMAs issued
-    }
-  } else {
-    // =================================================================== epilogue (warps 2..5)
-    const int quarter = warp & 3;                // TMEM lane quarter this warp may access
-    constexpr int CH_PER_WARP = (BN / 32) * 4 / EW;               // 32-column chunks this warp handles
-    const int c_begin = ((warp - 2) >> 2) * CH_PER_WARP * 32;     // EW == 4: 0
-    const int c_end = c_begin + CH_PER_WARP * 32;
-    auto epi_sync = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory"); };
-    const int r = quarter * 32 + lane;           // accumulator row == tile-local pixel
-    bool valid;
-    size_t pix;
-    row_to_pixel(p, r, n0, h0, w0, valid, pix);
-    if (p.cluster) {
-      // ---- cluster split-K, step 1: park this CTA's raw partial tile in its own shared memory.  The operand ring
-      // is free once tmem_full fires (all MMAs, hence all their smem reads, have completed).  Row stride BN + 4
-      // floats keeps the 16-B stores of a quarter-warp on distinct banks.
-      mbar_wait(tmem_full_bar, 0, p.error_flag, 3);
-      if (trace && threadIdx.x == 64) trace[4] = clock64();
-      if (p.timeline && threadIdx.x == 64) s_tl[2] = (long long)gtimer();
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + ((uint32_t)(quarter * 32) << 16);
-      const uint32_t red_row = smem_base + (uint32_t)r * (uint32_t)((BN + 4) * 4);
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32_acc<NPLANES, BN>(taddr_row + c0, v);   // warp-collective
-        if (valid) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) sts4(red_row + (uint32_t)(c0 + j) * 4u, v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-      }
-    } else if (p.tma_epi) {
-      // ---- staged epilogue.  Per-thread 16-B global accesses cost one LSU wavefront each (measured: ~8000 wavefronts
-      // per 128x128 tile = the whole epilogue).  Instead: finished values go into a SWIZZLE_128B staging tile (it
-      // aliases the operand ring, which is drained once tmem_full fires) and leave by ONE TMA store per plane and
-      // 64-column half; the residual tile was fetched by TMA during the K loop and is read with conflict-free LDS.
-      constexpr int HALVES = BN / 64;
-      constexpr int REGION = BM * 128;             // one (plane, half) tile: 128 rows x 128 B
-      const int sw = r & 7;
-      const uint32_t stg_row = smem_base + r * 128;              // shared-space addresses: explicit LDS / STS, no generic path
-      const uint32_t res_row = smem_base + res_off + r * 128;
-      const bool has_res = p.res != nullptr;
-      const bool relu = p.flags & DEFER_FLAG_RELU;
-      if (has_res) mbar_wait(res_full_bar, 0, p.error_flag, 4);
-      mbar_wait(tmem_full_bar, 0, p.error_flag, 3);
-      if (trace && threadIdx.x == 64) trace[4] = clock64();
-      if (p.timeline && threadIdx.x == 64) s_tl[2] = (long long)gtimer();
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32_acc<NPLANES, BN>(taddr_row + c0, v);   // warp-collective
-        if (!valid) continue;
-        const int half = c0 >> 6;
-        const int chb = (c0 & 63) >> 3;            // first 16-B chunk of this 32-column group inside its 128-B row
-        float acc[32];
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 sc = *reinterpret_cast<const float4*>(s_scale + c0 + j);
-          const float4 sf = *reinterpret_cast<const float4*>(s_shift + c0 + j);
-          acc[j] = fmaf(__uint_as_float(v[j]), sc.x, sf.x);
-          acc[j + 1] = fmaf(__uint_as_float(v[j + 1]), sc.y, sf.y);
-          acc[j + 2] = fmaf(__uint_as_float(v[j + 2]), sc.z, sf.z);
-          acc[j + 3] = fmaf(__uint_as_float(v[j + 3]), sc.w, sf.w);
-        }
-        if (has_res) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int ch = (chb + q) ^ sw;
-            const uint4 rh4 = lds4(res_row + half * REGION + ch * 16);
-            const uint32_t* hw = reinterpret_cast<const uint32_t*>(&rh4);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              acc[q * 8 + 2 * e] += __uint_as_float(hw[e] << 16);
-              acc[q * 8 + 2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u);
-            }
-            if (NPLANES == 2) {
-              const uint4 rl4 = lds4(res_row + (HALVES + half) * REGION + ch * 16);
-              const uint32_t* lw = reinterpret_cast<const uint32_t*>(&rl4);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                acc[q * 8 + 2 * e] += __uint_as_float(lw[e] << 16);
-                acc[q * 8 + 2 * e + 1] += __uint_as_float(lw[e] & 0xffff0000u);
-              }
-            }
-          }
-        }
-        if (relu) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = fmaxf(acc[j], 0.f);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 h, l;
-          uint32_t* hp = reinterpret_cast<uint32_t*>(&h);
-          uint32_t* lp = reinterpret_cast<uint32_t*>(&l);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            if (NPLANES == 2) {
-              split_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1], hp[e], lp[e]);
-            } else {
-              hp[e] = pack_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1]);
-            }
-          }
-          const int ch = (chb + q) ^ sw;
-          sts4(stg_row + half * REGION + ch * 16, h.x, h.y, h.z, h.w);
-          if (NPLANES == 2) sts4(stg_row + (HALVES + half) * REGION + ch * 16, l.x, l.y, l.z, l.w);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // staging writes -> visible to the TMA engine
-      epi_sync();
-      if (threadIdx.x == 64) {
-#pragma unroll
-        for (int h = 0; h < HALVES; ++h) {
-          tma_store_4d(&tmy0, smem_base + h * REGION, c_base + 64 * h, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-          if (NPLANES == 2)
-            tma_store_4d(&tmy1, smem_base + (HALVES + h) * REGION, c_base + 64 * h, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-        }
-        bulk_commit();
-        // default: wait until the tile is in global memory.  DEFER_UMMA_FAST bit 1: wait only until the TMA engine has
-        // read the staging tile (what must outlive the CTA); the writes complete before the grid does.
-        if (p.fast & 2) bulk_wait_read0();
-        else bulk_wait_all();
-      }
-    } else {
-    // the residual does not depend on the MMAs: fetch chunk 0 while the main loop is still running
-    // (only on the direct path; with split-K the finishing CTA is not known yet)
-    const __nv_bfloat16* rbase =
-        (p.res && valid) ? reinterpret_cast<const __nv_bfloat16*>(p.res) + pix * p.cout + c_base : nullptr;
-    uint4 rh[4], rl[4];
-    auto load_res = [&](int c0) {           // residual of one 32-channel chunk: 64 B per plane
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        rh[q] = *reinterpret_cast<const uint4*>(rbase + c0 + q * 8);
-        if (NPLANES == 2) rl[q] = *reinterpret_cast<const uint4*>(rbase + p.plane_out + c0 + q * 8);
-      }
-    };
-    const bool res_prefetched = rbase != nullptr && p.splits == 1;
-    if (res_prefetched) load_res(c_begin);
-    mbar_wait(tmem_full_bar, 0, p.error_flag, 3);
-    if (trace && threadIdx.x == 64) trace[4] = clock64();   // accumulator visible to the epilogue
-    if (p.timeline && threadIdx.x == 64) s_tl[2] = (long long)gtimer();
-    tc_fence_after();
-    const uint32_t taddr_row = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    const bool relu = p.flags & DEFER_FLAG_RELU;
-
-    bool do_final = true;
-    if (p.splits > 1) {
-      // ---- split-K: publish the raw partial tile, the last CTA of this (tile, n-block) reduces
-      const size_t tile_lin = (size_t)blockIdx.y * gridDim.x + blockIdx.x;
-      float* mine = p.partial + ((tile_lin * p.splits + split) * BM + r) * BN;
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32_acc<NPLANES, BN>(taddr_row + c0, v);
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          __stcg(reinterpret_cast<float4*>(mine + c0 + j),
-                 make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                             __uint_as_float(v[j + 3])));
-      }
-      __threadfence();
-      epi_sync();
-      if (threadIdx.x == 64) {
-        unsigned prev = atomicAdd(p.counters + tile_lin, 1u);
-        int last = (prev == (unsigned)(p.splits - 1));
-        if (last) p.counters[tile_lin] = 0;   // re-arm for the next launch
-        s_is_last = last;
-      }
-      epi_sync();
-      do_final = s_is_last != 0;
-      if (do_final) __threadfence();
-    }
-
-    if (do_final) {
-      const size_t tile_lin = (size_t)blockIdx.y * gridDim.x + blockIdx.x;
-#pragma unroll 1
-      for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-        float acc[32];
-        if (p.splits > 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-          if (valid) {
-            for (int s = 0; s < p.splits; ++s) {
-              const float* src = p.partial + ((tile_lin * p.splits + s) * BM + r) * BN + c0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 t = __ldcg(reinterpret_cast<const float4*>(src + j));
-                acc[j] += t.x; acc[j + 1] += t.y; acc[j + 2] += t.z; acc[j + 3] += t.w;
-              }
-            }
-          }
-        } else {
-          uint32_t v[32];
-          tmem_ld32_acc<NPLANES, BN>(taddr_row + c0, v);   // warp-collective: every lane takes part, stores are masked below
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = __uint_as_float(v[j]);
-        }
-        if (!valid) continue;
-        const size_t o = pix * p.cout + c_base + c0;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = fmaf(acc[j], s_scale[c0 + j], s_shift[c0 + j]);
-        if (rbase) {
-          if (c0 == c_begin && !res_prefetched) load_res(c_begin);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&rh[q]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              acc[q * 8 + 2 * e] += __low2float(hh[e]);
-              acc[q * 8 + 2 * e + 1] += __high2float(hh[e]);
-            }
-            if (NPLANES == 2) {
-              const __nv_bfloat162* ll = reinterpret_cast<const __nv_bfloat162*>(&rl[q]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                acc[q * 8 + 2 * e] += __low2float(ll[e]);
-                acc[q * 8 + 2 * e + 1] += __high2float(ll[e]);
-              }
-            }
-          }
-          if (c0 + 32 < c_end) load_res(c0 + 32);   // next chunk's residual is in flight during this chunk's stores
-        }
-        if (relu) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = fmaxf(acc[j], 0.f);
-        }
-        __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(p.y) + o;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 h, l;
-          uint32_t* hp = reinterpret_cast<uint32_t*>(&h);
-          uint32_t* lp = reinterpret_cast<uint32_t*>(&l);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            if (NPLANES == 2) {
-              split_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1], hp[e], lp[e]);
-            } else {
-              hp[e] = pack_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1]);
-            }
-          }
-          *reinterpret_cast<uint4*>(yp + q * 8) = h;
-          if (NPLANES == 2) *reinterpret_cast<uint4*>(yp + p.plane_out + q * 8) = l;
-        }
-      }
-    }
-    }   // !p.cluster
-  }
-
-  if (p.cluster) {
-    // ---- cluster split-K, step 2: the S CTAs of the cluster hold the S partial tiles of ONE output tile.  After a
-    // cluster barrier CTA j owns the tile rows {j, j + S, j + 2S, ...}: it sums the S partials of those rows in
-    // rank order (deterministic) straight out of its peers' shared memory (DSMEM), applies bias/BN, residual and
-    // ReLU and stores them - the K loop AND the epilogue are spread over S SMs, no global workspace.
-    __syncwarp();
-    cluster_sync_all();
-    if (warp >= 2) {
-      constexpr int FMT = NPLANES == 2 ? FMT_BF16X2 : FMT_BF16;
-      constexpr int NT = 32 * EW;                  // epilogue threads
-      constexpr int G = BN / 4;                    // float4 column groups per row
-      const int S = p.splits;                      // 2, 4 or 8
-      const int my_rank = (int)cluster_ctarank();
-      const int te = threadIdx.x - 64;
-      const int tpr = (NT * S) / BM;               // threads per row
-      const int q = te % tpr;
-      const int r = (te / tpr) * S + my_rank;
-      bool valid;
-      size_t pix;
-      row_to_pixel(p, r, n0, h0, w0, valid, pix);
-      if (valid) {
-        const bool relu = p.flags & DEFER_FLAG_RELU;
-        const uint32_t row_addr = smem_base + (uint32_t)r * (uint32_t)((BN + 4) * 4);
-        const size_t o = pix * p.cout + c_base;
-        auto reduce_groups = [&](int g, auto ngc) {
-          constexpr int NG = decltype(ngc)::value;
-          float4 v[NG][8];
-          float4 rs[NG];
-#pragma unroll
-          for (int u = 0; u < NG; ++u) {
-            const int col = (g + u * tpr) * 4;
-            if (p.res) rs[u] = act_load4<FMT>(p.res, p.plane_out, o + col);
-#pragma unroll
-            for (int s2 = 0; s2 < 8; ++s2)
-              if (s2 < S) v[u][s2] = dsmem_ld4(dsmem_map(row_addr + (uint32_t)col * 4u, (uint32_t)s2));
-          }
-#pragma unroll
-          for (int u = 0; u < NG; ++u) {
-            const int col = (g + u * tpr) * 4;
-            float4 a = v[u][0];
-#pragma unroll
-            for (int s2 = 1; s2 < 8; ++s2)
-              if (s2 < S) { a.x += v[u][s2].x; a.y += v[u][s2].y; a.z += v[u][s2].z; a.w += v[u][s2].w; }
-            const float4 sc = *reinterpret_cast<const float4*>(s_scale + col);
-            const float4 sf = *reinterpret_cast<const float4*>(s_shift + col);
-            a.x = fmaf(a.x, sc.x, sf.x); a.y = fmaf(a.y, sc.y, sf.y); a.z = fmaf(a.z, sc.z, sf.z); a.w = fmaf(a.w, sc.w, sf.w);
-            if (p.res) { a.x += rs[u].x; a.y += rs[u].y; a.z += rs[u].z; a.w += rs[u].w; }
-            if (relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
-            act_store4<FMT>(p.y, p.plane_out, o + col, a);
-          }
-        };
-        int g = q;
-        for (; g + tpr < G; g += 2 * tpr) reduce_groups(g, std::integral_constant<int, 2>());
-        if (g < G) reduce_groups(g, std::integral_constant<int, 1>());
-      }
-    }
-    __syncwarp();
-    cluster_sync_all();   // no CTA may leave (and free its shared memory) while a peer still reads it
-  }
-
-  // ---- teardown
-  if (trace && threadIdx.x == 64) trace[5] = clock64();     // epilogue stores issued
-  if (p.timeline && threadIdx.x == 64) s_tl[3] = (long long)gtimer();
-  tc_fence_before();
-  __syncthreads();
-  if (trace && threadIdx.x == 0) trace[6] = clock64();
-  if (p.timeline && threadIdx.x == 0) {
-    unsigned long long slot = atomicAdd(reinterpret_cast<unsigned long long*>(p.timeline), 1ull);
-    if (slot < (unsigned long long)p.timeline_cap) {
-      unsigned smid;
-      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-      long long* e = p.timeline + 8 + slot * 8;
-      e[0] = tl_t0;
-      e[1] = (long long)gtimer();
-      e[2] = (long long)smid;
-      e[3] = (long long)p.timeline_tag;
-      e[4] = s_tl[0];
-      e[5] = s_tl[1];
-      e[6] = s_tl[2];
-      e[7] = s_tl[3];
-    }
-  }
-  if (warp == 1) {
-    tc_fence_after();
-    constexpr uint32_t ncols = (NPLANES == 2 ? 2 : 1) * (BN < 32 ? 32 : BN);
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
-  }
-}
-
-// ==============================================================================================
-// Stage megakernel: a RUN of consecutive convolutions executed by ONE launch.
-//
-// At batch 1 every ResNet conv is a handful of 128-row tiles and a kernel launch (+ the dependency
-// latency between dependent launches) costs more than the tile itself; 52 launches per inference also
-// hit the device-wide launch rate when several microbatches are in flight.  Here one thread-block
-// CLUSTER (hardware co-scheduled, <= 16 CTAs) walks the whole op list: the tiles of an op are dealt
-// round-robin to the CTAs of the cluster, a hardware cluster barrier (barrier.cluster, release/acquire)
-// separates dependent ops, and barriers / TMEM / descriptors are set up once.  The warp roles of the
-// per-op kernel are kept and run continuously across tiles and ops:
-//   warp 0 TMA producer | warp 1 MMA issuer | warps 2-5 epilogue, with TWO TMEM accumulators so the
-//   epilogue of tile i overlaps the main loop of tile i+1.
-// Lanes (microbatches in flight) run one cluster each, concurrently.
-// ==============================================================================================
-struct alignas(128) MegaOp {
-  CUtensorMap tmx[2];
-  CUtensorMap tmw[2];
-  CUtensorMap tmy[2];       // output planes: 128-row x 64-channel boxes (TMA store, OOB rows clipped)
-  CUtensorMap tmr[2];       // residual planes, same geometry (TMA load into the staging tile)
-  KParams p;
-  int m_tiles, n_tiles;     // tiles of this op: m fastest
-  int direct;               // 1: per-thread st.global / ld.global epilogue (output in a peer GPU's slot)
-  int pad_[1];
-  // fused stem (conv_stem_kernel): the fp32 NHWC image the patch rows are built from, and the real conv geometry
-  const float* stem_x;
-  int stem_h, stem_w, stem_cin, stem_kh, stem_kw, stem_sh, stem_sw, stem_pad_t, stem_pad_l, stem_K;
-};
-
-constexpr int MEGA_BN = 64;
-constexpr int MEGA_ACC_BUFS = 2;
-constexpr int MEGA_EPI_WARPS = 8;
-constexpr int MEGA_THREADS = 64 + 32 * MEGA_EPI_WARPS;   // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-__device__ __forceinline__ void mega_epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-
-// smem of the mega kernel: [stages x STAGE ring | 2 residual tiles | 2 output tiles | barriers]
-// (a tile = NPLANES x 128 rows x 128 B, SWIZZLE_128B rows)
-template <int NPLANES>
-struct MegaSmem {
-  using L = SmemLayout<NPLANES, MEGA_BN>;
-  static constexpr int STAGING = NPLANES * BM * 128;           // one output / residual tile, all planes
-  __host__ __device__ static constexpr int rbuf_off(int stages) { return stages * L::STAGE; }
-  __host__ __device__ static constexpr int obuf_off(int stages) { return stages * L::STAGE + 2 * STAGING; }
-  __host__ __device__ static constexpr int bar_off(int stages) { return stages * L::STAGE + 4 * STAGING; }
-  __host__ __device__ static constexpr int total(int stages) { return bar_off(stages) + 256 + 1024; }
-  __host__ __device__ static constexpr int max_stages() {
-    int s = (227 * 1024 - 4 * STAGING - 256 - 1024) / L::STAGE;
-    return s > 6 ? 6 : s;
-  }
-};
-
-template <int NPLANES>
-__global__ void __launch_bounds__(MEGA_THREADS, 1)
-conv_mega_kernel(const MegaOp* __restrict__ ops, int n_ops, int stages, int use_cluster, int* error_flag) {
-  constexpr int BN = MEGA_BN;
-  using L = SmemLayout<NPLANES, BN>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  using MS = MegaSmem<NPLANES>;
-  const int STAGES = stages;
-  const uint32_t bar_base = smem_base + MS::bar_off(STAGES);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 2 + b); };
-  auto rfull_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 4 + b); };   // residual tile landed
-  auto rfree_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 6 + b); };   // residual tile consumed
-  auto ofree_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 8 + b); };   // output tile read by its TMA store
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + MS::bar_off(STAGES) + 8 * (2 * STAGES + 10));
-  const uint32_t rbuf_base = smem_base + MS::rbuf_off(STAGES);
-  const uint32_t obuf_base = smem_base + MS::obuf_off(STAGES);
-  uint8_t* rbuf_ptr = smem + MS::rbuf_off(STAGES);
-  uint8_t* obuf_ptr = smem + MS::obuf_off(STAGES);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  // cluster mode: one cluster walks a chain of dependent ops.  grid mode (n_ops == 1): a plain persistent
-  // grid deals the tiles of ONE op round-robin - no inter-CTA dependency, no cluster barrier.
-  const int rank = use_cluster ? (int)cluster_ctarank() : (int)blockIdx.x;
-  const int csize = use_cluster ? (int)cluster_nctarank() : (int)gridDim.x;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < MEGA_ACC_BUFS; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), MEGA_EPI_WARPS);      // one arrival per epilogue warp
-      mbar_init(rfull_bar(b), 1);
-      mbar_init(rfree_bar(b), MEGA_EPI_WARPS);
-      mbar_init(ofree_bar(b), 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    constexpr uint32_t ncols = MEGA_ACC_BUFS * BN;   // 128
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  // optional phase trace (debug): CTA 0 stamps globaltimer at role milestones of its first tiles
-  long long* trace = (n_ops > 0 && ops[0].p.trace && rank == 0) ? ops[0].p.trace : nullptr;
-  auto stamp = [&](uint32_t tile_seq, int slot) {
-    if (trace && tile_seq < 24) trace[tile_seq * 8 + slot] = (long long)gtimer();
-  };
-  // running pipeline state of each role (every role walks the same (op, tile, k-block) sequence)
-  int stage = 0;
-  uint32_t phase = 0;
-  uint32_t it = 0;       // tiles processed by this CTA so far -> accumulator / staging buffer and phase
-  uint32_t rit = 0;      // residual tiles so far -> residual buffer / phase (producer and epilogue warps)
-
-  for (int oi = 0; oi < n_ops; ++oi) {
-    const MegaOp& op = ops[oi];
+  uint32_t it = 0;   // k-blocks through the ring so far (same sequence in every role)
+  for (int o = 0; o < n_ops; ++o) {
+    const MegaOp& op = ops[o];
     const KParams& p = op.p;
-    const int n_tiles = op.m_tiles * op.n_tiles;
-    if (oi > 0) {
-      // dependent op: everything the cluster stored must be visible (also to the TMA / async proxy)
-      asm volatile("fence.proxy.async;" ::: "memory");
-      cluster_sync_all();
-      asm volatile("fence.proxy.async;" ::: "memory");
+    const int total = op.m_tiles * op.n_tiles;
+    int t_first, t_step;
+    if (MODE == 0) {
+      t_first = blockIdx.y * op.m_tiles + blockIdx.x;
+      t_step = total;
+    } else if (MODE == 1) {
+      t_first = blockIdx.x;
+      t_step = gridDim.x;
+    } else {
+      t_first = (int)cluster_ctarank();
+      t_step = (int)cluster_nctarank();
     }
-    if (warp == 0) {
-      // =================================================================== TMA producer
-      if (lane == 0) {
-        prefetch_tmap(&op.tmx[0]);
-        prefetch_tmap(&op.tmw[0]);
-        const uint32_t a_rows = p.flat ? BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
-        const uint32_t tx_bytes = NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE);
-        const bool res_tma = p.res != nullptr && !op.direct;
-        for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-          const int mt = tile % op.m_tiles, nt = tile / op.m_tiles;
-          int n0 = 0, h0 = 0, w0 = 0;
-          if (p.flat) {
-            w0 = mt * BM;
-          } else {
-            int tw = mt % p.tiles_w;
-            int t2 = mt / p.tiles_w;
-            n0 = (t2 / p.tiles_h) * p.tile_n;
-            h0 = (t2 % p.tiles_h) * p.tile_h;
-            w0 = tw * p.tile_w;
-          }
-          const int c_base = nt * BN;
-          stamp(it, 0);   // producer starts issuing this tile
-          if (res_tma) {
-            // residual tile -> rbuf[rb] (its own full/free barrier pair: prefetched as early as the epilogue allows)
-            const uint32_t rb = rit & 1, ur = rit >> 1;
-            ++rit;
-            mbar_wait(rfree_bar(rb), (ur & 1) ^ 1, error_flag, 15);
-            mbar_expect_tx(rfull_bar(rb), NPLANES * a_rows * 128u);
-            const uint32_t dst = rbuf_base + rb * MS::STAGING;
-            tma_load_4d(dst, &op.tmr[0], rfull_bar(rb), c_base, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-            if (NPLANES == 2)
-              tma_load_4d(dst + BM * 128, &op.tmr[1], rfull_bar(rb), c_base, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-          }
-          for (int kb = 0; kb < p.k_blocks; ++kb) {
-            mbar_wait(empty_bar(stage), phase ^ 1, error_flag, 11);
+    const int split = MODE == 0 ? (int)blockIdx.z : 0;
+    const int kb_begin = (split * p.k_blocks) / p.splits;   // balanced ranges; host guarantees k_blocks >= splits
+    const int kb_end = ((split + 1) * p.k_blocks) / p.splits;
+    const bool stem = op.stem_x != nullptr;
+
+    for (int t = t_first; t < total; t += t_step) {
+      const int m_tile = t % op.m_tiles;
+      const int c_base = (t / op.m_tiles) * BN;
+      int n0 = 0, h0 = 0, w0 = 0;
+      if (p.flat) {
+        w0 = m_tile * BM;
+      } else {
+        const int tw = m_tile % p.tiles_w;
+        const int t2 = m_tile / p.tiles_w;
+        n0 = (t2 / p.tiles_h) * p.tile_n;
+        h0 = (t2 % p.tiles_h) * p.tile_h;
+        w0 = tw * p.tile_w;
+      }
+
+      if (tid >= CONS_THREADS) {
+        // =================================================================== producer
+        const int ptid = tid - CONS_THREADS;
+        if (stem || ptid == 0) {
+          const uint32_t a_rows = p.flat ? (uint32_t)BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
+          uint32_t i2 = it;
+          for (int kb = kb_begin; kb < kb_end; ++kb, ++i2) {
+            const int stage = (int)(i2 % (uint32_t)stages);
+            const uint32_t phase = (i2 / (uint32_t)stages) & 1u;
+            mbar_wait(empty_bar(stage), phase ^ 1u, 1);
+            const uint32_t a_dst = ring + stage * L::STAGE;
+            const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
             const int tap = kb / p.cblocks;
             const int cb = kb - tap * p.cblocks;
-            const int khi = tap / p.kw;
-            const int kwi = tap - khi * p.kw;
-            const uint32_t a_dst = smem_base + stage * L::STAGE;
-            const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
-            mbar_expect_tx(full_bar(stage), tx_bytes);
-            int cw, ch, cn;
-            if (p.flat) {
-              cw = w0; ch = 0; cn = 0;
-            } else {
-              cw = w0 * p.sw + kwi - p.pad_l;
-              ch = h0 * p.sh + khi - p.pad_t;
-              cn = n0;
-            }
-            tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
-            tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
-            if (NPLANES == 2) {
-              tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
-              tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
-            }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-        }
-      }
-      __syncwarp();   // reconverge before the (warp-aligned) cluster barrier
-    } else if (warp == 1) {
-      // =================================================================== MMA issuer
-      if (lane == 0) {
-        constexpr uint32_t idesc = make_idesc<BN>();
-        for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-          const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-          mbar_wait(tempty_bar(buf), aphase ^ 1, error_flag, 12);   // epilogue drained this accumulator
-          stamp(it, 1);   // MMA: accumulator available
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + buf * BN;
-          uint32_t accum = 0;
-          for (int kb = 0; kb < p.k_blocks; ++kb) {
-            mbar_wait(full_bar(stage), phase, error_flag, 13);
-            tc_fence_after();
-            const uint32_t a_addr = smem_base + stage * L::STAGE;
-            const uint32_t b_addr = a_addr + NPLANES * L::A_PLANE;
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t a_hi = make_sw128_desc(a_addr + k * (UMMA_K * 2));
-              const uint64_t b_hi = make_sw128_desc(b_addr + k * (UMMA_K * 2));
-              if (NPLANES == 2) {
-                const uint64_t a_lo = make_sw128_desc(a_addr + L::A_PLANE + k * (UMMA_K * 2));
-                const uint64_t b_lo = make_sw128_desc(b_addr + L::B_PLANE + k * (UMMA_K * 2));
-                umma_bf16(tmem_d, a_lo, b_hi, idesc, accum);
-                accum = 1;
-                umma_bf16(tmem_d, a_hi, b_lo, idesc, accum);
+            if (stem) {
+              if (ptid == 0) {
+                mbar_expect_tx(full_bar(stage), NPLANES * (uint32_t)L::B_PLANE);
+                tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
+                if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
               }
-              umma_bf16(tmem_d, a_hi, b_hi, idesc, accum);
-              accum = 1;
+              stem_build<NPLANES>(op, a_dst, w0, kb, ptid);
+              asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
+              prod_bar_sync();
+              if (ptid == 0) mbar_arrive(full_bar(stage));
+            } else {
+              const int khi = tap / p.kw;
+              const int kwi = tap - khi * p.kw;
+              int cw = w0, ch = 0, cn = 0;
+              if (!p.flat) {
+                cw = w0 * p.sw + kwi - p.pad_l;
+                ch = h0 * p.sh + khi - p.pad_t;
+                cn = n0;
+              }
+              mbar_arrive_expect_tx(full_bar(stage), NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE));
+              tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
+              tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
+              if (NPLANES == 2) {
+                tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
+                tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
+              }
             }
-            umma_commit(empty_bar(stage));
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
-          umma_commit(tfull_bar(buf));
-          stamp(it, 2);   // MMA: all MMAs of the tile issued
+        }
+        it += (uint32_t)(kb_end - kb_begin);
+        continue;
+      }
+
+      // ===================================================================== consumers: main loop
+      const int wg = tid >> 7;
+      const int lane = tid & 31;
+      float acc[R];
+#pragma unroll
+      for (int i = 0; i < R; ++i) acc[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
+        const int stage = (int)(it % (uint32_t)stages);
+        mbar_wait(full_bar(stage), (it / (uint32_t)stages) & 1u, 2);
+        const uint32_t a_addr = ring + stage * L::STAGE + wg * (64 * 128);
+        const uint32_t b_addr = ring + stage * L::STAGE + NPLANES * L::A_PLANE;
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t a_hi = make_sw128_desc(a_addr + k * 32);
+          const uint64_t b_hi = make_sw128_desc(b_addr + k * 32);
+          wgmma_bf16<BN>(acc, a_hi, b_hi);
+          if (NPLANES == 2) {
+            wgmma_bf16<BN>(acc, make_sw128_desc(a_addr + L::A_PLANE + k * 32), b_hi);
+            wgmma_bf16<BN>(acc, a_hi, make_sw128_desc(b_addr + L::B_PLANE + k * 32));
+          }
+        }
+        wg_commit();
+        wg_wait<1>();   // the previous k-block's wgmmas are done: its stage may be refilled
+        acc_fence(acc);
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+        prev_stage = stage;
+      }
+      wg_wait<0>();
+      acc_fence(acc);
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+
+      // ===================================================================== consumers: epilogue
+      // wgmma m64nN accumulator layout: register i of thread (warp w, lane l) of warpgroup g holds row
+      // 64g + 16w + l/4 + 8*((i/2)&1), column 8*(i/4) + 2*(l%4) + (i&1)
+      const int row0 = wg * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);
+      const int col_l = 2 * (lane & 3);
+      bool valid0, valid1;
+      size_t pix0, pix1;
+      row_to_pixel(p, row0, n0, h0, w0, valid0, pix0);
+      row_to_pixel(p, row0 + 8, n0, h0, w0, valid1, pix1);
+
+      if (MODE == 0 && p.cluster) {
+        // ---- cluster split-K: the S CTAs of the cluster hold the S partial tiles of ONE output tile.  Each parks its
+        // partial in its own shared memory; after a cluster barrier CTA j reduces the column groups q = j, j + S, ...
+        // in rank order (deterministic) straight out of its peers' shared memory (DSMEM) and runs their epilogue.
+        cons_bar_sync();   // both warpgroups are done reading the ring
+        float4* red_buf = reinterpret_cast<float4*>(smem);
+#pragma unroll
+        for (int q = 0; q < R / 4; ++q)
+          red_buf[q * CONS_THREADS + tid] = make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]);
+        break;   // to the cluster reduction below (MODE 0 has exactly one tile)
+      }
+      if (MODE == 0 && p.splits > 1) {
+        // ---- grid split-K: publish the raw partial tile; the last CTA of this (tile, n-block) reduces them
+        const size_t tile_lin = (size_t)t;
+        float4* mine = reinterpret_cast<float4*>(p.partial) + (tile_lin * p.splits + split) * (R / 4) * CONS_THREADS;
+#pragma unroll
+        for (int q = 0; q < R / 4; ++q)
+          __stcg(mine + q * CONS_THREADS + tid, make_float4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
+        __threadfence();
+        cons_bar_sync();
+        if (tid == 0) {
+          const unsigned prev = atomicAdd(p.counters + tile_lin, 1u);
+          const int last = prev == (unsigned)(p.splits - 1);
+          if (last) p.counters[tile_lin] = 0;   // re-arm for the next launch
+          s_is_last = last;
+        }
+        cons_bar_sync();
+        if (!s_is_last) continue;
+        __threadfence();
+#pragma unroll
+        for (int i = 0; i < R; ++i) acc[i] = 0.f;
+        for (int s = 0; s < p.splits; ++s) {
+          const float4* src = reinterpret_cast<const float4*>(p.partial) + (tile_lin * p.splits + s) * (R / 4) * CONS_THREADS;
+#pragma unroll
+          for (int q = 0; q < R / 4; ++q) {
+            const float4 v = __ldcg(src + q * CONS_THREADS + tid);
+            acc[4 * q] += v.x; acc[4 * q + 1] += v.y; acc[4 * q + 2] += v.z; acc[4 * q + 3] += v.w;
+          }
         }
       }
-      __syncwarp();
-    } else {
-      // =================================================================== epilogue (warps 2..5)
-      // 8 epilogue warps: warp w reads TMEM lane quarter (w & 3) (hardware rule) and the 32-column half
-      // ((w - 2) >> 2) of the 64-column accumulator - two warps per scheduler hide each other's latencies
-      const int quarter = warp & 3;
-      const int r = quarter * 32 + lane;
-      const int chalf = (warp - 2) >> 2;
-      const bool relu = p.flags & DEFER_FLAG_RELU;
-      const bool direct = op.direct != 0;
-      const bool is_issuer = threadIdx.x == 64;     // elected thread: TMA stores + bulk-group bookkeeping
-      const float* scale_ptr = p.scale;             // hoisted: the op descriptor lives in global memory
-      const float* shift_ptr = p.shift;
-      float scv[32], sfv[32];                       // this warp's 32 channels of scale / shift
-      int cached_nt = -1;
-      for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-        const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-        const int mt = tile % op.m_tiles, nt = tile / op.m_tiles;
-        const int c_base = nt * BN;
+#pragma unroll
+      for (int q = 0; q < R / 4; ++q) {
+        const int c = c_base + 8 * q + col_l;
+        if (valid0) epi_pair<NPLANES>(p, pix0, c, acc[4 * q], acc[4 * q + 1]);
+        if (valid1) epi_pair<NPLANES>(p, pix1, c, acc[4 * q + 2], acc[4 * q + 3]);
+      }
+    }
+
+    if (MODE == 0 && p.cluster) {
+      cluster_sync_all();
+      if (tid < CONS_THREADS) {
+        const int lane = tid & 31;
+        const int row0 = (tid >> 7) * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);
+        const int m_tile = blockIdx.x;
         int n0 = 0, h0 = 0, w0 = 0;
-        bool valid;
-        size_t pix;
         if (p.flat) {
-          w0 = mt * BM;
-          int m = w0 + r;
-          valid = m < p.m_total;
-          pix = (size_t)m;
+          w0 = m_tile * BM;
         } else {
-          int tw0 = mt % p.tiles_w;
-          int t2 = mt / p.tiles_w;
+          const int t2 = m_tile / p.tiles_w;
           n0 = (t2 / p.tiles_h) * p.tile_n;
           h0 = (t2 % p.tiles_h) * p.tile_h;
-          w0 = tw0 * p.tile_w;
-          int tw = r % p.tile_w;
-          int t3 = r / p.tile_w;
-          int th = t3 % p.tile_h;
-          int tn = t3 / p.tile_h;
-          int nn = n0 + tn, oh = h0 + th, ow = w0 + tw;
-          valid = (tn < p.tile_n) && nn < p.n && oh < p.ho && ow < p.wo;
-          pix = ((size_t)nn * p.ho + oh) * p.wo + ow;
+          w0 = (m_tile % p.tiles_w) * p.tile_w;
         }
-        // staging tiles: SWIZZLE_128B rows of 128 B (64 channels), one per plane
-        const bool use_rbuf = (p.res != nullptr) && !direct;
-        const uint32_t rb = rit & 1, ur = rit >> 1;
-        if (use_rbuf) ++rit;
-        uint8_t* ostg = obuf_ptr + buf * MS::STAGING + r * 128;
-        const uint8_t* rstg = rbuf_ptr + rb * MS::STAGING + r * 128;
-        const int sw = r & 7;
-        const __nv_bfloat16* rbase =
-            (direct && p.res && valid) ? reinterpret_cast<const __nv_bfloat16*>(p.res) + pix * p.cout + c_base : nullptr;
-        uint4 rh[4], rl[4];
-        auto load_res = [&](int c0) {
-          if (direct) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              rh[q] = *reinterpret_cast<const uint4*>(rbase + c0 + q * 8);
-              if (NPLANES == 2) rl[q] = *reinterpret_cast<const uint4*>(rbase + p.plane_out + c0 + q * 8);
-            }
-          } else {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int ch = ((c0 >> 3) + q) ^ sw;
-              rh[q] = *reinterpret_cast<const uint4*>(rstg + ch * 16);
-              if (NPLANES == 2) rl[q] = *reinterpret_cast<const uint4*>(rstg + BM * 128 + ch * 16);
-            }
+        bool valid0, valid1;
+        size_t pix0, pix1;
+        row_to_pixel(p, row0, n0, h0, w0, valid0, pix0);
+        row_to_pixel(p, row0 + 8, n0, h0, w0, valid1, pix1);
+        const int S = p.splits;
+        const uint32_t mine = ring + (uint32_t)tid * 16u;
+        for (int q = (int)cluster_ctarank(); q < R / 4; q += S) {
+          const uint32_t addr = mine + (uint32_t)(q * CONS_THREADS) * 16u;
+          float4 a = dsmem_ld4(dsmem_map(addr, 0));
+          for (int s = 1; s < S; ++s) {
+            const float4 v = dsmem_ld4(dsmem_map(addr, (uint32_t)s));
+            a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
           }
-        };
-        const bool has_res = p.res != nullptr;
-        const int c0 = chalf * 32;
-        if (nt != cached_nt) {   // tiles run m-fastest: the channel block changes once per m_tiles tiles
-          cached_nt = nt;
-          const float4* sp = reinterpret_cast<const float4*>(scale_ptr + c_base + c0);
-          const float4* fp = reinterpret_cast<const float4*>(shift_ptr + c_base + c0);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 a4 = scale_ptr ? __ldg(sp + j) : make_float4(1.f, 1.f, 1.f, 1.f);
-            float4 b4 = shift_ptr ? __ldg(fp + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-            scv[4 * j] = a4.x; scv[4 * j + 1] = a4.y; scv[4 * j + 2] = a4.z; scv[4 * j + 3] = a4.w;
-            sfv[4 * j] = b4.x; sfv[4 * j + 1] = b4.y; sfv[4 * j + 2] = b4.z; sfv[4 * j + 3] = b4.w;
-          }
-        }
-        if (use_rbuf) mbar_wait(rfull_bar(rb), ur & 1, error_flag, 16);   // residual tile landed
-        if (has_res && (rbase || !direct)) load_res(c0);
-        if (use_rbuf) {                                                   // in registers: release the buffer
-          __syncwarp();
-          if (lane == 0) mbar_arrive(rfree_bar(rb));
-        }
-        if (is_issuer) stamp(it, 3);   // epilogue: residual in registers, waiting for the accumulator
-        mbar_wait(tfull_bar(buf), aphase, error_flag, 14);
-        if (is_issuer) stamp(it, 4);   // epilogue: accumulator ready
-        tc_fence_after();
-        const uint32_t taddr_row = tmem_base + buf * BN + ((uint32_t)(quarter * 32) << 16);
-        {
-          uint32_t v[32];
-          tmem_ld32(taddr_row + c0, v);
-          {
-            // this warp's part of the accumulator is in registers: hand the TMEM buffer back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(buf));
-          }
-          if (!(direct && !valid)) {
-          float acc[32];
-          const int c = c_base + c0;
-          // per-channel scale / shift of this warp's 32 columns: 16 independent 16-B loads (L1-resident,
-          // pointers hoisted out of the op descriptor), issued before the accumulator wait
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = fmaf(__uint_as_float(v[j]), scv[j], sfv[j]);
-          if (has_res && (rbase || !direct)) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&rh[q]);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                acc[q * 8 + 2 * e] += __low2float(hh[e]);
-                acc[q * 8 + 2 * e + 1] += __high2float(hh[e]);
-              }
-              if (NPLANES == 2) {
-                const __nv_bfloat162* ll = reinterpret_cast<const __nv_bfloat162*>(&rl[q]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  acc[q * 8 + 2 * e] += __low2float(ll[e]);
-                  acc[q * 8 + 2 * e + 1] += __high2float(ll[e]);
-                }
-              }
-            }
-          }
-          if (relu) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] = fmaxf(acc[j], 0.f);
-          }
-          __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(p.y) + pix * p.cout + c;
-          if (!direct) {
-            // obuf[buf] was last read by the TMA store of tile it-2 (issuer: wait_group.read 1 -> ofree)
-            const uint32_t u = it >> 1;
-            mbar_wait(ofree_bar(buf), buf == 0 ? ((u & 1) ^ 1) : (u & 1), error_flag, 17);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 h, l;
-            uint32_t* hp = reinterpret_cast<uint32_t*>(&h);
-            uint32_t* lp = reinterpret_cast<uint32_t*>(&l);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              if (NPLANES == 2) {
-                split_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1], hp[e], lp[e]);
-              } else {
-                hp[e] = pack_bf16x2(acc[q * 8 + 2 * e], acc[q * 8 + 2 * e + 1]);
-              }
-            }
-            if (direct) {
-              *reinterpret_cast<uint4*>(yp + q * 8) = h;
-              if (NPLANES == 2) *reinterpret_cast<uint4*>(yp + p.plane_out + q * 8) = l;
-            } else {
-              const int ch = ((c0 >> 3) + q) ^ sw;
-              *reinterpret_cast<uint4*>(ostg + ch * 16) = h;
-              if (NPLANES == 2) *reinterpret_cast<uint4*>(ostg + BM * 128 + ch * 16) = l;
-            }
-          }
-          }
-        }
-        if (!direct) {
-          // staging tile complete -> one TMA store per plane (full 128-B rows, rows outside the tensor clipped)
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          if (is_issuer) stamp(it, 5);   // epilogue: this thread's part of the tile is in staging
-          mega_epi_bar_sync();
-          if (is_issuer) stamp(it, 6);   // epilogue: all 8 warps done
-          if (is_issuer) {
-            const uint32_t src = obuf_base + buf * MS::STAGING;
-            tma_store_4d(&op.tmy[0], src, c_base, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-            if (NPLANES == 2) tma_store_4d(&op.tmy[1], src + BM * 128, c_base, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-            bulk_commit();
-          }
-        }
-        // one ofree arrival per tile (direct tiles too, so the parity bookkeeping stays uniform): the store of
-        // tile it-1 has finished reading obuf[buf ^ 1], which tile it+1 will fill
-        if (is_issuer) {
-          asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-          mbar_arrive(ofree_bar(buf ^ 1));
-          stamp(it, 7);   // epilogue: previous store has released its staging tile
-        }
-        __syncwarp();   // the issuer's warp reconverges before the next warp-collective tcgen05.ld
-      }
-      // all output of this op must be globally visible before the next (dependent) op / kernel end
-      if (is_issuer) bulk_wait_all();
-    }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    constexpr uint32_t ncols = MEGA_ACC_BUFS * BN;
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
-  }
-  // no CTA may exit while a peer could still be inside a cluster barrier
-  if (use_cluster) cluster_sync_all();
-}
-
-// ==============================================================================================
-// Streaming persistent convolution kernel (round 2): the executor of every conv with enough tiles.
-//
-// Measured on B200 (tools/microbench/fill_bench.cu, profiles/r02_fill_bench.txt): TMA delivers ~14 TB/s of
-// L2-resident tiles into shared memory chip-wide (~97 GB/s per SM) when ~190 KB are in flight per SM, but the round
-// trip under load is ~2 us - a CTA's fill rate is (operand bytes in flight) / 2 us.  The round-1 persistent kernel
-// kept 128 KB of its shared memory as epilogue staging and only 2 x 48 KB in flight: 48 GB/s per SM, 6-7 TB/s
-// chip-wide - the number every conv launch was stuck at.  This kernel gives the shared memory to the operand ring:
-//   * ring of S stages x (A 128 x 64 + B BN x 64, all planes); BN = 64 or 128 (one N = BN MMA per k-step);
-//   * epilogue staging is U small "units" (one 64-column chunk of a tile, all planes: 32 KB fp32-parity / 16 KB
-//     bf16).  A unit serves BOTH directions: the residual chunk is TMA-loaded INTO it, the epilogue warps read it,
-//     add and overwrite it in place, and one TMA store ships it out;
-//   * S and U are chosen per op at run time: K-heavy ops get S x STAGE ~ 190 KB and one unit, output-heavy ops
-//     (1 - 4 k-blocks per tile) get a short ring and 3 - 4 units so residual fetch, math and store of successive
-//     chunks overlap.
-//   * tcgen05.mma has a ~100-cycle floor per instruction on B200 whatever N is (measured with the phase trace: 12
-//     instructions per k-block take 1200 cycles for N = 64 and for N = 128 alike), so the fp32-parity path issues TWO
-//     instructions per K = 16 step instead of three: the hi and lo planes of the weights sit back to back in shared
-//     memory and act as ONE 2*BN-row B operand,  a_hi x [b_hi | b_lo] -> accumulator columns [0, BN) and [BN, 2BN),
-//     then a_lo x b_hi -> columns [0, BN); the epilogue adds the two column blocks (hi*lo is the small term).
-// Warp roles (352 threads): warp 0 operand producer (TMA), warp 1 MMA issuer (two TMEM accumulators of BN columns),
-// warp 2 chunk manager (residual loads, TMA stores, bulk-group bookkeeping), warps 3-10 epilogue math.
-// All roles walk the same (tile, chunk) sequence; every wait is bounded (mbar_wait traps after 2 s).
-// ==============================================================================================
-constexpr int STREAM_EPI_WARPS = 8;
-constexpr int STREAM_THREADS = 96 + 32 * STREAM_EPI_WARPS;   // 352
-constexpr int STREAM_CTL_BYTES = 512;
-constexpr int STREAM_MAX_UNITS = 6;
-
-template <int NPLANES, int BN>
-struct StreamSmem {
-  using L = SmemLayout<NPLANES, BN>;
-  static constexpr int UNIT = NPLANES * BM * 128;            // one 64-column chunk of an output tile, all planes
-  __host__ __device__ static constexpr int unit_off(int stages) { return stages * L::STAGE; }
-  __host__ __device__ static constexpr int ctl_off(int stages, int units) { return stages * L::STAGE + units * UNIT; }
-  __host__ __device__ static constexpr int total(int stages, int units) { return ctl_off(stages, units) + STREAM_CTL_BYTES + 1024; }
-};
-
-template <int NPLANES, int BN>
-__global__ void __launch_bounds__(STREAM_THREADS, 1)
-conv_stream_kernel(const MegaOp* __restrict__ opp, int stages, int units, int pdl, int* error_flag) {
-  using L = SmemLayout<NPLANES, BN>;
-  using SS = StreamSmem<NPLANES, BN>;
-  constexpr int CH = BN / 64;                      // 64-column chunks per tile
-  constexpr int ACC_COLS = NPLANES == 2 ? 2 * BN : BN;   // TMEM columns of one accumulator (fp32 parity: [hi-terms | a_hi x b_lo])
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  const int STAGES = stages, U = units;
-  const uint32_t bar_base = smem_base + SS::ctl_off(STAGES, U);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };                      // [0, 8)
-  auto empty_bar = [&](int s) { return bar_base + 8u * (8 + s); };               // [8, 16)
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (16 + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (18 + b); };
-  auto ready_bar = [&](int u) { return bar_base + 8u * (20 + u); };              // [20, 26) unit holds the residual / may be written
-  auto done_bar = [&](int u) { return bar_base + 8u * (26 + u); };               // [26, 32) unit holds the finished chunk
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SS::ctl_off(STAGES, U) + 8 * 32);
-  const uint32_t unit_base = smem_base + SS::unit_off(STAGES);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const MegaOp& op = *opp;
-  const KParams& p = op.p;
-  const int n_tiles = op.m_tiles * op.n_tiles;     // n_tiles counted in BN-wide column blocks (host: cout / BN)
-  const int rank = (int)blockIdx.x, csize = (int)gridDim.x;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), STREAM_EPI_WARPS);
-    }
-    for (int u = 0; u < U; ++u) {
-      mbar_init(ready_bar(u), 1);
-      mbar_init(done_bar(u), STREAM_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    constexpr uint32_t ncols = 2 * ACC_COLS;         // two accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (pdl) {
-    // Programmatic dependent launch: everything above (barrier init, TMEM allocation, reading the op descriptor) overlapped
-    // the tail of the previous kernel of this lane; its outputs are visible only after this wait.  Our own dependents may
-    // start their prologue as soon as SMs free up.
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
-
-  // optional phase trace (DEFER_UMMA_TRACE through defer_k_conv): CTA 0 stamps %globaltimer at role milestones of its
-  // first 8 tiles - 64 slots per tile: 0 producer starts the tile, 1 producer issued its last k-block, 2 MMA got the
-  // accumulator, 3 MMA issued everything, 4 epilogue saw the accumulator, 5 epilogue finished its last chunk,
-  // 6 chunk manager issued the last store; 8 + kb: operands of k-block kb landed (first 40 k-blocks)
-  long long* trace = (p.trace && rank == 0) ? p.trace : nullptr;
-  auto stamp = [&](uint32_t tile_seq, int slot) {
-    if (trace && tile_seq < 8 && slot < 64) trace[tile_seq * 64 + slot] = (long long)gtimer();
-  };
-  const uint32_t a_rows = p.flat ? BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
-  const bool direct = op.direct != 0;
-  const bool has_res = p.res != nullptr;
-
-  auto tile_coords = [&](int tile, int& n0, int& h0, int& w0, int& c_base) {
-    const int mt = tile % op.m_tiles, nt = tile / op.m_tiles;
-    n0 = 0; h0 = 0; w0 = 0;
-    if (p.flat) {
-      w0 = mt * BM;
-    } else {
-      const int tw = mt % p.tiles_w;
-      const int t2 = mt / p.tiles_w;
-      n0 = (t2 / p.tiles_h) * p.tile_n;
-      h0 = (t2 % p.tiles_h) * p.tile_h;
-      w0 = tw * p.tile_w;
-    }
-    c_base = nt * BN;
-  };
-
-  if (warp == 0) {
-    // =================================================================== operand producer
-    if (lane == 0) {
-      prefetch_tmap(&op.tmx[0]);
-      prefetch_tmap(&op.tmw[0]);
-      const uint32_t tx_bytes = NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE);
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t pit = 0;
-      for (int tile = rank; tile < n_tiles; tile += csize, ++pit) {
-        int n0, h0, w0, c_base;
-        tile_coords(tile, n0, h0, w0, c_base);
-        stamp(pit, 0);
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1, error_flag, 21);
-          const int tap = kb / p.cblocks;
-          const int cb = kb - tap * p.cblocks;
-          const int khi = tap / p.kw;
-          const int kwi = tap - khi * p.kw;
-          const uint32_t a_dst = smem_base + stage * L::STAGE;
-          const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
-          mbar_expect_tx(full_bar(stage), tx_bytes);
-          int cw, ch, cn;
-          if (p.flat) {
-            cw = w0; ch = 0; cn = 0;
-          } else {
-            cw = w0 * p.sw + kwi - p.pad_l;
-            ch = h0 * p.sh + khi - p.pad_t;
-            cn = n0;
-          }
-          tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
-          tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
-          if (NPLANES == 2) {
-            tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
-            tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        stamp(pit, 1);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // =================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc<BN>();
-      constexpr uint32_t idesc_wide = make_idesc<(NPLANES == 2 ? 2 * BN : BN)>();
-      int stage = 0;
-      uint32_t phase = 0, it = 0;
-      for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-        const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(buf), aphase ^ 1, error_flag, 22);     // epilogue drained this accumulator
-        stamp(it, 2);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * ACC_COLS;
-        uint32_t accum = 0;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(full_bar(stage), phase, error_flag, 23);
-          stamp(it, 8 + kb);
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * L::STAGE;
-          const uint32_t b_addr = a_addr + NPLANES * L::A_PLANE;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t a_hi = make_sw128_desc(a_addr + k * (UMMA_K * 2));
-            const uint64_t b_hi = make_sw128_desc(b_addr + k * (UMMA_K * 2));   // NPLANES == 2: the 2*BN rows [b_hi | b_lo]
-            if (NPLANES == 2) {
-              const uint64_t a_lo = make_sw128_desc(a_addr + L::A_PLANE + k * (UMMA_K * 2));
-              umma_bf16(tmem_d, a_hi, b_hi, idesc_wide, accum);   // cols [0,BN) += a_hi b_hi ; cols [BN,2BN) += a_hi b_lo
-              umma_bf16(tmem_d, a_lo, b_hi, idesc, 1);            // cols [0,BN) += a_lo b_hi
-            } else {
-              umma_bf16(tmem_d, a_hi, b_hi, idesc, accum);
-            }
-            accum = 1;
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar(buf));
-        stamp(it, 3);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 2) {
-    // =================================================================== chunk manager
-    // chunk j = (j / CH)-th tile of this CTA, 64-column block j % CH; it lives in unit j % U.
-    if (lane == 0 && !direct) {
-      const int my_tiles = rank < n_tiles ? (n_tiles - rank + csize - 1) / csize : 0;
-      const int total = my_tiles * CH;
-      if (has_res) prefetch_tmap(&op.tmr[0]);
-      prefetch_tmap(&op.tmy[0]);
-      auto coords = [&](int j, int& n0, int& h0, int& w0, int& c0) {
-        int c_base;
-        tile_coords(rank + (j / CH) * csize, n0, h0, w0, c_base);
-        c0 = c_base + (j % CH) * 64;
-      };
-      auto prepare = [&](int j) {               // make unit j % U ready for chunk j
-        const int u = j % U;
-        if (has_res) {
-          int n0, h0, w0, c0;
-          coords(j, n0, h0, w0, c0);
-          mbar_expect_tx(ready_bar(u), NPLANES * a_rows * 128u);
-          const uint32_t dst = unit_base + u * SS::UNIT;
-          tma_load_4d(dst, &op.tmr[0], ready_bar(u), c0, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-          if (NPLANES == 2) tma_load_4d(dst + BM * 128, &op.tmr[1], ready_bar(u), c0, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-        } else {
-          mbar_arrive(ready_bar(u));
-        }
-      };
-      auto retire = [&](int j) {                // ship chunk j out of its unit
-        const int u = j % U;
-        mbar_wait(done_bar(u), (uint32_t)(j / U) & 1u, error_flag, 24);
-        int n0, h0, w0, c0;
-        coords(j, n0, h0, w0, c0);
-        const uint32_t src = unit_base + u * SS::UNIT;
-        tma_store_4d(&op.tmy[0], src, c0, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-        if (NPLANES == 2) tma_store_4d(&op.tmy[1], src + BM * 128, c0, w0, p.flat ? 0 : h0, p.flat ? 0 : n0);
-        bulk_commit();
-        if (j % CH == CH - 1) stamp((uint32_t)(j / CH), 6);
-      };
-      if (U == 1) {
-        for (int j = 0; j < total; ++j) {
-          prepare(j);
-          retire(j);
-          bulk_wait_read0();
-        }
-      } else {
-        int prepared = 0;
-        for (; prepared < U - 1 && prepared < total; ++prepared) prepare(prepared);
-        for (int j = 0; j < total; ++j) {
-          retire(j);
-          if (prepared < total) {
-            // unit (j - 1) % U is next: the store of chunk j - 1 must have finished READING it
-            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-            prepare(prepared++);
-          }
+          const int c = blockIdx.y * BN + 8 * q + 2 * (lane & 3);
+          if (valid0) epi_pair<NPLANES>(p, pix0, c, a.x, a.y);
+          if (valid1) epi_pair<NPLANES>(p, pix1, c, a.z, a.w);
         }
       }
-      bulk_wait_all();    // every output byte of this CTA is in global memory before the grid completes
+      cluster_sync_all();   // no CTA may leave (and free its shared memory) while a peer still reads it
     }
-    __syncwarp();
-  } else {
-    // =================================================================== epilogue math (warps 3..10)
-    const int e = warp - 3;
-    const int quarter = warp & 3;                // TMEM lane quarter this warp may access
-    const int chalf = e >> 2;                    // which 32 of the chunk's 64 columns
-    const int r = quarter * 32 + lane;           // accumulator row == tile-local pixel
-    const int sw = r & 7;
-    const bool relu = p.flags & DEFER_FLAG_RELU;
-    const float* scale_ptr = p.scale;
-    const float* shift_ptr = p.shift;
-    uint32_t it = 0, j = 0;
-    for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-      const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-      int n0, h0, w0, c_base;
-      tile_coords(tile, n0, h0, w0, c_base);
-      bool valid;
-      size_t pix;
-      row_to_pixel(p, r, n0, h0, w0, valid, pix);
-      mbar_wait(tfull_bar(buf), aphase, error_flag, 25);
-      if (threadIdx.x == 96) stamp(it, 4);
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + buf * ACC_COLS + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-      for (int c = 0; c < CH; ++c, ++j) {
-        const int col0 = c * 64 + chalf * 32;        // first accumulator column of this warp's 32
-        const int chn = c_base + col0;               // first output channel
-        const int u = (int)(j % (uint32_t)U);
-        const uint32_t stg = unit_base + u * SS::UNIT + r * 128;     // shared-space address of this thread's staging row
-        if (!direct) mbar_wait(ready_bar(u), (j / (uint32_t)U) & 1u, error_flag, 26);   // residual landed / unit free
-        uint32_t v[32];
-        tmem_ld32(taddr_row + col0, v);               // warp-collective
-        if (NPLANES == 2) {
-          uint32_t v2[32];
-          tmem_ld32(taddr_row + BN + col0, v2);       // the a_hi x b_lo block of the same output columns
-#pragma unroll
-          for (int q = 0; q < 32; ++q) v[q] = __float_as_uint(__uint_as_float(v[q]) + __uint_as_float(v2[q]));
-        }
-        if (c == CH - 1) {
-          // the whole accumulator is in registers (of all chunks): hand the TMEM buffer back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));
-        }
-        float acc[32];
-        {
-          // per-channel scale / shift of these 32 channels (L1-resident after the first tile of a column block)
-          const float4* sp = reinterpret_cast<const float4*>(scale_ptr + chn);
-          const float4* fp = reinterpret_cast<const float4*>(shift_ptr + chn);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 a4 = scale_ptr ? __ldg(sp + q) : make_float4(1.f, 1.f, 1.f, 1.f);
-            const float4 b4 = shift_ptr ? __ldg(fp + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-            acc[4 * q] = fmaf(__uint_as_float(v[4 * q]), a4.x, b4.x);
-            acc[4 * q + 1] = fmaf(__uint_as_float(v[4 * q + 1]), a4.y, b4.y);
-            acc[4 * q + 2] = fmaf(__uint_as_float(v[4 * q + 2]), a4.z, b4.z);
-            acc[4 * q + 3] = fmaf(__uint_as_float(v[4 * q + 3]), a4.w, b4.w);
-          }
-        }
-        if (has_res) {
-          if (!direct) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int ch16 = ((chalf * 4) + q) ^ sw;
-              const uint4 rh4 = lds4(stg + ch16 * 16);
-              const uint32_t* hw = reinterpret_cast<const uint32_t*>(&rh4);
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                acc[q * 8 + 2 * t] += __uint_as_float(hw[t] << 16);
-                acc[q * 8 + 2 * t + 1] += __uint_as_float(hw[t] & 0xffff0000u);
-              }
-              if (NPLANES == 2) {
-                const uint4 rl4 = lds4(stg + BM * 128 + ch16 * 16);
-                const uint32_t* lw = reinterpret_cast<const uint32_t*>(&rl4);
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  acc[q * 8 + 2 * t] += __uint_as_float(lw[t] << 16);
-                  acc[q * 8 + 2 * t + 1] += __uint_as_float(lw[t] & 0xffff0000u);
-                }
-              }
-            }
-          } else if (valid) {
-            const __nv_bfloat16* rb = reinterpret_cast<const __nv_bfloat16*>(p.res) + pix * p.cout + chn;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint4 rh4 = *reinterpret_cast<const uint4*>(rb + q * 8);
-              const uint32_t* hw = reinterpret_cast<const uint32_t*>(&rh4);
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                acc[q * 8 + 2 * t] += __uint_as_float(hw[t] << 16);
-                acc[q * 8 + 2 * t + 1] += __uint_as_float(hw[t] & 0xffff0000u);
-              }
-              if (NPLANES == 2) {
-                const uint4 rl4 = *reinterpret_cast<const uint4*>(rb + p.plane_out + q * 8);
-                const uint32_t* lw = reinterpret_cast<const uint32_t*>(&rl4);
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  acc[q * 8 + 2 * t] += __uint_as_float(lw[t] << 16);
-                  acc[q * 8 + 2 * t + 1] += __uint_as_float(lw[t] & 0xffff0000u);
-                }
-              }
-            }
-          }
-        }
-        if (relu) {
-#pragma unroll
-          for (int q = 0; q < 32; ++q) acc[q] = fmaxf(acc[q], 0.f);
-        }
-        __nv_bfloat16* yp = reinterpret_cast<__nv_bfloat16*>(p.y) + pix * p.cout + chn;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 h, l;
-          uint32_t* hp = reinterpret_cast<uint32_t*>(&h);
-          uint32_t* lp = reinterpret_cast<uint32_t*>(&l);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            if (NPLANES == 2) {
-              split_bf16x2(acc[q * 8 + 2 * t], acc[q * 8 + 2 * t + 1], hp[t], lp[t]);
-            } else {
-              hp[t] = pack_bf16x2(acc[q * 8 + 2 * t], acc[q * 8 + 2 * t + 1]);
-            }
-          }
-          if (direct) {
-            if (valid) {
-              *reinterpret_cast<uint4*>(yp + q * 8) = h;
-              if (NPLANES == 2) *reinterpret_cast<uint4*>(yp + p.plane_out + q * 8) = l;
-            }
-          } else {
-            const int ch16 = ((chalf * 4) + q) ^ sw;
-            sts4(stg + ch16 * 16, h.x, h.y, h.z, h.w);
-            if (NPLANES == 2) sts4(stg + BM * 128 + ch16 * 16, l.x, l.y, l.z, l.w);
-          }
-        }
-        if (!direct) {
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // this thread's staging writes -> TMA engine
-          __syncwarp();
-          if (lane == 0) mbar_arrive(done_bar(u));
-        }
-        if (threadIdx.x == 96 && c == CH - 1) stamp(it, 5);
-      }
+    if (MODE == 2 && o + 1 < n_ops) {
+      // the next op reads this op's output through TMA (async proxy): order the generic-proxy stores before it
+      asm volatile("fence.proxy.async.global;" ::: "memory");
+      cluster_sync_all();
     }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    constexpr uint32_t ncols = 2 * ACC_COLS;
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
   }
 }
 
-// ==============================================================================================
-// Fused stem: [ZeroPadding2D +] Conv2D with a few input channels (RGB, fp32 image) + bias/BN + ReLU on the tensor cores
-// WITHOUT a patch matrix in global memory (round 1 wrote and re-read 9.6 MB per image for a 0.6 MB input).
-//
-// GEMM view: M = output pixels (flat, 128 per tile), N = 64, K = kh*kw*cin padded to a multiple of 64 (147 -> 192).
-// In NHWC a patch is kh runs of kw*cin CONTIGUOUS floats, so k -> (kernel row a, offset jj) and one range check on the
-// flat column index covers the left / right zero padding.  Per tile:
-//   * warp 0 (producer) bulk-copies the few fp32 input rows the tile's pixels need into shared memory (one
-//     cp.async.bulk, double-buffered) and TMA-loads the weight k-blocks into the operand ring;
-//   * warps 7-14 (builders, two threads per tile row) turn those rows into the A operand: K-major SWIZZLE_128B rows of bf16 hi / lo planes,
-//     written with st.shared straight into the ring stage, then fence.proxy.async + arrive on the stage's full barrier;
-//   * warp 1 issues the same two-instruction fp32-parity MMAs as conv_stream_kernel into one of two TMEM accumulators;
-//   * warps 3-6 run the epilogue (scale/shift, ReLU, hi/lo split into a swizzled staging unit), warp 2 TMA-stores it.
-// Requirements (host checks them, otherwise the im2col + GEMM pair is used): C_out == 64, (ho*wo) % 128 == 0 (a tile
-// never straddles two images), output stored locally (no peer slot), no residual.
-// ==============================================================================================
-constexpr int STEM_EPI_WARPS = 4;
-constexpr int STEM_BUILD_WARPS = 8;       // two threads per tile row: each builds 4 of the 8 16-byte chunks of a k-block row
-constexpr int STEM_THREADS = 96 + 32 * (STEM_EPI_WARPS + STEM_BUILD_WARPS);   // 480
-constexpr int STEM_CTL_BYTES = 2048;      // barriers + TMEM slot (first 512 B) | k -> (byte offset, kernel row, column) table (<= 384 entries)
-constexpr int STEM_TABLE_OFF = 512;
+template <int NPLANES, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_umma_kernel(const __grid_constant__ MegaOp op, int stages, int pdl) {
+  conv_body<NPLANES, BN, 0>(&op, 1, stages, pdl);
+}
+
+template <int NPLANES, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  conv_body<NPLANES, BN, 1>(ops, 1, stages, pdl);
+}
 
 template <int NPLANES>
-struct StemSmem {
-  using L = SmemLayout<NPLANES, 64>;
-  static constexpr int UNIT = NPLANES * BM * 128;
-  __host__ __device__ static constexpr int unit_off(int stages) { return stages * L::STAGE; }
-  __host__ __device__ static constexpr int in_off(int stages) { return stages * L::STAGE + 2 * UNIT; }
-  __host__ __device__ static constexpr int ctl_off(int stages, int in_bytes) { return in_off(stages) + 2 * in_bytes; }
-  __host__ __device__ static constexpr int total(int stages, int in_bytes) { return ctl_off(stages, in_bytes) + STEM_CTL_BYTES + 1024; }
-};
-
-template <int NPLANES>
-__global__ void __launch_bounds__(STEM_THREADS, 1)
-conv_stem_kernel(const MegaOp* __restrict__ opp, int stages, int in_bytes, int pdl, int* error_flag) {
-  constexpr int BN = 64;
-  using L = SmemLayout<NPLANES, BN>;
-  using SS = StemSmem<NPLANES>;
-  constexpr int ACC_COLS = NPLANES == 2 ? 2 * BN : BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t smem_base = smem_u32(smem);
-  const int STAGES = stages;
-  const uint32_t bar_base = smem_base + SS::ctl_off(STAGES, in_bytes);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };                      // [0, 8): 1 producer + 4 builder warps
-  auto empty_bar = [&](int s) { return bar_base + 8u * (8 + s); };               // [8, 16)
-  auto tfull_bar = [&](int b) { return bar_base + 8u * (16 + b); };
-  auto tempty_bar = [&](int b) { return bar_base + 8u * (18 + b); };
-  auto ready_bar = [&](int u) { return bar_base + 8u * (20 + u); };              // staging unit may be written
-  auto done_bar = [&](int u) { return bar_base + 8u * (22 + u); };               // staging unit holds a finished tile
-  auto in_full_bar = [&](int b) { return bar_base + 8u * (24 + b); };            // input rows landed
-  auto in_empty_bar = [&](int b) { return bar_base + 8u * (26 + b); };           // builders are done with them
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SS::ctl_off(STAGES, in_bytes) + 8 * 28);
-  const uint32_t unit_base = smem_base + SS::unit_off(STAGES);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const MegaOp& op = *opp;
-  const KParams& p = op.p;
-  const int n_tiles = op.m_tiles;                  // one 64-wide column block
-  const int rank = (int)blockIdx.x, csize = (int)gridDim.x;
-  const int H = op.stem_h, W = op.stem_w, CIN = op.stem_cin;
-  const int row_len = W * CIN;                     // floats per input row
-  const int run = op.stem_kw * CIN;                // contiguous floats per kernel row of a patch
-  const int hw_out = p.ho * p.wo;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1 + STEM_BUILD_WARPS);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), STEM_EPI_WARPS);
-      mbar_init(ready_bar(b), 1);
-      mbar_init(done_bar(b), STEM_EPI_WARPS);
-      mbar_init(in_full_bar(b), 1);
-      mbar_init(in_empty_bar(b), STEM_BUILD_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    constexpr uint32_t ncols = 2 * ACC_COLS;
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (pdl) {
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  }
-
-  // optional phase trace (DEFER_STEM_TRACE=<file>): CTA 0, first 8 tiles, 64 slots each: 0 producer issued the input rows,
-  // 1 builders saw them, 2 MMA got the accumulator, 3 MMA issued the tile, 4 epilogue saw the accumulator, 5 epilogue done,
-  // 6 store issued, 8 + kb builder finished k-block kb, 16 + kb MMA saw k-block kb complete
-  long long* trace = (p.trace && rank == 0) ? p.trace : nullptr;
-  auto stamp = [&](uint32_t tile_seq, int slot) {
-    if (trace && tile_seq < 8 && slot < 64) trace[tile_seq * 64 + slot] = (long long)gtimer();
-  };
-  // input rows a tile needs: pixels [p0, p0 + 128) of image nb cover output rows oh0..oh1
-  auto tile_rows = [&](int tile, int& nb, int& oh0, int& ih_lo, int& n_rows) {
-    const int p0 = tile * BM;
-    nb = p0 / hw_out;
-    const int q0 = p0 - nb * hw_out;
-    oh0 = q0 / p.wo;
-    const int oh1 = (q0 + BM - 1) / p.wo;
-    int lo = oh0 * op.stem_sh - op.stem_pad_t;
-    int hi = oh1 * op.stem_sh - op.stem_pad_t + op.stem_kh - 1;
-    if (lo < 0) lo = 0;
-    if (hi > H - 1) hi = H - 1;
-    ih_lo = lo;
-    n_rows = hi - lo + 1;
-  };
-
-  if (warp == 0) {
-    // =================================================================== producer: input rows + weight k-blocks
-    if (lane == 0) {
-      prefetch_tmap(&op.tmw[0]);
-      const uint32_t b_bytes = NPLANES * (uint32_t)L::B_PLANE;
-      int stage = 0;
-      uint32_t phase = 0, it = 0;
-      for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-        const uint32_t ib = it & 1, iph = (it >> 1) & 1;
-        int nb, oh0, ih_lo, n_rows;
-        tile_rows(tile, nb, oh0, ih_lo, n_rows);
-        mbar_wait(in_empty_bar(ib), iph ^ 1, error_flag, 31);
-        const uint32_t bytes = (uint32_t)n_rows * (uint32_t)row_len * 4u;
-        mbar_expect_tx(in_full_bar(ib), bytes);
-        const float* src = op.stem_x + ((size_t)nb * H + ih_lo) * row_len;
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(smem_base + SS::in_off(STAGES) + ib * in_bytes), "l"(src), "r"(bytes), "r"(in_full_bar(ib)) : "memory");
-        stamp(it, 0);
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1, error_flag, 32);
-          const uint32_t b_dst = smem_base + stage * L::STAGE + NPLANES * L::A_PLANE;
-          mbar_expect_tx(full_bar(stage), b_bytes);
-          tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), kb * BK, 0, 0);
-          if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), kb * BK, 0, 0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // =================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc<BN>();
-      constexpr uint32_t idesc_wide = make_idesc<(NPLANES == 2 ? 2 * BN : BN)>();
-      int stage = 0;
-      uint32_t phase = 0, it = 0;
-      for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-        const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-        mbar_wait(tempty_bar(buf), aphase ^ 1, error_flag, 33);
-        stamp(it, 2);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + buf * ACC_COLS;
-        uint32_t accum = 0;
-        for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(full_bar(stage), phase, error_flag, 34);
-          stamp(it, 16 + kb);
-          tc_fence_after();
-          const uint32_t a_addr = smem_base + stage * L::STAGE;
-          const uint32_t b_addr = a_addr + NPLANES * L::A_PLANE;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t a_hi = make_sw128_desc(a_addr + k * (UMMA_K * 2));
-            const uint64_t b_hi = make_sw128_desc(b_addr + k * (UMMA_K * 2));
-            if (NPLANES == 2) {
-              const uint64_t a_lo = make_sw128_desc(a_addr + L::A_PLANE + k * (UMMA_K * 2));
-              umma_bf16(tmem_d, a_hi, b_hi, idesc_wide, accum);
-              umma_bf16(tmem_d, a_lo, b_hi, idesc, 1);
-            } else {
-              umma_bf16(tmem_d, a_hi, b_hi, idesc, accum);
-            }
-            accum = 1;
-          }
-          umma_commit(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(tfull_bar(buf));
-        stamp(it, 3);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 2) {
-    // =================================================================== store manager (two staging units)
-    if (lane == 0) {
-      prefetch_tmap(&op.tmy[0]);
-      uint32_t it = 0;
-      mbar_arrive(ready_bar(0));
-      mbar_arrive(ready_bar(1));
-      for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-        const uint32_t u = it & 1, ph = (it >> 1) & 1;
-        mbar_wait(done_bar(u), ph, error_flag, 35);
-        const uint32_t src = unit_base + u * SS::UNIT;
-        tma_store_4d(&op.tmy[0], src, 0, tile * BM, 0, 0);
-        if (NPLANES == 2) tma_store_4d(&op.tmy[1], src + BM * 128, 0, tile * BM, 0, 0);
-        bulk_commit();
-        stamp(it, 6);
-        if (tile + csize < n_tiles) {
-          // unit u ^ 1 (tile it + 1) is already released; unit u is needed again by tile it + 2: its store (this one)
-          // must have finished reading - checked one iteration later, when only the newest group may still be pending
-          if (it >= 1) {
-            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-            mbar_arrive(ready_bar(u ^ 1));
-          }
-        }
-      }
-      bulk_wait_all();
-    }
-    __syncwarp();
-  } else if (warp < 3 + STEM_EPI_WARPS) {
-    // =================================================================== epilogue (warps 3..6): 64 columns per thread row
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const int sw = r & 7;
-    const bool relu = p.flags & DEFER_FLAG_RELU;
-    const float* scale_ptr = p.scale;
-    const float* shift_ptr = p.shift;
-    uint32_t it = 0;
-    for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-      const uint32_t buf = it & 1, aphase = (it >> 1) & 1;
-      mbar_wait(tfull_bar(buf), aphase, error_flag, 36);
-      if (threadIdx.x == 96) stamp(it, 4);
-      tc_fence_after();
-      mbar_wait(ready_bar(buf), aphase, error_flag, 37);       // staging unit `buf` is free (its previous store has read it)
-      const uint32_t taddr_row = tmem_base + buf * ACC_COLS + ((uint32_t)(quarter * 32) << 16);
-      const uint32_t stg = unit_base + buf * SS::UNIT + r * 128;
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        const int col0 = half * 32;
-        uint32_t v[32];
-        tmem_ld32(taddr_row + col0, v);
-        if (NPLANES == 2) {
-          uint32_t v2[32];
-          tmem_ld32(taddr_row + BN + col0, v2);
-#pragma unroll
-          for (int q = 0; q < 32; ++q) v[q] = __float_as_uint(__uint_as_float(v[q]) + __uint_as_float(v2[q]));
-        }
-        if (half == 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));
-        }
-        float acc[32];
-        {
-          const float4* sp = reinterpret_cast<const float4*>(scale_ptr + col0);
-          const float4* fp = reinterpret_cast<const float4*>(shift_ptr + col0);
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 a4 = scale_ptr ? __ldg(sp + q) : make_float4(1.f, 1.f, 1.f, 1.f);
-            const float4 b4 = shift_ptr ? __ldg(fp + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-            acc[4 * q] = fmaf(__uint_as_float(v[4 * q]), a4.x, b4.x);
-            acc[4 * q + 1] = fmaf(__uint_as_float(v[4 * q + 1]), a4.y, b4.y);
-            acc[4 * q + 2] = fmaf(__uint_as_float(v[4 * q + 2]), a4.z, b4.z);
-            acc[4 * q + 3] = fmaf(__uint_as_float(v[4 * q + 3]), a4.w, b4.w);
-          }
-        }
-        if (relu) {
-#pragma unroll
-          for (int q = 0; q < 32; ++q) acc[q] = fmaxf(acc[q], 0.f);
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 h, l;
-          uint32_t* hp = reinterpret_cast<uint32_t*>(&h);
-          uint32_t* lp = reinterpret_cast<uint32_t*>(&l);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            if (NPLANES == 2) split_bf16x2(acc[q * 8 + 2 * t], acc[q * 8 + 2 * t + 1], hp[t], lp[t]);
-            else hp[t] = pack_bf16x2(acc[q * 8 + 2 * t], acc[q * 8 + 2 * t + 1]);
-          }
-          const int ch16 = ((half * 4) + q) ^ sw;
-          sts4(stg + ch16 * 16, h.x, h.y, h.z, h.w);
-          if (NPLANES == 2) sts4(stg + BM * 128 + ch16 * 16, l.x, l.y, l.z, l.w);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(done_bar(buf));
-      if (threadIdx.x == 96) stamp(it, 5);
-    }
-  } else {
-    // =================================================================== A builders (warps 7..14): two threads per tile row
-    const int bt = threadIdx.x - 32 * (3 + STEM_EPI_WARPS);          // 0..255
-    const int r = bt & (BM - 1);
-    const int g0 = (bt >> 7) * 4;                                    // this thread's 4 chunks (32 k) of every k-block
-    const int sw = r & 7;
-    // k -> patch geometry, computed once per CTA: entry = byte offset of element k inside the staged rows (20 bits) |
-    // kernel row a << 20 (a = 31 for the K padding: never valid) | column offset jj << 25
-    const uint32_t tbl = smem_base + SS::ctl_off(STAGES, in_bytes) + STEM_TABLE_OFF;
-    for (int k = bt; k < p.k_blocks * BK; k += 32 * STEM_BUILD_WARPS) {
-      const int a = k / run, jj = k - a * run;
-      const uint32_t e = k < op.stem_K ? ((uint32_t)((a * row_len + jj) * 4) | ((uint32_t)a << 20) | ((uint32_t)jj << 25))
-                                       : (31u << 20);
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(tbl + (uint32_t)k * 4u), "r"(e) : "memory");
-    }
-    // (measured: making the element loads unconditional - address select onto a zero word instead of a branch - is slower,
-    // 117 vs 103 us per 32 images: the builders are not bound by branch / load dependencies)
-    asm volatile("bar.sync 2, %0;" ::"n"(32 * STEM_BUILD_WARPS) : "memory");   // builder warps only
-    int stage = 0;
-    uint32_t phase = 0, it = 0;
-    for (int tile = rank; tile < n_tiles; tile += csize, ++it) {
-      const uint32_t ib = it & 1, iph = (it >> 1) & 1;
-      int nb, oh0, ih_lo, n_rows;
-      tile_rows(tile, nb, oh0, ih_lo, n_rows);
-      const int q = tile * BM + r - nb * hw_out;       // pixel index inside the image
-      const int oh = q / p.wo, ow = q - oh * p.wo;
-      const int ih0 = oh * op.stem_sh - op.stem_pad_t;                 // input row of kernel row 0
-      const int col0 = (ow * op.stem_sw - op.stem_pad_l) * CIN;        // flat column of the patch's first element
-      // kernel rows whose input row exists (zero padding above / below; bit 31 stays 0 = the K padding): one bit each
-      uint32_t rowmask = 0;
-      for (int a = 0; a < op.stem_kh; ++a) {
-        const int ih = ih0 + a;
-        if (ih >= ih_lo && ih < ih_lo + n_rows) rowmask |= 1u << a;
-      }
-      const bool colfast = col0 >= 0 && col0 + run <= row_len;         // no left / right padding inside this patch
-      // shared-space byte address of the patch's first element (may point before the buffer: only valid elements are read)
-      const int rows = (int)(smem_base + SS::in_off(STAGES) + ib * in_bytes) + ((ih0 - ih_lo) * row_len + col0) * 4;
-      mbar_wait(in_full_bar(ib), iph, error_flag, 38);
-      if (bt == 0) stamp(it, 1);
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1, error_flag, 39);
-        const uint32_t a_row = smem_base + stage * L::STAGE + r * 128;
-        const uint32_t tk = tbl + (uint32_t)(kb * BK + g0 * 8) * 4u;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const uint4 e0 = lds4(tk + g * 32), e1 = lds4(tk + g * 32 + 16);   // warp-uniform addresses: broadcast loads
-          const uint32_t ent[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
-          float v[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint32_t e = ent[j];
-            float val = 0.f;
-            if ((rowmask >> ((e >> 20) & 31u)) & 1u) {
-              const int cj = col0 + (int)(e >> 25);
-              if (colfast || (cj >= 0 && cj < row_len)) val = lds_f32((uint32_t)(rows + (int)(e & 0xFFFFFu)));
-            }
-            v[j] = val;
-          }
-          const int ch16 = (g0 + g) ^ sw;
-          if (NPLANES == 2) {
-            uint4 hv, lv;
-            split_bf16x2(v[0], v[1], hv.x, lv.x);
-            split_bf16x2(v[2], v[3], hv.y, lv.y);
-            split_bf16x2(v[4], v[5], hv.z, lv.z);
-            split_bf16x2(v[6], v[7], hv.w, lv.w);
-            sts4(a_row + ch16 * 16, hv.x, hv.y, hv.z, hv.w);
-            sts4(a_row + L::A_PLANE + ch16 * 16, lv.x, lv.y, lv.z, lv.w);
-          } else {
-            uint4 hv;
-            hv.x = pack_bf16x2(v[0], v[1]);
-            hv.y = pack_bf16x2(v[2], v[3]);
-            hv.z = pack_bf16x2(v[4], v[5]);
-            hv.w = pack_bf16x2(v[6], v[7]);
-            sts4(a_row + ch16 * 16, hv.x, hv.y, hv.z, hv.w);
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // st.shared -> visible to tcgen05.mma (async proxy)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full_bar(stage));
-        if (bt == 0) stamp(it, 8 + kb);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(in_empty_bar(ib));
-    }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    constexpr uint32_t ncols = 2 * ACC_COLS;
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(ncols) : "memory");
-  }
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_mega_kernel(const MegaOp* __restrict__ ops, int n_ops, int stages) {
+  conv_body<NPLANES, MEGA_BN, 2>(ops, n_ops, stages, 0);
 }
 
 // weights: fp32 HWIO [tap][cin][cout]  ->  bf16 [plane][tap][cout][cin]
@@ -2098,36 +659,72 @@ int encode_map(CUtensorMap* map, void* base, int rank, const uint64_t* dims, con
   return DEFER_OK;
 }
 
-template <int NPLANES, int BN, int EW>
-int launch_t(const UmmaConvPlan& plan, const UmmaConvLaneArgs& a, const KParams& kp, cudaStream_t st) {
-  using L = SmemLayout<NPLANES, BN>;
-  constexpr int SMEM_MAX = 225 * 1024;   // opt-in limit is 227 KB per block INCLUDING static shared memory
-  static bool attr_set[64] = {false};
+template <auto kernel>
+int set_smem_attr(bool cluster16 = false) {
+  static bool attr_set[64] = {false};   // one flag array per kernel instantiation
   int dev = 0;
   DEFER_CUDA(cudaGetDevice(&dev));
   if (dev < 64 && !attr_set[dev]) {
-    DEFER_CUDA(cudaFuncSetAttribute(conv_umma_kernel<NPLANES, BN, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX));
-    prefer_max_smem(conv_umma_kernel<NPLANES, BN, EW>);
+    DEFER_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP));
+    if (cluster16) DEFER_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    prefer_max_smem(kernel);
     attr_set[dev] = true;
   }
-  int stages = kp.stages < 1 ? 1 : (kp.stages > L::MAX_STAGES ? L::MAX_STAGES : kp.stages);
-  while (stages > 1 && L::total(stages) + kp.res_stage_bytes > SMEM_MAX) --stages;
-  const size_t smem = (size_t)L::total(stages) + kp.res_stage_bytes;
-  KParams kq = kp;
-  kq.stages = stages;
-  dim3 grid(plan.tiles_n * plan.tiles_h * plan.tiles_w, plan.cout / BN, plan.splits);
+  return DEFER_OK;
+}
+
+int sm_count() {
+  static int sms[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev >= 64) return 1;
+  if (!sms[dev]) cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
+  return sms[dev] > 0 ? sms[dev] : 1;
+}
+
+void fill_op(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, MegaOp* out) {
+  MegaOp& op = *out;
+  memset(&op, 0, sizeof op);
+  op.tmx[0] = a.tmap_x[0];
+  op.tmx[1] = a.tmap_x[1];
+  op.tmw[0] = P.tmap_w[0];
+  op.tmw[1] = P.tmap_w[1];
+  KParams& kp = op.p;
+  kp.n = P.n; kp.ho = P.ho; kp.wo = P.wo; kp.cout = P.cout;
+  kp.tile_n = P.tile_n; kp.tile_h = P.tile_h; kp.tile_w = P.tile_w; kp.tiles_h = P.tiles_h; kp.tiles_w = P.tiles_w;
+  kp.flat = P.flat;
+  kp.m_total = P.n * P.ho * P.wo;
+  kp.kh = P.kh; kp.kw = P.kw; kp.sh = P.sh; kp.sw = P.sw; kp.pad_t = P.pad_t; kp.pad_l = P.pad_l;
+  kp.cblocks = P.cin / 64;
+  kp.k_blocks = P.k_blocks;
+  kp.splits = P.splits;
+  kp.cluster = P.cluster;
+  kp.flags = P.flags;
+  kp.scale = P.scale; kp.shift = P.shift;
+  kp.res = (P.flags & DEFER_FLAG_RESIDUAL) ? a.res : nullptr;
+  kp.y = a.y;
+  kp.partial = a.partial;
+  kp.counters = a.counters;
+  kp.plane_out = (size_t)P.n * P.ho * P.wo * P.cout;
+  op.m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
+  op.n_tiles = P.cout / P.bn;
+}
+
+template <int NPLANES, int BN>
+int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t st) {
+  using L = Smem<NPLANES, BN>;
+  DEFER_TRY((set_smem_attr<conv_umma_kernel<NPLANES, BN>>()));
+  MegaOp op;
+  fill_op(P, a, &op);
+  // >= 2: a consumer releases a stage only once the NEXT k-block's wgmmas are issued (wgmma.wait_group 1)
+  int stages = P.stages < 2 ? 2 : (P.stages > L::max_stages() ? L::max_stages() : P.stages);
+  const size_t smem = (size_t)L::total(stages, P.cluster != 0);
+  dim3 grid(op.m_tiles, op.n_tiles, P.splits);
   static const int pdl = env_int("DEFER_PDL", 0);
-  kq.pdl = pdl;
-  // tensor maps of the output / residual tiles (staged epilogue); unused otherwise - pass valid dummies
-  const CUtensorMap& ty0 = kq.tma_epi ? a.tmap_y[0] : a.tmap_x[0];
-  const CUtensorMap& ty1 = kq.tma_epi ? a.tmap_y[NPLANES - 1] : a.tmap_x[0];
-  const CUtensorMap& tr0 = (kq.tma_epi && kq.res) ? a.tmap_r[0] : a.tmap_x[0];
-  const CUtensorMap& tr1 = (kq.tma_epi && kq.res) ? a.tmap_r[NPLANES - 1] : a.tmap_x[0];
-  if (pdl || kq.cluster) {
+  if (pdl || P.cluster) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof cfg);
     cfg.gridDim = grid;
-    cfg.blockDim = dim3(64 + 32 * EW, 1, 1);
+    cfg.blockDim = dim3(NUM_THREADS, 1, 1);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[2];
@@ -2137,22 +734,79 @@ int launch_t(const UmmaConvPlan& plan, const UmmaConvLaneArgs& a, const KParams&
       attr[na].val.programmaticStreamSerializationAllowed = 1;
       ++na;
     }
-    if (kq.cluster) {   // the `splits` CTAs of one output tile (grid.z) are one thread-block cluster
+    if (P.cluster) {   // the `splits` CTAs of one output tile (grid.z) are one thread-block cluster
       attr[na].id = cudaLaunchAttributeClusterDimension;
       attr[na].val.clusterDim.x = 1;
       attr[na].val.clusterDim.y = 1;
-      attr[na].val.clusterDim.z = (unsigned)plan.splits;
+      attr[na].val.clusterDim.z = (unsigned)P.splits;
       ++na;
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<NPLANES, BN, EW>, a.tmap_x[0], a.tmap_x[NPLANES - 1], plan.tmap_w[0],
-                                  plan.tmap_w[NPLANES - 1], ty0, ty1, tr0, tr1, kq));
+    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<NPLANES, BN>, op, stages, pdl));
     return DEFER_OK;
   }
-  conv_umma_kernel<NPLANES, BN, EW><<<grid, 64 + 32 * EW, smem, st>>>(a.tmap_x[0], a.tmap_x[NPLANES - 1], plan.tmap_w[0],
-                                                                    plan.tmap_w[NPLANES - 1], ty0, ty1, tr0, tr1, kq);
+  conv_umma_kernel<NPLANES, BN><<<grid, NUM_THREADS, smem, st>>>(op, stages, 0);
   DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
+// persistent grid over the tiles of one op in device memory: every CTA walks ceil(n_tiles / grid) tiles, so the launch
+// lasts `rounds` tile-times whatever the grid is; take the SMALLEST grid that still finishes in the minimum number of
+// rounds and leave the other SMs to the lanes running next to this one
+template <int NPLANES, int BN>
+int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
+  using L = Smem<NPLANES, BN>;
+  DEFER_TRY((set_smem_attr<conv_stream_kernel<NPLANES, BN>>()));
+  if (stages > L::max_stages()) stages = L::max_stages();
+  if (stages < 2) stages = 2;
+  const int sms = sm_count();
+  int grid = sms < n_tiles ? sms : n_tiles;
+  const int rounds = (n_tiles + grid - 1) / grid;
+  grid = (n_tiles + rounds - 1) / rounds;
+  const size_t smem = (size_t)L::total(stages, false);
+  static const int pdl = env_int("DEFER_PDL", 0);
+  if (pdl) {
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof cfg);
+    cfg.gridDim = dim3(grid, 1, 1);
+    cfg.blockDim = dim3(NUM_THREADS, 1, 1);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_stream_kernel<NPLANES, BN>, reinterpret_cast<const MegaOp*>(dev_op), stages, 1));
+    return DEFER_OK;
+  }
+  conv_stream_kernel<NPLANES, BN><<<grid, NUM_THREADS, smem, st>>>(reinterpret_cast<const MegaOp*>(dev_op), stages, 0);
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
+template <int NPLANES>
+int launch_mega_t(const void* dev_ops, int n_ops, int stages, cudaStream_t st) {
+  using L = Smem<NPLANES, MEGA_BN>;
+  DEFER_TRY(set_smem_attr<conv_mega_kernel<NPLANES>>(true));
+  if (stages < 2) stages = 2;   // see launch_op_t
+  if (stages > L::max_stages()) stages = L::max_stages();
+  const int cluster = umma_mega_cluster_size();
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof cfg);
+  cfg.gridDim = dim3(cluster, 1, 1);
+  cfg.blockDim = dim3(NUM_THREADS, 1, 1);
+  cfg.dynamicSmemBytes = L::total(stages, false);
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_mega_kernel<NPLANES>, reinterpret_cast<const MegaOp*>(dev_ops), n_ops, stages));
   return DEFER_OK;
 }
 
@@ -2171,18 +825,11 @@ bool umma_conv_supported(int fmt, int n, int h, int w, int cin, int ho, int wo, 
   return true;
 }
 
-static void timeline_init();
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
-
 int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int kw,
                       int sh, int sw, int pad_t, int pad_l, uint32_t flags, const float* w_hwio_dev, const float* scale_dev,
                       const float* shift_dev, bool mega, int stream_bn) {
   UmmaConvPlan& P = *plan;
   P = UmmaConvPlan();
-  timeline_init();
   P.fmt = fmt;
   P.nplanes = fmt == FMT_BF16X2 ? 2 : 1;
   P.n = n; P.h = h; P.w = w; P.cin = cin; P.ho = ho; P.wo = wo; P.cout = cout;
@@ -2224,17 +871,9 @@ int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin,
   }
   const int m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
 
-  // ---- N tile, split-K and ring depth.
-  // With several microbatches in flight the GPU is bound by L2->SM operand traffic and launch rate, not
-  // by the parallelism of one launch (measured: BN = 128 wherever C_out allows and split-K only below 4
-  // CTAs gave +16 % inferences/s over BN = 64 / 16-CTA targets).  The A tile is re-read once per N tile
-  // and the weights once per M tile, so fat N tiles cut traffic; split-K adds partial-tile traffic.
+  // ---- N tile, split-K and ring depth.  The A tile is re-read once per N tile and the weights once per M tile, so
+  // wide N tiles cut L2 -> SM traffic; split-K adds partial-tile traffic and is kept for launches of very few CTAs.
   P.bn = (cout % 128 == 0 && (long long)m_tiles * (cout / 128) >= env_int("DEFER_UMMA_BN128_MIN_CTAS", 1)) ? 128 : 64;
-  // staged (TMA) epilogue: default.  With a residual the tile's residual copy needs its own shared memory (64 KB for a
-  // 128-wide fp32-parity tile); DEFER_UMMA_TE_RES_BN64=1 switches those ops to 64-wide tiles (two CTAs per SM, twice
-  // the CTAs) - measured equal within noise, so the wide tile stays the default.
-  P.tma_epi = env_int("DEFER_UMMA_TMA_EPI", 1) ? 1 : 0;
-  if (P.tma_epi && (flags & DEFER_FLAG_RESIDUAL) && env_int("DEFER_UMMA_TE_RES_BN64", 0)) P.bn = 64;
   int force_bn = env_int("DEFER_UMMA_BN", 0);
   if (force_bn == 64 || (force_bn == 128 && cout % 128 == 0)) P.bn = force_bn;
   int ctas = m_tiles * (cout / P.bn);
@@ -2254,10 +893,9 @@ int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin,
     int per = (P.k_blocks + force_split - 1) / force_split;
     P.splits = (P.k_blocks + per - 1) / per;
   }
-  // ---- cluster split-K (default): at batch 1 a launch has few tiles and each CTA's K loop is bound by what ONE SM
-  // can pull out of L2 (~0.7 us per 64 KB k-block measured), followed by a 128-column epilogue in one warp per
-  // scheduler.  A cluster of S CTAs per output tile cuts both by S; the partial tiles meet in distributed shared
-  // memory.  S = largest of {8, 4, 2} that leaves >= DEFER_UMMA_CSPLIT_KB k-blocks per CTA.
+  // ---- cluster split-K (opt-in, DEFER_UMMA_CLUSTER=1): S CTAs per output tile split the K loop and the epilogue;
+  // the partial tiles meet in distributed shared memory.  S = largest of {8, 4, 2} that leaves >= DEFER_UMMA_CSPLIT_KB
+  // k-blocks per CTA.
   P.cluster = 0;
   if (env_int("DEFER_UMMA_CLUSTER", 0) && force_split <= 0 && !mega) {
     const int min_kb = env_int("DEFER_UMMA_CSPLIT_KB", 4);
@@ -2285,19 +923,9 @@ int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin,
   }
   {
     int kb_per = (P.k_blocks + P.splits - 1) / P.splits;
-    int st = kb_per <= 2 ? kb_per : (kb_per <= 6 ? 2 : 4);
-    if (P.cluster) {
-      // short K loops: put every k-block in flight at once; the ring must also hold the fp32 partial tile
-      st = kb_per;
-      const int stage_bytes = P.nplanes * (BM + P.bn) * 128;
-      const int red_bytes = BM * (P.bn + 4) * 4;
-      const int need = (red_bytes + stage_bytes - 1) / stage_bytes;
-      int cap = env_int("DEFER_UMMA_CSPLIT_STAGES", 3);
-      if (st > cap) st = cap;
-      if (st < need) st = need;
-    }
+    int st = kb_per <= 2 ? 2 : (kb_per <= 6 ? 3 : 4);
     int force_st = env_int("DEFER_UMMA_STAGES", 0);
-    if (force_st > 0 && !P.cluster) st = force_st;
+    if (force_st > 0) st = force_st;
     P.stages = st;
   }
 
@@ -2348,37 +976,6 @@ int umma_conv_bind(const UmmaConvPlan& P, UmmaConvLaneArgs* a, const void* x, co
   if (P.nplanes == 1) a->tmap_x[1] = a->tmap_x[0];
   a->res = res;
   a->y = y;
-  a->has_out_maps = false;
-  if (P.splits == 1) {
-    // output / residual tiles as 64-channel TMA boxes (staged epilogues: per-op, persistent-grid, megakernel)
-    size_t yelems = (size_t)P.n * P.ho * P.wo * P.cout;
-    for (int pl = 0; pl < P.nplanes; ++pl) {
-      for (int which = 0; which < 2; ++which) {
-        const void* basep = which == 0 ? (const void*)y : res;
-        CUtensorMap* dst = which == 0 ? &a->tmap_y[pl] : &a->tmap_r[pl];
-        if (!basep) { memset(dst, 0, sizeof(CUtensorMap)); continue; }
-        uint8_t* base = (uint8_t*)basep + pl * yelems * 2;
-        uint32_t es[4] = {1, 1, 1, 1};
-        if (P.flat) {
-          uint64_t m = (uint64_t)P.n * P.ho * P.wo;
-          uint64_t dims[4] = {(uint64_t)P.cout, m, 1, 1};
-          uint64_t strides[3] = {(uint64_t)P.cout * 2, m * P.cout * 2, m * P.cout * 2};
-          uint32_t box[4] = {64, BM, 1, 1};
-          DEFER_TRY(encode_map(dst, base, 4, dims, strides, box, es));
-        } else {
-          uint64_t dims[4] = {(uint64_t)P.cout, (uint64_t)P.wo, (uint64_t)P.ho, (uint64_t)P.n};
-          uint64_t strides[3] = {(uint64_t)P.cout * 2, (uint64_t)P.wo * P.cout * 2, (uint64_t)P.ho * P.wo * P.cout * 2};
-          uint32_t box[4] = {64, (uint32_t)P.tile_w, (uint32_t)P.tile_h, (uint32_t)P.tile_n};
-          DEFER_TRY(encode_map(dst, base, 4, dims, strides, box, es));
-        }
-      }
-    }
-    if (P.nplanes == 1) {
-      a->tmap_y[1] = a->tmap_y[0];
-      a->tmap_r[1] = a->tmap_r[0];
-    }
-    a->has_out_maps = true;
-  }
   a->partial = nullptr;
   a->counters = nullptr;
   if (P.splits > 1 && !P.cluster) {
@@ -2397,98 +994,12 @@ void umma_conv_unbind(UmmaConvLaneArgs* a) {
   a->counters = nullptr;
 }
 
-// DEFER_TIMELINE=<path> (debug): every CTA of the per-op conv kernel logs {start, end, SM, op tag, 4 phase stamps}
-// with %globaltimer; written when a stage is destroyed; summarised by tools/timeline_stats.py.
-constexpr int TIMELINE_CAP = 1 << 19;
-static long long* g_timeline = nullptr;
-static long long* g_stem_trace = nullptr;   // DEFER_STEM_TRACE: phase stamps of conv_stem_kernel's CTA 0 (debug)
-void umma_timeline_dump() {
-  if (g_stem_trace && getenv("DEFER_STEM_TRACE")) {
-    long long hb[8 * 64];
-    if (cudaMemcpy(hb, g_stem_trace, sizeof hb, cudaMemcpyDeviceToHost) == cudaSuccess) {
-      FILE* f = fopen(getenv("DEFER_STEM_TRACE"), "a");
-      if (f) {
-        fprintf(f, "# conv_stem_kernel, CTA 0, ns since the first stamp\n");
-        for (int i = 0; i < 8; ++i) {
-          if (!hb[i * 64]) continue;
-          fprintf(f, "tile %d:", i);
-          for (int j = 0; j < 64; ++j)
-            if (hb[i * 64 + j]) fprintf(f, " %d=%lld", j, hb[i * 64 + j] - hb[0]);
-          fprintf(f, "\n");
-        }
-        fclose(f);
-      }
-    }
-  }
-  const char* path = getenv("DEFER_TIMELINE");
-  if (!g_timeline || !path) return;
-  std::vector<long long> h(8 + (size_t)TIMELINE_CAP * 8);
-  if (cudaMemcpy(h.data(), g_timeline, h.size() * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return;
-  long long n = h[0] < TIMELINE_CAP ? h[0] : TIMELINE_CAP;
-  FILE* f = fopen(path, "w");
-  if (!f) return;
-  for (long long i = 0; i < n; ++i) {
-    const long long* e = h.data() + 8 + i * 8;
-    fprintf(f, "%lld %lld %lld %lld %lld %lld %lld %lld\n", e[0], e[1], e[2], e[3], e[4], e[5], e[6], e[7]);
-  }
-  fclose(f);
-}
-static void timeline_init() {   // called from umma_conv_prepare: never inside a stream capture
-  static bool tried = false;
-  if (tried) return;
-  tried = true;
-  if (!getenv("DEFER_TIMELINE")) return;
-  size_t bytes = (8 + (size_t)TIMELINE_CAP * 8) * sizeof(long long);
-  if (cudaMalloc((void**)&g_timeline, bytes) == cudaSuccess) cudaMemset(g_timeline, 0, bytes);
-  else g_timeline = nullptr;
-}
-
-static void fill_kparams(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, KParams* out) {
-  KParams& kp = *out;
-  kp.n = P.n; kp.ho = P.ho; kp.wo = P.wo; kp.cout = P.cout;
-  kp.tile_n = P.tile_n; kp.tile_h = P.tile_h; kp.tile_w = P.tile_w; kp.tiles_h = P.tiles_h; kp.tiles_w = P.tiles_w;
-  kp.flat = P.flat;
-  kp.m_total = P.n * P.ho * P.wo;
-  kp.kh = P.kh; kp.kw = P.kw; kp.sh = P.sh; kp.sw = P.sw; kp.pad_t = P.pad_t; kp.pad_l = P.pad_l;
-  kp.cblocks = P.cin / 64;
-  kp.k_blocks = P.k_blocks;
-  kp.splits = P.splits;
-  kp.cluster = P.cluster;
-  kp.stages = P.stages;
-  static const int epi_direct = env_int("DEFER_EPILOGUE_DIRECT", 0);
-  kp.fast = env_int("DEFER_UMMA_FAST", 0);   // read per launch (launches are captured into graphs once; tests toggle it)
-  kp.tma_epi = (P.tma_epi && a.has_out_maps && !a.direct_out && P.splits == 1 && !P.cluster && !epi_direct) ? 1 : 0;
-  kp.res_stage_bytes = 0;
-  kp.flags = P.flags;
-  kp.scale = P.scale; kp.shift = P.shift;
-  kp.res = (P.flags & DEFER_FLAG_RESIDUAL) ? a.res : nullptr;
-  if (kp.tma_epi && kp.res) kp.res_stage_bytes = P.nplanes * (P.bn / 64) * BM * 128;
-  kp.y = a.y;
-  kp.partial = a.partial;
-  kp.counters = a.counters;
-  kp.plane_out = (size_t)P.n * P.ho * P.wo * P.cout;
-  kp.error_flag = nullptr;
-  kp.trace = a.trace;
-  kp.timeline = g_timeline;
-  kp.timeline_cap = g_timeline ? TIMELINE_CAP : 0;
-  kp.timeline_tag = (P.ho << 20) | (P.kh << 16) | (P.cout & 0xffff);
-  kp.pdl = 0;
-}
-
 int launch_conv_umma(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t st) {
-  KParams kp;
-  fill_kparams(P, a, &kp);
-  // measured at batch 1 / 16 lanes: 4 warps + 2 CTAs/SM 11.4k inf/s, 8 warps + 1 CTA/SM 10.5k
-  static const int ew = env_int("DEFER_UMMA_EPI_WARPS", 4);
-  if (ew != 8) {
-    if (P.nplanes == 2) return P.bn == 128 ? launch_t<2, 128, 4>(P, a, kp, st) : launch_t<2, 64, 4>(P, a, kp, st);
-    return P.bn == 128 ? launch_t<1, 128, 4>(P, a, kp, st) : launch_t<1, 64, 4>(P, a, kp, st);
-  }
-  if (P.nplanes == 2) return P.bn == 128 ? launch_t<2, 128, 8>(P, a, kp, st) : launch_t<2, 64, 8>(P, a, kp, st);
-  return P.bn == 128 ? launch_t<1, 128, 8>(P, a, kp, st) : launch_t<1, 64, 8>(P, a, kp, st);
+  if (P.nplanes == 2) return P.bn == 128 ? launch_op_t<2, 128>(P, a, st) : launch_op_t<2, 64>(P, a, st);
+  return P.bn == 128 ? launch_op_t<1, 128>(P, a, st) : launch_op_t<1, 64>(P, a, st);
 }
 
-// ---- megakernel host side
+// ---- persistent / megakernel host side
 size_t umma_mega_op_bytes() { return sizeof(MegaOp); }
 
 int umma_mega_fill(void* host_dst, const UmmaConvPlan& P, const UmmaConvLaneArgs& a) {
@@ -2497,197 +1008,44 @@ int umma_mega_fill(void* host_dst, const UmmaConvPlan& P, const UmmaConvLaneArgs
     return DEFER_ERR_STATE;
   }
   MegaOp op;
-  memset(&op, 0, sizeof op);
-  op.tmx[0] = a.tmap_x[0];
-  op.tmx[1] = a.tmap_x[1];
-  op.tmw[0] = P.tmap_w[0];
-  op.tmw[1] = P.tmap_w[1];
-  op.tmy[0] = a.tmap_y[0];
-  op.tmy[1] = a.tmap_y[1];
-  op.tmr[0] = a.tmap_r[0];
-  op.tmr[1] = a.tmap_r[1];
-  op.direct = (a.direct_out || !a.has_out_maps || env_int("DEFER_EPILOGUE_DIRECT", 0)) ? 1 : 0;
-  fill_kparams(P, a, &op.p);
-  op.m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
-  op.n_tiles = P.cout / P.bn;
+  fill_op(P, a, &op);
   memcpy(host_dst, &op, sizeof op);
   return DEFER_OK;
 }
 
+// 8 CTAs is the portable cluster size; up to 16 are allowed on H100 where a GPC has the SMs free
 int umma_mega_cluster_size() {
   static int cached = 0;
   if (cached) return cached;
-  int want = env_int("DEFER_MEGA_CLUSTER", 16);
+  int want = env_int("DEFER_MEGA_CLUSTER", 8);
   if (want < 1) want = 1;
   if (want > 16) want = 16;
   cached = want;
   return cached;
 }
 
-template <int NPLANES>
-static int launch_mega_t(const void* dev_ops, int n_ops, int stages, cudaStream_t st) {
-  using L = SmemLayout<NPLANES, MEGA_BN>;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  DEFER_CUDA(cudaGetDevice(&dev));
-  using MS = MegaSmem<NPLANES>;
-  if (stages < 1) stages = 1;
-  if (stages > MS::max_stages()) stages = MS::max_stages();
-  if (dev < 64 && !attr_set[dev]) {
-    DEFER_CUDA(cudaFuncSetAttribute(conv_mega_kernel<NPLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    MS::total(MS::max_stages())));
-    DEFER_CUDA(cudaFuncSetAttribute(conv_mega_kernel<NPLANES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    prefer_max_smem(conv_mega_kernel<NPLANES>);
-    attr_set[dev] = true;
-  }
-  const int cluster = umma_mega_cluster_size();
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof cfg);
-  cfg.gridDim = dim3(cluster, 1, 1);
-  cfg.blockDim = dim3(MEGA_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = MS::total(stages);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  const MegaOp* ops = reinterpret_cast<const MegaOp*>(dev_ops);
-  int* err = nullptr;
-  int use_cluster = 1;
-  DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_mega_kernel<NPLANES>, ops, n_ops, stages, use_cluster, err));
-  return DEFER_OK;
-}
-
-// ONE op on a persistent grid (many tiles: batched microbatches / large feature maps)
-template <int NPLANES>
-static int launch_persist_t(const void* dev_op, int n_tiles, cudaStream_t st) {
-  using L = SmemLayout<NPLANES, MEGA_BN>;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  DEFER_CUDA(cudaGetDevice(&dev));
-  using MS = MegaSmem<NPLANES>;
-  if (dev < 64 && !attr_set[dev]) {
-    DEFER_CUDA(cudaFuncSetAttribute(conv_mega_kernel<NPLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    MS::total(MS::max_stages())));
-    DEFER_CUDA(cudaFuncSetAttribute(conv_mega_kernel<NPLANES>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    prefer_max_smem(conv_mega_kernel<NPLANES>);
-    attr_set[dev] = true;
-  }
-  static int sms = 0;
-  if (!sms) DEFER_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  int stages = env_int("DEFER_PERSIST_STAGES", MS::max_stages());
-  if (stages > MS::max_stages()) stages = MS::max_stages();
-  if (stages < 1) stages = 1;
-  int per_sm = (227 * 1024) / MS::total(stages);
-  if (per_sm > 2) per_sm = 2;
-  if (per_sm < 1) per_sm = 1;
-  int grid = sms * per_sm;
-  if (grid > n_tiles) grid = n_tiles;
-  const MegaOp* ops = reinterpret_cast<const MegaOp*>(dev_op);
-  int* err = nullptr;
-  conv_mega_kernel<NPLANES><<<grid, MEGA_THREADS, MS::total(stages), st>>>(ops, 1, stages, 0, err);
-  DEFER_CUDA(cudaGetLastError());
-  return DEFER_OK;
-}
-
+// ONE op on a persistent grid (many tiles: batched microbatches / large feature maps), 64-wide N tiles
 int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st) {
-  return nplanes == 2 ? launch_persist_t<2>(dev_op, n_tiles, st) : launch_persist_t<1>(dev_op, n_tiles, st);
+  const int stages = env_int("DEFER_PERSIST_STAGES", MAX_STAGES);
+  return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 
-// ---- streaming persistent kernel: host side
-template <int NPLANES, int BN>
-static int launch_stream_t(const void* dev_op, int n_tiles, int k_blocks, cudaStream_t st) {
-  using SS = StreamSmem<NPLANES, BN>;
-  using L = SmemLayout<NPLANES, BN>;
-  constexpr int SMEM_CAP = 227 * 1024 - 256;      // opt-in limit per block (the kernel has no static shared memory)
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  DEFER_CUDA(cudaGetDevice(&dev));
-  if (dev < 64 && !attr_set[dev]) {
-    DEFER_CUDA(cudaFuncSetAttribute(conv_stream_kernel<NPLANES, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP));
-    prefer_max_smem(conv_stream_kernel<NPLANES, BN>);
-    attr_set[dev] = true;
-  }
-  static int sms = 0;
-  if (!sms) DEFER_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  // shared-memory split: K-heavy tiles want every byte in the operand ring (fill rate = bytes in flight / ~2 us),
-  // output-heavy tiles (a few k-blocks each) want several staging units so residual fetch, math and store overlap
-  const bool kheavy = k_blocks >= env_int("DEFER_STREAM_KHEAVY", 6);
-  // one k-block per tile (K = 64): the ring needs a single stage per tile in flight, everything else goes to staging
-  // units so 3-4 residual chunks are prefetched (measured: 34 -> 29 us on the 56x56 64->256 convs at batch 16)
-  int units = kheavy ? 1 : (k_blocks == 1 ? (BN == 64 ? 5 : 4) : env_int("DEFER_STREAM_LIGHT_UNITS", BN == 64 ? 4 : 3));
-  units = env_int("DEFER_STREAM_UNITS", units);
-  if (units < 1) units = 1;
-  if (units > STREAM_MAX_UNITS) units = STREAM_MAX_UNITS;
-  int stages = (SMEM_CAP - STREAM_CTL_BYTES - 1024 - units * SS::UNIT) / L::STAGE;
-  if (!kheavy) {
-    const int cap = env_int("DEFER_STREAM_LIGHT_STAGES", 0);
-    if (cap > 0 && stages > cap) stages = cap;
-  }
-  stages = env_int("DEFER_STREAM_STAGES", stages);
-  if (stages > 8) stages = 8;
-  while (stages > 1 && SS::total(stages, units) > SMEM_CAP) --stages;
-  if (stages < 1 || SS::total(stages, units) > SMEM_CAP) {
-    set_error("conv_stream: shared memory split failed (BN %d, %d units)", BN, units);
-    return DEFER_ERR_INVALID;
-  }
-  // Every CTA walks ceil(n_tiles / grid) tiles, so the launch lasts `rounds` tile-times whatever the grid is: take the
-  // SMALLEST grid that still finishes in the minimum number of rounds (448 tiles: 112 CTAs x 4 instead of 148 x 3.03)
-  // and leave the other SMs to the lanes running next to this one.
-  int grid = sms < n_tiles ? sms : n_tiles;
-  if (env_int("DEFER_STREAM_EVEN_GRID", 1)) {
-    const int rounds = (n_tiles + grid - 1) / grid;
-    grid = (n_tiles + rounds - 1) / rounds;
-  }
-  int* err = nullptr;
-  static const int pdl = env_int("DEFER_PDL", 0);
-  if (pdl) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3(grid, 1, 1);
-    cfg.blockDim = dim3(STREAM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = SS::total(stages, units);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_stream_kernel<NPLANES, BN>, reinterpret_cast<const MegaOp*>(dev_op), stages, units, 1, err));
-    return DEFER_OK;
-  }
-  conv_stream_kernel<NPLANES, BN><<<grid, STREAM_THREADS, SS::total(stages, units), st>>>(reinterpret_cast<const MegaOp*>(dev_op),
-                                                                                         stages, units, 0, err);
-  DEFER_CUDA(cudaGetLastError());
-  return DEFER_OK;
-}
-
+// ONE op on the streaming persistent grid: every byte of shared memory goes to the operand ring (the epilogue runs from
+// the accumulator registers), so the producer keeps the next tile's operands in flight during this tile's epilogue
 int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, cudaStream_t st) {
-  if (bn == 128) return nplanes == 2 ? launch_stream_t<2, 128>(dev_op, n_tiles, k_blocks, st) : launch_stream_t<1, 128>(dev_op, n_tiles, k_blocks, st);
-  if (bn == 64) return nplanes == 2 ? launch_stream_t<2, 64>(dev_op, n_tiles, k_blocks, st) : launch_stream_t<1, 64>(dev_op, n_tiles, k_blocks, st);
+  (void)k_blocks;
+  const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
+  if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 128>(dev_op, n_tiles, stages, st);
+  if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
   set_error("conv_stream: unsupported N tile %d", bn);
   return DEFER_ERR_INVALID;
 }
 
 // ---- fused stem: host side
-int umma_stem_in_bytes(int wo, int w, int cin, int kh, int sh) {
-  const int span = (BM + wo - 2) / wo;            // a 128-pixel tile touches at most span + 1 output rows
-  const int rows = span * sh + kh;
-  return ((rows * w * cin * 4) + 1023) / 1024 * 1024;
-}
-
 bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags) {
+  (void)n; (void)h; (void)w; (void)cin; (void)ho; (void)wo; (void)kh; (void)sh;
   if (fmt != FMT_BF16X2 && fmt != FMT_BF16) return false;
-  if (cout != 64 || (flags & DEFER_FLAG_RESIDUAL)) return false;
-  if (((long long)ho * wo) % BM != 0) return false;              // a tile never straddles two images
-  if ((w * cin * 4) % 16 != 0) return false;                      // bulk copies move whole 16-byte units
-  using SS2 = StemSmem<2>;
-  const int in_bytes = umma_stem_in_bytes(wo, w, cin, kh, sh);
-  (void)n; (void)h;
-  return SS2::total(2, in_bytes) <= 227 * 1024 - 256;
+  return cout == 64 && !(flags & DEFER_FLAG_RESIDUAL);
 }
 
 void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l) {
@@ -2697,66 +1055,15 @@ void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, in
   op->stem_kh = kh; op->stem_kw = kw; op->stem_sh = sh; op->stem_sw = sw;
   op->stem_pad_t = pad_t; op->stem_pad_l = pad_l;
   op->stem_K = kh * kw * cin;
-  if (getenv("DEFER_STEM_TRACE") && !g_stem_trace) {
-    if (cudaMalloc((void**)&g_stem_trace, 8 * 64 * sizeof(long long)) == cudaSuccess) cudaMemset(g_stem_trace, 0, 8 * 64 * sizeof(long long));
-    else g_stem_trace = nullptr;
-  }
-  if (g_stem_trace) op->p.trace = g_stem_trace;
 }
 
-template <int NPLANES>
-static int launch_stem_t(const void* dev_op, int n_tiles, int in_bytes, cudaStream_t st) {
-  using SS = StemSmem<NPLANES>;
-  using L = SmemLayout<NPLANES, 64>;
-  constexpr int SMEM_CAP = 227 * 1024 - 256;
-  static bool attr_set[64] = {false};
-  int dev = 0;
-  DEFER_CUDA(cudaGetDevice(&dev));
-  if (dev < 64 && !attr_set[dev]) {
-    DEFER_CUDA(cudaFuncSetAttribute(conv_stem_kernel<NPLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_CAP));
-    prefer_max_smem(conv_stem_kernel<NPLANES>);
-    attr_set[dev] = true;
-  }
-  static int sms = 0;
-  if (!sms) DEFER_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  int stages = (SMEM_CAP - STEM_CTL_BYTES - 1024 - 2 * SS::UNIT - 2 * in_bytes) / L::STAGE;
-  if (stages > 8) stages = 8;
-  if (stages < 2) {
-    set_error("conv_stem: shared memory split failed (%d input bytes)", in_bytes);
-    return DEFER_ERR_INVALID;
-  }
-  int grid = sms < n_tiles ? sms : n_tiles;
-  const int rounds = (n_tiles + grid - 1) / grid;
-  grid = (n_tiles + rounds - 1) / rounds;
-  int* err = nullptr;
-  static const int pdl = env_int("DEFER_PDL", 0);
-  if (pdl) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3(grid, 1, 1);
-    cfg.blockDim = dim3(STEM_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = SS::total(stages, in_bytes);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_stem_kernel<NPLANES>, reinterpret_cast<const MegaOp*>(dev_op), stages, in_bytes, 1, err));
-    return DEFER_OK;
-  }
-  conv_stem_kernel<NPLANES><<<grid, STEM_THREADS, SS::total(stages, in_bytes), st>>>(reinterpret_cast<const MegaOp*>(dev_op), stages,
-                                                                                   in_bytes, 0, err);
-  DEFER_CUDA(cudaGetLastError());
-  return DEFER_OK;
-}
-
-int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, int in_bytes, cudaStream_t st) {
-  return nplanes == 2 ? launch_stem_t<2>(dev_op, n_tiles, in_bytes, st) : launch_stem_t<1>(dev_op, n_tiles, in_bytes, st);
+int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st) {
+  const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
+  return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st) {
-  int stages = env_int("DEFER_MEGA_STAGES", 3);
+  int stages = env_int("DEFER_MEGA_STAGES", 4);
   return nplanes == 2 ? launch_mega_t<2>(dev_ops, n_ops, stages, st) : launch_mega_t<1>(dev_ops, n_ops, stages, st);
 }
 

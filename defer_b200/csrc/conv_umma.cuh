@@ -1,4 +1,4 @@
-// conv_umma.cuh - interface of the tcgen05 implicit-GEMM convolution (conv_umma.cu).
+// conv_umma.cuh - interface of the wgmma implicit-GEMM convolution (conv_umma.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -20,10 +20,8 @@ struct UmmaConvPlan {
   int k_blocks = 0;        // taps * cin / 64
   int splits = 1;          // split-K factor (grid.z)
   int cluster = 0;         // 1: the splits of a tile are one thread-block cluster, reduced through DSMEM
-  int tma_epi = 1;         // staged epilogue (TMA residual load + TMA store) wherever one CTA owns a whole tile
-  int stages = 4;          // smem ring depth (run-time: fewer stages -> more CTAs per SM)
+  int stages = 4;          // smem ring depth of the one-tile-per-CTA kernel (fewer stages -> more CTAs per SM)
   int stream = 0;          // 1: plan of the streaming persistent kernel (conv_stream_kernel), N tile = bn
-  size_t smem_bytes = 0;
   void* w_dev = nullptr;   // transformed weights
   const float* scale = nullptr;
   const float* shift = nullptr;
@@ -34,15 +32,11 @@ struct UmmaConvPlan {
 // Per-lane binding: tensor maps of the input activation planes + raw pointers for the epilogue.
 struct UmmaConvLaneArgs {
   CUtensorMap tmap_x[2];
-  CUtensorMap tmap_y[2];             // output tile boxes (TMA store epilogue), valid when has_out_maps
-  CUtensorMap tmap_r[2];             // residual tile boxes
-  bool has_out_maps = false;
-  bool direct_out = false;           // output lives in a peer GPU's slot: keep the per-thread st.global epilogue
+  bool direct_out = false;           // output lives in a peer GPU's slot (the epilogue's plain stores reach it)
   const void* res = nullptr;
   void* y = nullptr;
   float* partial = nullptr;          // split-K partial tiles (per lane: lanes run concurrently)
   unsigned int* counters = nullptr;  // split-K arrival counters, one per output tile
-  long long* trace = nullptr;        // debug: per-CTA phase stamps (see DEFER_UMMA_TRACE)
 };
 
 bool umma_conv_supported(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int kw, int sh, int sw,
@@ -54,21 +48,19 @@ int umma_conv_bind(const UmmaConvPlan& plan, UmmaConvLaneArgs* args, const void*
 void umma_conv_unbind(UmmaConvLaneArgs* args);
 int launch_conv_umma(const UmmaConvPlan& plan, const UmmaConvLaneArgs& args, cudaStream_t st);
 void umma_conv_release(UmmaConvPlan& plan);
-void umma_timeline_dump();   // DEFER_TIMELINE=<path>: write the per-CTA log collected so far
 
 // Stage megakernel: a run of consecutive convs in ONE cluster launch (conv_umma.cu, conv_mega_kernel).
 size_t umma_mega_op_bytes();
 int umma_mega_fill(void* host_dst, const UmmaConvPlan& plan, const UmmaConvLaneArgs& args);   // one op descriptor
 int umma_mega_cluster_size();
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st);
-// one op on the streaming persistent kernel (deep operand ring, in-place chunked epilogue): ops with many tiles
+// one op on the streaming persistent kernel (deep operand ring, epilogue from the accumulator registers)
 int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, cudaStream_t st);
-// fused stem (conv_stem_kernel): conv over a few-channel fp32 image with the im2col done inside the tcgen05 kernel
+// fused stem: conv over a few-channel fp32 image with the im2col done inside the persistent kernel
 bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags);
-int umma_stem_in_bytes(int wo, int w, int cin, int kh, int sh);
 void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l);
-int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, int in_bytes, cudaStream_t st);
-// one op on a persistent grid (same kernel, grid mode): for ops with many tiles
+int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st);
+// one op on a persistent grid (64-wide N tiles): for ops with many tiles
 int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st);
 
 }  // namespace defer

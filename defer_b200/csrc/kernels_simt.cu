@@ -1,10 +1,10 @@
-// kernels_simt.cu - SIMT kernels of the stage forward pass (sm_100a).
+// kernels_simt.cu - SIMT kernels of the stage forward pass (sm_90a).
 //
 // These are the non-contraction ops of the reference's `model.predict` (src/node.py:105-106):
 // max-pool, global-average-pool, dense (HBM-bound GEMV at batch 1), softmax, standalone
 // BN/ReLU/Add/ZeroPad for arbitrary cut points, format encode/decode, and the device-side flag
 // kernels of the hop.  It also holds the exact-fp32 FFMA implicit-GEMM convolution that (a) serves
-// shapes the tcgen05 kernel does not take (C_in = 3 stem) and (b) is the in-library cross-check of
+// shapes the wgmma kernel does not take (C_in = 3 stem) and (b) is the in-library cross-check of
 // the tensor-core path.
 #include <stdlib.h>
 
@@ -328,15 +328,14 @@ int launch_conv_simt(int fmt, bool x_is_f32, const ConvParams& p, cudaStream_t s
 // Tensor-core stem, step 1: im2col of the fp32 RGB image into the stage's activation format.
 // Row m = output pixel, column k = (kh * KW + kw) * C_in + ci  (the HWIO order of the shipped filter, so the
 // filter bank IS the [K, C_out] GEMM operand), zero for taps in the padding and for k >= K up to K_pad (a
-// multiple of 64).  The result feeds the tcgen05 conv kernel as a 1x1 convolution over K_pad channels.
+// multiple of 64).  The result feeds the wgmma conv kernel as a 1x1 convolution over K_pad channels.
 // One thread = 8 consecutive k of one pixel: a 16-byte store per bf16 plane.
 // =============================================================================================
 // One CTA = one output row of one image.  The kh input rows that row needs are staged in shared memory with coalesced
 // 16-byte loads (rows in the zero padding are stored as zeros); a patch is then kh runs of kw*cin CONTIGUOUS floats
 // (NHWC), so k -> (kernel row a, offset jj) and one range check on the flat column index covers the left / right
 // padding.  One work item = 8 consecutive k of one pixel = a 16-byte store per bf16 plane; consecutive items are
-// consecutive addresses, so the patch matrix is written fully coalesced.  (Round 1 gathered every element with a
-// scalar global load: 9 us per image; this version is bound by the patch-matrix write.)
+// consecutive addresses, so the patch matrix is written fully coalesced.
 template <int FMT>
 __global__ void __launch_bounds__(256) stem_im2col_kernel(const float* __restrict__ x, void* __restrict__ out, int n, int h,
                                                           int w, int cin, int kh, int kw, int sh, int sw, int pad_t,
@@ -620,9 +619,13 @@ int launch_gap(int fmt, const void* x, void* y, int n, int h, int w, int c, cuda
 constexpr int DENSE_TB = 128;     // units per block
 constexpr int DENSE_MAXB = 8;     // batch chunk held in registers
 
+// split counts aim at ~2 waves of the 132 SMs of an H100 SXM; a fixed number (not the device's) keeps the summation
+// order, and so the bits of the result, the same on every GPU
+constexpr int DENSE_WAVE_SMS = 132;
+
 int dense_splits(int n, int in_features, int units) {
   int col_blocks = (units + DENSE_TB - 1) / DENSE_TB;
-  int want = (2 * 148 + col_blocks - 1) / col_blocks;  // ~2 waves of 148 SMs
+  int want = (2 * DENSE_WAVE_SMS + col_blocks - 1) / col_blocks;
   int max_split = (in_features + 31) / 32;              // at least 32 rows per split
   int s = want < max_split ? want : max_split;
   int min_split = (in_features + 1023) / 1024;          // keep the x slice of a split small in smem
@@ -704,7 +707,7 @@ size_t dense_workspace_bytes(int n, int in_features, int units) {
 
 static int dense_fused_splits(int n, int F, int U) {
   const int col_blocks = (U + DF_COLS - 1) / DF_COLS;
-  int want = (2 * 148 + col_blocks - 1) / col_blocks;
+  int want = (2 * DENSE_WAVE_SMS + col_blocks - 1) / col_blocks;
   int max_split = F / 64;                   // >= 8 rows per warp
   if (max_split < 1) max_split = 1;
   int s = want < max_split ? want : max_split;

@@ -80,13 +80,12 @@ struct Buf {
 
 struct OpRt {
   defer_op_desc d;
-  int backend = 1;          // 1 SIMT, 2 tcgen05, 4 tensor-core stem (im2col of the fp32 image + tcgen05 1x1 conv)
+  int backend = 1;          // 1 SIMT, 2 wgmma, 4 tensor-core stem (im2col of the fp32 image + wgmma 1x1 conv)
   int k_pad = 0;            // backend 4: padded patch length (multiple of 64)
   void* w_pad = nullptr;    // backend 4: zero-padded [k_pad, cout] fp32 filter matrix
-  bool persist = false;     // tcgen05 conv with many tiles: persistent-grid launch (overlapped epilogue)
+  bool persist = false;     // wgmma conv with many tiles: persistent-grid launch (overlapped epilogue)
   bool stem_fused = false;  // backend 4 without a patch matrix: conv_stem_kernel builds the A operand from the fp32 image
-  int stem_in_bytes = 0;
-  bool stream = false;      // ... on the streaming kernel (conv_stream_kernel); false = round-1 conv_mega_kernel grid mode
+  bool stream = false;      // ... with the plan's N tile (64 | 128); false = the 64-wide persistent grid (DEFER_STREAM=0, launch_conv_persistent)
   int n_tiles64 = 0;
   UmmaConvPlan umma;        // valid when backend == 2
   std::string kname;
@@ -111,13 +110,12 @@ struct Lane {
 };
 
 // How a non-last stage's output reaches the next GPU's input slot (DEFER_HOP, read when the stage is created):
-//   HOP_COPY   (default) the last op writes a LOCAL buffer with its normal (TMA-store) epilogue; then the lane waits for the
+//   HOP_COPY   (default) the last op writes a LOCAL buffer; then the lane waits for the
 //              slot's free flag and a cudaMemcpyAsync (copy engine, captured in the lane graph) ships it over NVLink in
 //              full-line bursts - the north star's cudaMemcpyPeerAsync hop.  Compute never blocks on back-pressure and no
-//              SM spends time on 16-byte peer stores (measured round 2: the per-thread peer-store epilogue capped every
-//              multi-GPU pipeline at ~30 k inf/s, 51 MB per 16-image microbatch out of stage 0 at ~150 GB/s).
-//   HOP_TMA    the last op's TMA store targets the peer slot directly (tensor map encoded on the mapped peer address).
-//   HOP_DIRECT round-1 behaviour: per-thread st.global of the epilogue into the peer slot.
+//              SM spends time on small peer stores.
+//   HOP_TMA    the last op's epilogue stores into the peer slot directly (same stores as HOP_DIRECT on this kernel).
+//   HOP_DIRECT per-thread st.global of the epilogue into the peer slot.
 enum HopMode { HOP_COPY = 0, HOP_TMA = 1, HOP_DIRECT = 2 };
 
 struct Mark {                 // steady-state timing: an event recorded right behind one chosen microbatch
@@ -154,7 +152,7 @@ struct defer_stage_s {
   cudaEvent_t job_t0 = nullptr, job_t1 = nullptr;
   Mark marks[2];
   int hop = HOP_COPY;
-  // megakernel groups: runs of consecutive tcgen05 convs executed by one cluster launch per lane
+  // megakernel groups: runs of consecutive wgmma convs executed by one cluster launch per lane
   struct MegaGroup {
     int first = 0, last = 0;
     std::vector<void*> dev_ops;   // per lane: device array of op descriptors
@@ -194,8 +192,7 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
   switch (d.kind) {
     case DEFER_OP_CONV: {
       if (op.backend == 4 && op.stem_fused)
-        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w,
-                                op.stem_in_bytes, st);
+        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w, st);
       if (op.backend == 4)
         DEFER_TRY(launch_stem_im2col(fmt, (const float*)x, L.im2col[oi], nb, bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t,
                                      d.pad_l, bo.h, bo.w, op.k_pad, st));
@@ -370,14 +367,14 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
   DEFER_CHECK(cfg->input_buf >= 0 && cfg->input_buf < n_bufs && cfg->output_buf >= 0 && cfg->output_buf < n_bufs &&
                   cfg->input_buf != cfg->output_buf,
               "bad input/output buffer ids");
-  DEFER_CHECK(!(cfg->conv_backend == 2 && cfg->fmt == DEFER_FMT_F32), "tcgen05 conv backend needs BF16X2 or BF16 format");
+  DEFER_CHECK(!(cfg->conv_backend == 2 && cfg->fmt == DEFER_FMT_F32), "wgmma conv backend needs BF16X2 or BF16 format");
   int ndev = 0;
   DEFER_CUDA(cudaGetDeviceCount(&ndev));
   DEFER_CHECK(cfg->device >= 0 && cfg->device < ndev, "device %d not present (%d visible)", cfg->device, ndev);
   {
     cudaDeviceProp prop;
     DEFER_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-    DEFER_CHECK(prop.major == 10, "device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major,
+    DEFER_CHECK(prop.major == 9, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
                 prop.minor);
   }
 
@@ -487,10 +484,9 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         if (cfg->conv_backend == 1) can_umma = false;
         op.backend = can_umma ? 2 : 1;
         op.kname = can_umma ? "conv_umma_kernel" : "conv_simt_kernel";
-        // RGB stem (fp32 image in, few input channels): im2col to a K_pad-channel patch matrix, then the tcgen05 kernel
-        // as a 1x1 conv - the fp32 FFMA stem costs ~6 us of the WHOLE GPU per image, the tensor-core one < 1 us
-        // DEFER_TC_STEM: 0 off, 1 strided stems only (ResNet 7x7/2), 2 (default) every eligible first conv (VGG's 3x3/1 too:
-        // +4 % on VGG16, parity 2e-5)
+        // RGB stem (fp32 image in, few input channels): im2col to a K_pad-channel patch matrix, then the wgmma kernel
+        // as a 1x1 conv (the fp32 FFMA stem runs 147 MACs per output on the SIMT pipe; the tensor cores take them instead)
+        // DEFER_TC_STEM: 0 off, 1 strided stems only (ResNet 7x7/2), 2 (default) every eligible first conv (VGG's 3x3/1 too)
         static const int tc_stem = getenv("DEFER_TC_STEM") ? atoi(getenv("DEFER_TC_STEM")) : 2;
         const int K = d.kh * d.kw * bi.c;
         if (tc_stem && cfg->conv_backend != 1 && cfg->fmt != DEFER_FMT_F32 && bi.elem == DEFER_BUF_F32 && bi.c < 64 && K <= 256 &&
@@ -646,7 +642,6 @@ int defer_stage_destroy(defer_stage_t s) {
   if (!s) return DEFER_OK;
   cudaSetDevice(s->cfg.device);
   cudaDeviceSynchronize();
-  umma_timeline_dump();
   for (auto& L : s->lanes) {
     if (L.exec) cudaGraphExecDestroy(L.exec);
     if (L.graph) cudaGraphDestroy(L.graph);
@@ -699,7 +694,7 @@ int defer_stage_describe(defer_stage_t s, char* buf, size_t buf_len) {
     o += line;
     if ((op.backend == 2 || op.backend == 4) && op.umma.ready) {
       const UmmaConvPlan& u = op.umma;
-      snprintf(line, sizeof line, "       tcgen05 tiles: m=%d x n=%d (BN %d) x k-splits %d%s, %d k-blocks, ring %d -> %d CTAs\n",
+      snprintf(line, sizeof line, "       wgmma tiles: m=%d x n=%d (BN %d) x k-splits %d%s, %d k-blocks, ring %d -> %d CTAs\n",
                u.tiles_n * u.tiles_h * u.tiles_w, u.cout / u.bn, u.bn, u.splits, u.cluster ? " (cluster, DSMEM reduce)" : "",
                u.k_blocks, u.stages, u.tiles_n * u.tiles_h * u.tiles_w * (u.cout / u.bn) * u.splits);
       o += line;
@@ -843,7 +838,7 @@ int defer_stage_finalize(defer_stage_t s) {
   DEFER_CHECK(s->cfg.is_first || s->has_prod, "finalize: stage is not first and has no producer link");
   DEFER_CHECK(s->cfg.is_last || s->has_cons, "finalize: stage is not last and has no consumer link");
   DEFER_TRY(set_device(s));
-  // megakernel groups: maximal runs of consecutive tcgen05 convs (DEFER_MEGA=0 disables)
+  // megakernel groups: maximal runs of consecutive wgmma convs (DEFER_MEGA=0 disables)
   s->op_group.assign(s->ops.size(), -1);
   {
     const char* e = getenv("DEFER_MEGA");
@@ -863,7 +858,7 @@ int defer_stage_finalize(defer_stage_t s) {
       i = j + 1;
     }
   }
-  // tcgen05 conv plans need final buffer addresses (TMA tensor maps embed them)
+  // wgmma conv plans need final buffer addresses (TMA tensor maps embed them)
   for (int oi = 0; oi < (int)s->ops.size(); ++oi) {
     OpRt& op = s->ops[oi];
     if (op.backend != 2 && op.backend != 4) continue;
@@ -883,11 +878,11 @@ int defer_stage_finalize(defer_stage_t s) {
     // Executor choice.  Ops of a megakernel group keep the group's 64-wide tiles.  Otherwise an op with enough output
     // tiles runs on the streaming persistent kernel (deep operand ring, overlapped in-place epilogue); small ops keep
     // the one-tile-per-CTA kernel (BN = 128 where C_out allows, split-K below 4 CTAs).
-    //   DEFER_STREAM=0           -> round-1 persistent kernel (conv_mega_kernel in grid mode) instead
+    //   DEFER_STREAM=0           -> the persistent grid with 64-wide N tiles only (launch_conv_persistent) instead
     //   DEFER_STREAM_MIN_TILES   -> threshold in 128 x 64 tiles (default 96)
-    //   DEFER_STREAM_BN          -> force the N tile (64 | 128); default 128 whenever C_out % 128 == 0 (tcgen05.mma has a
-    //                               ~100-cycle floor per instruction: wide N tiles halve the instruction count and the
-    //                               SM-time per output; DEFER_STREAM_BN128_TILES = minimum tile count to allow it)
+    //   DEFER_STREAM_BN          -> force the N tile (64 | 128); default 128 whenever C_out % 128 == 0 (the A tile is
+    //                               fetched once per N tile: wide N tiles halve the activation traffic;
+    //                               DEFER_STREAM_BN128_TILES = minimum tile count to allow it)
     const int stream_on = getenv("DEFER_STREAM") ? atoi(getenv("DEFER_STREAM")) : 1;
     int stream_bn = 0;
     for (int attempt = 0; attempt < 2; ++attempt) {
@@ -932,7 +927,6 @@ int defer_stage_finalize(defer_stage_t s) {
       op.stem_fused = stem && fuse && op.stream && op.umma.bn == 64 && op.umma.flat && out_local &&
                       umma_stem_fusable(s->cfg.fmt, s->cfg.batch, bi.h, bi.w, bi.c, bo.h, bo.w, bo.c, d.kh, d.sh, d.flags);
       if (op.stem_fused) {
-        op.stem_in_bytes = umma_stem_in_bytes(bo.w, bi.w, bi.c, d.kh, d.sh);
         op.kname = "conv_stem_kernel";
         op.n_kernels = 1;
       }

@@ -1,4 +1,4 @@
-"""Graph partitioner with the reference's signatures (``/root/reference/src/dag_util.py:3-31``).
+"""Graph partitioner with the reference's signatures (``src/dag_util.py:3-31``).
 
 ``construct_model(model, start, end, part_name)`` returns the sub-model that computes every layer
 strictly after ``start`` through ``end``; its input *is* ``start``'s output tensor.  The walk is the

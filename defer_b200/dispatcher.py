@@ -1,10 +1,10 @@
-"""Dispatcher with the reference's API (``/root/reference/src/dispatcher.py:20-115``).
+"""Dispatcher with the reference's API (``src/dispatcher.py:20-115``).
 
 ``DEFER(computeNodes).run_defer(model, partition_layers, input_stream, output_stream)`` - same names,
 same arguments, same blocking behaviour (callers run it in a daemon thread, ``test/test.py:42``).
 What changed underneath:
 
-* ``computeNodes[i]`` is a GPU ordinal (or ``"cuda:i"``) of one 8xB200 box instead of an IP;
+* ``computeNodes[i]`` is a GPU ordinal (or ``"cuda:i"``) of one 8xH100 box instead of an IP;
 * ``_dispatchModels`` still ships ``to_json()`` + ``get_weights()`` per stage (``dispatcher.py:49,57``)
   but "shipping" is an upload into that GPU's HBM through ``defer_stage_create`` (same process) or a
   ``torch.distributed`` object send to the rank that owns the GPU (one process per GPU);

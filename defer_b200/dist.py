@@ -1,5 +1,5 @@
 """One-process-per-GPU plumbing (``torchrun``): the control plane that replaces the reference's TCP
-ports 5001/5002 and its per-node polling (``/root/reference/src/dispatcher.py:44-65``,
+ports 5001/5002 and its per-node polling (``src/dispatcher.py:44-65``,
 ``src/node.py:20-75``).
 
 * stage shipment (architecture JSON + weights + next hop) : ``torch.distributed`` object scatter (gloo);
@@ -34,8 +34,10 @@ class DistContext:
         self.out_elems = int(out_elems) * int(batch)
         self._runner = None
         self._owns_group = False
+        # a gloo-only world may have more ranks than the host has GPUs: those ranks stay on the CPU
+        self.cuda = torch.cuda.is_available() and self.local_rank < torch.cuda.device_count()
         if not dist.is_initialized():
-            use_cuda = torch.cuda.is_available()
+            use_cuda = self.cuda
             if backend is None:
                 backend = "cpu:gloo,cuda:nccl" if use_cuda else "gloo"
             if use_cuda:
@@ -66,7 +68,7 @@ class DistContext:
     # ------------------------------------------------------------------ collectives (control plane only)
     def barrier(self):
         if self.world > 1:
-            if self.torch.cuda.is_available():
+            if self.cuda:
                 self.dist.barrier(device_ids=[self.local_rank])
             else:
                 self.dist.barrier()
@@ -74,7 +76,7 @@ class DistContext:
     def max_over_ranks(self, value: float) -> float:
         if self.world == 1:
             return float(value)
-        dev = f"cuda:{self.local_rank}" if self.torch.cuda.is_available() else "cpu"
+        dev = f"cuda:{self.local_rank}" if self.cuda else "cpu"
         t = self.torch.tensor([float(value)], dtype=self.torch.float64, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return float(t.item())
@@ -82,7 +84,7 @@ class DistContext:
     def sum_over_ranks(self, value: float) -> float:
         if self.world == 1:
             return float(value)
-        dev = f"cuda:{self.local_rank}" if self.torch.cuda.is_available() else "cpu"
+        dev = f"cuda:{self.local_rank}" if self.cuda else "cpu"
         t = self.torch.tensor([float(value)], dtype=self.torch.float64, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.SUM)
         return float(t.item())

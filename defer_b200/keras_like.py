@@ -1,6 +1,6 @@
 """Keras-free layer-DAG IR exposing exactly the surface DEFER touches.
 
-The reference partitions a ``tf.keras.Model`` (``/root/reference/src/dag_util.py:3-31``,
+The reference partitions a ``tf.keras.Model`` (``src/dag_util.py:3-31``,
 ``src/dispatcher.py:27-42``) and ships ``to_json()`` + ``get_weights()`` to each node
 (``src/dispatcher.py:49,57``; rebuilt with ``model_from_json`` + ``set_weights`` at
 ``src/node.py:31,34``).  TensorFlow is not installable here, so this module is a small

@@ -1,11 +1,11 @@
 """Stage runtime: the per-GPU counterpart of the reference compute node
-(``/root/reference/src/node.py:19-127``).
+(``src/node.py:19-127``).
 
 ``StageRunner`` owns one stage handle of ``libdefer_b200.so``: it is what a reference node holds after
 ``model_from_json`` + ``set_weights`` + ``_make_predict_function`` (``src/node.py:31-38``), and its
 ``step`` is the body of the hot loop ``_data_client`` (``src/node.py:103-108``) - except that the
 whole recv -> predict -> send of one microbatch is a single asynchronous CUDA-graph launch:
-wait-input-flag -> fused sm_100a kernels -> copy-engine hop into the next GPU's input slot -> release flags.
+wait-input-flag -> fused sm_90a kernels -> copy-engine hop into the next GPU's input slot -> release flags.
 
 ``Node`` keeps the reference's class name and thread roles for the one-process-per-GPU deployment
 (``torchrun``): it receives its stage from the dispatcher (``_model_socket`` / ``_weights_socket``

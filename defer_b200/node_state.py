@@ -1,5 +1,5 @@
 """Shared per-node state - the interface of the reference's ``NodeState``
-(``/root/reference/src/node_state.py:6-41``) on a condition variable.
+(``src/node_state.py:6-41``) on a condition variable.
 
 Same constructor and the same four attributes (``chunk_size`` read-only; ``next_node``, ``model``,
 ``weights`` settable), including the reference's "empty string means not set yet" sentinel
@@ -74,9 +74,9 @@ class NodeState:
 
 
 # ------------------------------------------------------------------------------------------------------
-# Wire framing of the reference transport (``/root/reference/src/node_state.py:43-101``): an 8-byte
+# Wire framing of the reference transport (``src/node_state.py:43-101``): an 8-byte
 # big-endian length followed by the payload, written / read in slices of at most ``chunk_size`` bytes on
-# a non-blocking socket, waiting with ``select`` whenever the kernel buffer is full / empty.  The B200 hot
+# a non-blocking socket, waiting with ``select`` whenever the kernel buffer is full / empty.  The GPU hot
 # path never uses it (the hop is an NVLink store) - it exists so that host-side tooling can talk to
 # reference-style peers (SURVEY.md 8f, rank 2) and so the two names of the reference module resolve.
 # ------------------------------------------------------------------------------------------------------

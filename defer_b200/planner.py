@@ -1,7 +1,7 @@
 """Stage planner: a (sub-)model in wire format -> fused-op plan for ``defer_stage_create``.
 
 This is the host half of what ``model_from_json`` + ``_make_predict_function`` do on a reference node
-(``/root/reference/src/node.py:31-37``): turn the layer list into something executable.  Here the
+(``src/node.py:31-37``): turn the layer list into something executable.  Here the
 executable form is a short list of fused ops (``include/defer_b200.h``):
 
 * ``[ZeroPadding2D] -> Conv2D -> [BatchNormalization] -> [Add(other)] -> [relu]`` becomes ONE

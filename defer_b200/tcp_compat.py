@@ -1,7 +1,7 @@
 """Network-transport compatibility mode (SURVEY.md 8f, rank 2): the reference's TCP control and data plane, so that a
-B200 stage can sit in a chain with reference-style peers (edge devices, other boxes) instead of - or next to - the NVLink hop.
+H100 stage can sit in a chain with reference-style peers (edge devices, other boxes) instead of - or next to - the NVLink hop.
 
-What the reference does on the wire (``/root/reference/src/dispatcher.py:44-80``, ``src/node.py:20-108``), restated:
+What the reference does on the wire (``src/dispatcher.py:44-80``, ``src/node.py:20-108``), restated:
 
 * three TCP ports per node: 5000 activations, 5001 architecture + next hop, 5002 weights (``src/dispatcher.py:18``);
 * weights (``:5002``): an 8-byte big-endian array count, then one frame per array (``socket_send`` framing of
@@ -17,7 +17,7 @@ wheels import - wire-compatible with the reference) and ``RawCodec`` (a self-des
 raw bytes) for chains made of defer_b200 peers.  Either way the hop is lossless, like the NVLink copy.
 
 This module is host-side only and never on the GPU hot path; the compute of a ``TcpNode`` is whatever ``predict`` callable it
-is given (a ``StageRunner.predict`` on a B200, or any stand-in in tests).
+is given (a ``StageRunner.predict`` on an H100, or any stand-in in tests).
 """
 from __future__ import annotations
 
@@ -212,7 +212,7 @@ class TcpNode:
     """Node half: the reference's four threads (``src/node.py:110-124``) around a pluggable stage builder.
 
     ``build_stage(model_json, weights) -> predict`` is what replaces ``model_from_json`` + ``set_weights`` +
-    ``_make_predict_function`` (``src/node.py:31-37``); on a B200 it is
+    ``_make_predict_function`` (``src/node.py:31-37``); on an H100 it is
     ``lambda j, w: StageRunner.from_wire(j, w, device=0, ...).predict``.
     """
 

@@ -5,8 +5,8 @@
  *     out  = part.predict(inpt)                                (src/node.py:105-106)
  *     socket_send(lz4(zfp(out)), next_node)                    (src/node.py:107-108)
  * and the dispatcher feeds / drains the chain (src/dispatcher.py:85-105).  This library replaces
- * exactly that: a *stage* is a fused-op plan + weights resident in HBM on one B200; its forward
- * pass is hand-written sm_100a kernels captured in a CUDA graph per in-flight lane; the hop is a
+ * exactly that: a *stage* is a fused-op plan + weights resident in HBM on one H100; its forward
+ * pass is hand-written sm_90a kernels captured in a CUDA graph per in-flight lane; the hop is a
  * copy-engine transfer (or, optionally, the last kernel's own stores) of the stage output into the
  * next stage's input slot over NVLink (peer or CUDA-IPC mapped) followed by a release flag - no host
  * round trip, no codec (the reference codec is lossless, src/node.py:76-79, so a raw copy is
@@ -47,9 +47,9 @@ typedef enum defer_status {
 /* Activation storage format inside a stage and across hops. */
 typedef enum defer_fmt {
   DEFER_FMT_F32 = 0,     /* IEEE fp32, SIMT FFMA contractions (exact-order fp32)                       */
-  DEFER_FMT_BF16X2 = 1,  /* fp32 carried as two bf16 planes (hi + lo, 4 B/elem): tcgen05 bf16x3 MMAs,  */
+  DEFER_FMT_BF16X2 = 1,  /* fp32 carried as two bf16 planes (hi + lo, 4 B/elem): wgmma bf16x3 MMAs,    */
                          /* fp32 accumulate - ~2^-16 relative per layer, meets the 1e-3 fp32 parity bar */
-  DEFER_FMT_BF16 = 2     /* one bf16 plane, tcgen05 bf16 MMA, fp32 accumulate (the bf16 configs)       */
+  DEFER_FMT_BF16 = 2     /* one bf16 plane, wgmma bf16 MMA, fp32   accumulate (the bf16 configs)       */
 } defer_fmt;
 
 typedef enum defer_op_kind {
@@ -102,7 +102,7 @@ typedef struct defer_stage_config {
   int32_t output_buf;      /* buffer id of the stage output */
   int32_t is_first;        /* 1: input arrives from host via defer_stage_submit */
   int32_t is_last;         /* 1: output is read back by defer_stage_result */
-  int32_t conv_backend;    /* 0 auto, 1 SIMT only, 2 tcgen05 where eligible (error if fmt == F32) */
+  int32_t conv_backend;    /* 0 auto, 1 SIMT only, 2 wgmma where eligible (error if fmt == F32) */
   int32_t use_graph;       /* 1: capture each lane's chain into a CUDA graph (default), 0: eager launches */
   int32_t wait_timeout_ms; /* device-side flag wait budget; 0 = default (4000 ms) */
 } defer_stage_config;
@@ -205,11 +205,11 @@ DEFER_API int defer_host_unregister(void* ptr);
 
 /* ---- per-kernel entry points (raw device pointers, e.g. torch.Tensor.data_ptr(); NHWC) ------ */
 /* Each runs ONE kernel on `stream` (cudaStream_t as void*, NULL = default) so it can be parity-
- * tested and ncu-profiled alone.  Activation tensors are in `fmt`; planes of BF16X2 are
+ * tested and profiled alone.  Activation tensors are in `fmt`; planes of BF16X2 are
  * [hi | lo], lo at element offset n*h*w*c. Weights: fp32 HWIO + fp32 scale/shift (may be NULL). */
-/* backend: 1 SIMT FFMA | 2 tcgen05, one tile per CTA (conv_umma_kernel) | 3 round-1 persistent grid (conv_mega_kernel) |
+/* backend: 1 SIMT FFMA | 2 wgmma, one tile per CTA (conv_umma_kernel) | 3 persistent grid, 64-wide N tiles (conv_stream_kernel) |
  *          4 / 5 streaming persistent kernel (conv_stream_kernel) with 64- / 128-wide N tiles |
- *          6 / 7 the same with the per-thread (peer-memory capable) epilogue */
+ *          6 / 7 the same, planned for an output in a peer GPU's slot */
 DEFER_API int defer_k_conv(int fmt, int backend,
                  const void* x, int x_is_f32, const float* w_hwio, const float* scale, const float* shift,
                  const void* residual, void* y,

@@ -2,7 +2,7 @@
 
 PARITY UNPINNED WITH RESPECT TO THE REFERENCE ITSELF: ANRGUSC/DEFER cannot be executed in this image - its
 arithmetic lives in un-vendored, un-pinned third-party wheels (TensorFlow ~1.14 + keras_applications 1.0.8, zfpy,
-lz4; call sites ``/root/reference/src/node.py:31,34,106``, ``src/dispatcher.py:49,57``, ``test/test.py:14``) that are
+lz4; call sites ``src/node.py:31,34,106``, ``src/dispatcher.py:49,57``, ``test/test.py:14``) that are
 not installed and not installable offline, and none of its scripts compares a value (``test/test.py:34`` prints
 shapes).  This file therefore restates the *published* Keras layer semantics those call sites rely on.
 

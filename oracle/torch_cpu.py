@@ -2,7 +2,7 @@
 format built on ``torch.nn.functional`` (oneDNN/MKL, all host cores).
 
 Used (a) to cross-check ``oracle/keras_ref.py`` and (b) as the *timed* CPU stand-in for the
-reference's TensorFlow-CPU ``model.predict`` (``/root/reference/test/local_infer.py:16-23``,
+reference's TensorFlow-CPU ``model.predict`` (``test/local_infer.py:16-23``,
 ``src/node.py:105-106``) in ``bench.py``'s ``cpu_baseline`` and ``--impl reference`` legs:
 TensorFlow is not installable here, so the baseline is a port (``cpu_baseline.kind = "port"``).
 PARITY UNPINNED - see ``oracle/keras_ref.py``.  Never imported by the product.

@@ -1,4 +1,7 @@
-"""Per-kernel GPU parity through the C-ABI entry points (defer_k_*), torch tensors as containers only."""
+"""Per-kernel GPU parity through the C-ABI entry points (defer_k_*), torch tensors as containers only.
+
+Tests named `test_conv_tcgen05_*` keep the names they had when the tensor-core convolution targeted Blackwell; they
+exercise the sm_90a wgmma kernels (defer_k_conv backends 2-7) - there is no Blackwell path in this library."""
 import ctypes as C
 import os
 
@@ -286,21 +289,22 @@ def test_conv_tcgen05_cluster_matches_single_cta(torch_cuda, monkeypatch):
 
 
 @pytest.mark.parametrize("fmt_name", ["bf16x2", "bf16"])
-@pytest.mark.parametrize("mode", ["direct", "staged_res_bn64", "staged_bn64"])
+@pytest.mark.parametrize("mode", ["ring2", "ring_deep", "staged_bn64"])
 def test_conv_tcgen05_epilogue_variants(torch_cuda, fmt_name, mode, monkeypatch):
-    """The per-thread st.global epilogue (kept for peer-GPU outputs) and the staged TMA epilogue (default) with the
-    residual tile in 64- or 128-wide N tiles give the same answers - bitwise, the arithmetic is identical."""
+    """The one-tile-per-CTA kernel with the shallowest operand ring (two stages: every fill waits for the previous k-block), a deep ring and
+    64-wide N tiles gives the same answers as the default plan - bitwise, the K order per output is the same."""
     torch, lib = torch_cuda
+    monkeypatch.setenv("DEFER_UMMA_SPLITK", "0")       # split-K would change the summation order
     shapes = [(1, 56, 56, 64, 256, 1, 1, 0), (1, 28, 28, 128, 128, 3, 1, 1), (2, 14, 14, 256, 1024, 1, 1, 0),
               (1, 7, 7, 512, 2048, 1, 1, 0), (1, 56, 56, 256, 512, 1, 2, 0)]
     ref_y = []
     for i, shape in enumerate(shapes):
         _, y, _ = _conv_case(torch, lib, fmt_name, 2, *shape, relu=True, residual=(i != 1), seed=10 + i)
         ref_y.append(y)
-    if mode == "direct":
-        monkeypatch.setenv("DEFER_UMMA_TMA_EPI", "0")
-    elif mode == "staged_res_bn64":
-        monkeypatch.setenv("DEFER_UMMA_TE_RES_BN64", "1")
+    if mode == "ring2":
+        monkeypatch.setenv("DEFER_UMMA_STAGES", "2")
+    elif mode == "ring_deep":
+        monkeypatch.setenv("DEFER_UMMA_STAGES", "8")
     else:
         monkeypatch.setenv("DEFER_UMMA_BN", "64")
     for i, shape in enumerate(shapes):
@@ -311,7 +315,7 @@ def test_conv_tcgen05_epilogue_variants(torch_cuda, fmt_name, mode, monkeypatch)
 
 @pytest.mark.parametrize("fmt_name", ["bf16x2", "bf16"])
 def test_conv_persistent_grid_kernel(torch_cuda, fmt_name):
-    """backend 3: the persistent-grid kernel (TMA-store / TMA-residual epilogue, double-buffered TMEM)."""
+    """backend 3: the persistent grid with 64-wide N tiles (each CTA walks many tiles through one operand ring)."""
     torch, lib = torch_cuda
     for i, shape in enumerate([(8, 56, 56, 64, 256, 1, 1, 0), (4, 56, 56, 64, 64, 3, 1, 1), (8, 28, 28, 256, 512, 1, 2, 0),
                                (3, 14, 14, 256, 256, 3, 1, 1)]):
@@ -341,16 +345,18 @@ def test_stem_kernel_f32_input(torch_cuda):
         assert R.rel_err(y, ref) <= (5e-3 if fmt_name == "bf16" else 2e-5), fmt_name
 
 
-@pytest.mark.parametrize("fast", [1, 2, 3])
-def test_conv_tcgen05_fast_flags_bitwise(torch_cuda, fast, monkeypatch):
-    """DEFER_UMMA_FAST only moves loads / relaxes a wait: results must be bit-identical to the default kernel."""
+@pytest.mark.parametrize("backend", [3, 4, 5])
+def test_conv_persistent_executors_match_one_tile_per_cta(torch_cuda, backend, monkeypatch):
+    """The persistent grid (64- and 128-wide N tiles, each CTA walking many tiles through one operand ring) and the
+    one-tile-per-CTA grid compute every output with the same K order: results must be bit-identical."""
     torch, lib = torch_cuda
-    shapes = [(1, 56, 56, 64, 256, 1, 1, 0), (1, 14, 14, 256, 256, 3, 1, 1), (1, 7, 7, 2048, 512, 1, 1, 0)]
-    ref = [_conv_case(torch, lib, "bf16x2", 2, *sh, relu=True, residual=(i != 1), seed=20 + i)[1] for i, sh in enumerate(shapes)]
-    monkeypatch.setenv("DEFER_UMMA_FAST", str(fast))
+    monkeypatch.setenv("DEFER_UMMA_SPLITK", "0")
+    shapes = [(1, 56, 56, 64, 256, 1, 1, 0), (1, 14, 14, 256, 256, 3, 1, 1), (1, 7, 7, 2048, 512, 1, 1, 0),
+              (4, 28, 28, 128, 128, 3, 1, 1)]
     for i, sh in enumerate(shapes):
-        err, y, _ = _conv_case(torch, lib, "bf16x2", 2, *sh, relu=True, residual=(i != 1), seed=20 + i)
-        assert err <= TOL["bf16x2"] and np.array_equal(y, ref[i]), (fast, sh)
+        _, ref, _ = _conv_case(torch, lib, "bf16x2", 2, *sh, relu=True, residual=(i != 1), seed=20 + i)
+        err, y, _ = _conv_case(torch, lib, "bf16x2", backend, *sh, relu=True, residual=(i != 1), seed=20 + i)
+        assert err <= TOL["bf16x2"] and np.array_equal(y, ref), (backend, sh)
 
 
 @pytest.mark.parametrize("fmt_name", ["bf16x2", "bf16"])
@@ -415,16 +421,16 @@ def test_conv_stream_kernel(torch_cuda, fmt_name, shape):
             assert np.array_equal(outs[(backend, residual)], outs[(4, residual)]), (shape, backend, residual)
 
 
-@pytest.mark.parametrize("units,stages", [(1, 0), (2, 0), (3, 0), (4, 2), (2, 1)])
-def test_conv_stream_kernel_smem_splits(torch_cuda, units, stages, monkeypatch):
-    """Every (ring depth, staging units) split the host may pick must give the same bits."""
+@pytest.mark.parametrize("fmt_name,stages", [("bf16x2", 2), ("bf16x2", 3), ("bf16x2", 4), ("bf16", 2), ("bf16", 6),
+                                             ("bf16", 8)])
+def test_conv_stream_kernel_ring_depths(torch_cuda, fmt_name, stages, monkeypatch):
+    """Every operand-ring depth of the persistent kernel (the host clamps it to what fits in 227 KB) must give the same
+    bits, including rings shallower than a tile's K loop, where the producer refills stages mid-tile."""
     torch, lib = torch_cuda
     shapes = [(4, 56, 56, 64, 256, 1, 1, 0), (3, 14, 14, 256, 256, 3, 1, 1)]
-    ref = [_conv_case(torch, lib, "bf16x2", 5, *sh, relu=True, residual=True, seed=7 + j)[1] for j, sh in enumerate(shapes)]
-    monkeypatch.setenv("DEFER_STREAM_UNITS", str(units))
-    if stages:
-        monkeypatch.setenv("DEFER_STREAM_STAGES", str(stages))
+    ref = [_conv_case(torch, lib, fmt_name, 5, *sh, relu=True, residual=True, seed=7 + j)[1] for j, sh in enumerate(shapes)]
+    monkeypatch.setenv("DEFER_STREAM_STAGES", str(stages))
     for j, sh in enumerate(shapes):
         for backend in (4, 5):
-            err, y, _ = _conv_case(torch, lib, "bf16x2", backend, *sh, relu=True, residual=True, seed=7 + j)
-            assert err <= TOL["bf16x2"] and np.array_equal(y, ref[j]), (units, stages, sh, backend)
+            err, y, _ = _conv_case(torch, lib, fmt_name, backend, *sh, relu=True, residual=True, seed=7 + j)
+            assert err <= TOL[fmt_name] and np.array_equal(y, ref[j]), (stages, sh, backend)

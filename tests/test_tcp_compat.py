@@ -1,5 +1,5 @@
 """Network-transport compatibility mode (SURVEY.md 8f rank 2): the reference's TCP handshake and data plane
-(/root/reference/src/dispatcher.py:44-105, src/node.py:20-108) over real localhost sockets - weight count + framed
+(reference src/dispatcher.py:44-105, src/node.py:20-108) over real localhost sockets - weight count + framed
 arrays on the weights port, JSON + next hop + 0x06 ACK on the model port, framed activations node -> node ->
 dispatcher - with a 2-stage ResNet-style model whose stage compute is the CPU oracle (test infrastructure)."""
 import queue

@@ -1,5 +1,5 @@
 """The reference's TCP framing (src/node_state.py:43-101): 8-byte big-endian length + chunked payload on
-non-blocking sockets.  Host-side compatibility helper; not on the B200 hot path."""
+non-blocking sockets.  Host-side compatibility helper; not on the GPU hot path."""
 import socket
 import threading
 

@@ -1,6 +1,6 @@
-// fill_bench.cu - how fast can the SMs of a B200 pull L2-resident tiles into shared memory with TMA, and does
-// `.multicast::cluster` lift the chip-wide cap?  (Design input for the conv kernels: their K loops are bound by this
-// path, tools/fill_model.py.)
+// fill_bench.cu - how fast can the SMs of an H100 pull L2-resident tiles into shared memory with TMA, and does
+// `.multicast::cluster` lift the chip-wide cap?  (Design input for the conv kernels: their operand ring is fed by this
+// path.)
 //
 //   mode 0: unicast, every CTA streams DISTINCT 16 KB tiles
 //   mode 1: unicast, the C CTAs of a cluster request the SAME tile in the same round (does L2 merge the requests?)
@@ -8,7 +8,7 @@
 // Every CTA receives S tiles per round (S x 16 KB ring), then the cluster synchronises and the ring is reused.
 // Output: delivered GB/s = bytes landing in shared memory / time (CUDA events), per mode and cluster size.
 //
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fill_bench fill_bench.cu -lcuda
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fill_bench fill_bench.cu -lcuda
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -153,7 +153,7 @@ int main(int argc, char** argv) {
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
-  printf("# B200 TMA fill benchmark: %d SMs, working set %zu MB, %d rounds x %d tiles x 16 KB per CTA\n", sms, total_mb, rounds, STAGES);
+  printf("# TMA fill benchmark: %d SMs, working set %zu MB, %d rounds x %d tiles x 16 KB per CTA\n", sms, total_mb, rounds, STAGES);
   printf("# mode csize grid  time_ms  delivered_GBs  per_SM_GBs\n");
   const int modes[] = {0, 1, 2};
   const int csizes[] = {1, 2, 4, 8};
@@ -198,7 +198,7 @@ int main(int argc, char** argv) {
   }
   CK(cudaFuncSetAttribute(share_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   printf("# experiment 2: sharing groups (no clusters). group rot grid time_ms delivered_GBs per_SM_GBs\n");
-  const int groups[] = {1, 2, 4, 8, 16, 37, 148};
+  const int groups[] = {1, 2, 4, 8, 16, sms / 4, sms};   // up to every SM reading the same tiles
   for (int gi = 0; gi < 7; ++gi) {
     for (int rot = 0; rot < 2; ++rot) {
       const int g = groups[gi];

@@ -1,4 +1,4 @@
-"""Run one conv shape through defer_k_conv a few times (for ncu captures).
+"""Run one conv shape through defer_k_conv a few times (a driver for profilers and for debugging one shape).
 usage: run_one_conv.py fmt backend n h w cin cout k s pad [iters]"""
 import sys
 from pathlib import Path

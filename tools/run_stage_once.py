@@ -1,5 +1,6 @@
 """Run one coalesced microbatch of a model through a single stage twice; the second pass sits between
-cudaProfilerStart/Stop so `ncu --profile-from-start off` captures exactly one launch of every kernel of the step.
+cudaProfilerStart/Stop, so a profiler that honours that capture range records exactly one launch of every kernel of the
+step.
 usage: run_stage_once.py [model] [dtype] [batch] [cuts,comma,separated]   (cuts -> a pipeline on one GPU, exercising the
 standalone element-wise kernels and the hop)"""
 import sys
