@@ -418,13 +418,14 @@ int launch_stem_im2col(int fmt, const float* x, void* out, int n, int h, int w, 
   }
   const unsigned grid = (unsigned)((size_t)n * ho);
   auto go = [&](auto kernel) -> int {
-    static bool attr_set[64] = {false};
+    // the two instantiations have the same type, so this lambda (and its static) is shared: one flag per format
+    static bool attr_set[3][64] = {};
     int dev = 0;
     DEFER_CUDA(cudaGetDevice(&dev));
-    if (dev < 64 && !attr_set[dev]) {
+    if (dev < 64 && !attr_set[fmt][dev]) {
       DEFER_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
       prefer_max_smem(kernel);
-      attr_set[dev] = true;
+      attr_set[fmt][dev] = true;
     }
     kernel<<<grid, 256, smem, st>>>(x, out, n, h, w, cin, kh, kw, sh, sw, pad_t, pad_l, ho, wo, K, K_pad);
     DEFER_CUDA(cudaGetLastError());

@@ -487,7 +487,7 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         // RGB stem (fp32 image in, few input channels): im2col to a K_pad-channel patch matrix, then the wgmma kernel
         // as a 1x1 conv (the fp32 FFMA stem runs 147 MACs per output on the SIMT pipe; the tensor cores take them instead)
         // DEFER_TC_STEM: 0 off, 1 strided stems only (ResNet 7x7/2), 2 (default) every eligible first conv (VGG's 3x3/1 too)
-        static const int tc_stem = getenv("DEFER_TC_STEM") ? atoi(getenv("DEFER_TC_STEM")) : 2;
+        const int tc_stem = getenv("DEFER_TC_STEM") ? atoi(getenv("DEFER_TC_STEM")) : 2;
         const int K = d.kh * d.kw * bi.c;
         if (tc_stem && cfg->conv_backend != 1 && cfg->fmt != DEFER_FMT_F32 && bi.elem == DEFER_BUF_F32 && bi.c < 64 && K <= 256 &&
             bo.c % 64 == 0 && !(d.flags & DEFER_FLAG_RESIDUAL) && d.sh <= 2 && d.sw <= 2 &&
@@ -922,7 +922,7 @@ int defer_stage_finalize(defer_stage_t s) {
     if (op.persist) op.kname = std::string(stem ? "stem_im2col+" : "") + (op.stream ? "conv_stream_kernel" : "conv_mega_kernel(grid)");
     // fused stem: no patch matrix at all when the tile geometry allows it and the output stays on this GPU
     {
-      static const int fuse = getenv("DEFER_STEM_FUSED") ? atoi(getenv("DEFER_STEM_FUSED")) : 1;
+      const int fuse = getenv("DEFER_STEM_FUSED") ? atoi(getenv("DEFER_STEM_FUSED")) : 1;
       const bool out_local = s->hop == HOP_COPY || !((d.out == s->cfg.output_buf) && !s->cfg.is_last);
       op.stem_fused = stem && fuse && op.stream && op.umma.bn == 64 && op.umma.flat && out_local &&
                       umma_stem_fusable(s->cfg.fmt, s->cfg.batch, bi.h, bi.w, bi.c, bo.h, bo.w, bo.c, d.kh, d.sh, d.flags);

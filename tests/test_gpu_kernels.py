@@ -2,19 +2,13 @@
 
 Tests named `test_conv_tcgen05_*` keep the names they had when the tensor-core convolution targeted Blackwell; they
 exercise the sm_90a wgmma kernels (defer_k_conv backends 2-7) - there is no Blackwell path in this library."""
-import ctypes as C
-import os
-
 import numpy as np
 import pytest
 
+from conv_check import FMTS, TOL, _alloc_act, _conv_case, _decode, _encode, _ptr, _quantise, ConvCase, check_executors
 from defer_b200 import _cabi as A
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
-
-FMTS = {"f32": A.FMT_F32, "bf16x2": A.FMT_BF16X2, "bf16": A.FMT_BF16}
-# tolerance on max|y-ref|/max|ref| per format: exact-order fp32, bf16x3 split (~2^-16), plain bf16 storage
-TOL = {"f32": 2e-5, "bf16x2": 2e-4, "bf16": 2e-2}
 
 
 @pytest.fixture(scope="module")
@@ -23,83 +17,6 @@ def torch_cuda():
     import torch
     assert torch.cuda.is_available()
     return torch, lib
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def _encode(torch, lib, x_np, fmt):
-    x = torch.from_numpy(np.ascontiguousarray(x_np, np.float32)).cuda()
-    if fmt == A.FMT_F32:
-        return x
-    n = x.numel()
-    planes = 2 if fmt == A.FMT_BF16X2 else 1
-    y = torch.empty(planes * n, dtype=torch.bfloat16, device="cuda")
-    A.check(lib.defer_k_encode(fmt, _ptr(x), _ptr(y), n, None))
-    return y
-
-
-def _decode(torch, lib, y, fmt, shape):
-    if fmt == A.FMT_F32:
-        return y.cpu().numpy().reshape(shape)
-    n = int(np.prod(shape))
-    out = torch.empty(n, dtype=torch.float32, device="cuda")
-    A.check(lib.defer_k_decode(fmt, _ptr(y), _ptr(out), n, None))
-    return out.cpu().numpy().reshape(shape)
-
-
-def _alloc_act(torch, fmt, n_elems):
-    if fmt == A.FMT_F32:
-        return torch.zeros(n_elems, dtype=torch.float32, device="cuda")
-    return torch.zeros((2 if fmt == A.FMT_BF16X2 else 1) * n_elems, dtype=torch.bfloat16, device="cuda")
-
-
-def _quantise(x, fmt):
-    """What the stage format can represent (so the oracle sees the same inputs the kernel does)."""
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(x, np.float32))
-    if fmt == A.FMT_F32:
-        return x.astype(np.float32)
-    hi = t.to(torch.bfloat16)
-    if fmt == A.FMT_BF16:
-        return hi.float().numpy()
-    lo = (t - hi.float()).to(torch.bfloat16)
-    return (hi.float() + lo.float()).numpy()
-
-
-def _conv_case(torch, lib, fmt_name, backend, n, h, w, cin, cout, k, s, pad, relu, residual, seed=0):
-    from oracle import keras_ref as R
-    fmt = FMTS[fmt_name]
-    rng = np.random.default_rng(seed)
-    x = rng.standard_normal((n, h, w, cin), dtype=np.float32)
-    wk = rng.standard_normal((k, k, cin, cout), dtype=np.float32) * np.float32(np.sqrt(2.0 / (k * k * cin)))
-    scale = rng.uniform(0.5, 1.5, cout).astype(np.float32)
-    shift = (rng.standard_normal(cout) * 0.2).astype(np.float32)
-    ho = (h + 2 * pad - k) // s + 1
-    wo = (w + 2 * pad - k) // s + 1
-    res = rng.standard_normal((n, ho, wo, cout), dtype=np.float32) if residual else None
-    xq = _quantise(x, fmt)
-    wq = _quantise(wk, fmt) if backend >= 2 else wk
-    ref = R.conv2d(np.pad(xq.astype(np.float64), ((0, 0), (pad, pad), (pad, pad), (0, 0))), wq.astype(np.float64), None,
-                   (s, s), "valid")
-    ref = ref * scale.astype(np.float64) + shift.astype(np.float64)
-    if residual:
-        ref = ref + _quantise(res, fmt).astype(np.float64)
-    if relu:
-        ref = np.maximum(ref, 0)
-    xd = _encode(torch, lib, x, fmt)
-    rd = _encode(torch, lib, res, fmt) if residual else None
-    wd = torch.from_numpy(wk).cuda()
-    sd, fd = torch.from_numpy(scale).cuda(), torch.from_numpy(shift).cuda()
-    yd = _alloc_act(torch, fmt, n * ho * wo * cout)
-    flags = (A.FLAG_RELU if relu else 0)
-    A.check(lib.defer_k_conv(fmt, backend, _ptr(xd), 0, _ptr(wd), _ptr(sd), _ptr(fd), _ptr(rd), _ptr(yd),
-                             n, h, w, cin, cout, k, k, s, s, pad, pad, pad, pad, flags, None))
-    torch.cuda.synchronize()
-    y = _decode(torch, lib, yd, fmt, (n, ho, wo, cout))
-    err = R.rel_err(y, ref)
-    return err, y, ref
 
 
 # the distinct conv shapes of ResNet50 at batch 1 (SURVEY.md 8d) + batch / edge variants
@@ -112,6 +29,13 @@ RESNET_SHAPES = [
     (1, 14, 14, 1024, 256, 1, 1, 0), (1, 14, 14, 1024, 512, 1, 2, 0), (1, 7, 7, 512, 512, 3, 1, 1),
     (1, 7, 7, 512, 2048, 1, 1, 0), (1, 7, 7, 2048, 512, 1, 1, 0), (1, 14, 14, 1024, 2048, 1, 2, 0),
     (3, 7, 7, 512, 512, 3, 1, 1), (2, 28, 28, 128, 128, 3, 1, 1), (5, 14, 14, 256, 256, 3, 1, 1),
+    # tile geometry outside ResNet50 (umma_conv_prepare): VGG-wide rows (wo > 128: two 112-wide parts), a ragged
+    # tile_w (131 = 66 + 65), odd input at stride 2, 5x5 and 7x7 over 64 channels, tile_n = 2 with a ragged batch,
+    # a 2x2 map with odd channel-block counts (3 in, 5 out), a 1x1 map, padding larger than k - 1, 288 k-blocks
+    (1, 224, 224, 64, 64, 3, 1, 1), (1, 130, 131, 64, 128, 3, 1, 1), (3, 57, 57, 64, 128, 3, 2, 1),
+    (1, 28, 28, 64, 64, 5, 1, 2), (1, 14, 14, 64, 64, 7, 1, 3), (5, 7, 7, 512, 512, 3, 1, 1),
+    (4, 2, 2, 192, 320, 3, 1, 1), (1, 1, 1, 64, 64, 1, 1, 0), (2, 9, 9, 64, 64, 3, 1, 3),
+    (1, 14, 14, 2048, 512, 3, 1, 1),
 ]
 
 
@@ -125,12 +49,14 @@ def test_conv_simt_shapes(torch_cuda, fmt_name):
 
 @pytest.mark.parametrize("fmt_name", ["bf16x2", "bf16"])
 @pytest.mark.parametrize("shape", RESNET_SHAPES, ids=lambda s: "x".join(map(str, s)))
-def test_conv_tcgen05_shapes(torch_cuda, fmt_name, shape):
+def test_conv_tcgen05_shapes(torch_cuda, fmt_name, shape, monkeypatch):
+    """Every wgmma executor against the oracle (global and per-channel error), bit-identical to each other."""
     torch, lib = torch_cuda
     n, h, w, cin, cout, k, s, pad = shape
     i = RESNET_SHAPES.index(shape)
-    err, y, ref = _conv_case(torch, lib, fmt_name, 2, n, h, w, cin, cout, k, s, pad, relu=(i % 2 == 0), residual=(i % 3 == 0), seed=i)
-    assert err <= TOL[fmt_name], (fmt_name, shape, err)
+    case = ConvCase(fmt_name, (n, h, w, cin, cout, k, k, s, s, pad, pad, pad, pad), relu=(i % 2 == 0), residual=(i % 3 == 0),
+                    seed=i)
+    check_executors(torch, lib, case, monkeypatch)
 
 
 def test_conv_tcgen05_vs_simt_same_inputs(torch_cuda):
