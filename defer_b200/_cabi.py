@@ -17,14 +17,15 @@ LINK_TOKEN_BYTES = 256
 
 # enums (include/defer_b200.h)
 FMT_F32, FMT_BF16X2, FMT_BF16 = 0, 1, 2
-OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY = range(1, 11)
+OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS = range(1, 12)
 FLAG_RELU, FLAG_RESIDUAL = 1, 2
-BUF_ACT, BUF_F32 = 0, 1
+BUF_ACT, BUF_F32, BUF_U8 = 0, 1, 2
 OK, ERR_INVALID, ERR_CUDA, ERR_TIMEOUT, ERR_STATE = 0, -1, -2, -3, -4
 
 FMT_NAMES = {FMT_F32: "f32", FMT_BF16X2: "bf16x2", FMT_BF16: "bf16"}
 OP_NAMES = {OP_CONV: "conv", OP_MAXPOOL: "maxpool", OP_GAP: "gap", OP_DENSE: "dense", OP_SOFTMAX: "softmax",
-            OP_AFFINE: "affine", OP_RELU: "relu", OP_ADD: "add", OP_PAD: "pad", OP_COPY: "copy"}
+            OP_AFFINE: "affine", OP_RELU: "relu", OP_ADD: "add", OP_PAD: "pad", OP_COPY: "copy",
+            OP_PREPROCESS: "preprocess"}
 
 
 class BufDesc(C.Structure):
@@ -94,6 +95,7 @@ PROTOTYPES = {
     "defer_k_eltwise": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, C.c_uint32, _vp]),
     "defer_k_encode": (_i, [_i, _vp, _vp, _u64, _vp]),
     "defer_k_decode": (_i, [_i, _vp, _vp, _u64, _vp]),
+    "defer_k_preprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
 }
 
 _LIB = None

@@ -92,6 +92,44 @@ def synthetic_input(batch: int = 1, shape=(224, 224, 3), seed: int = 0) -> np.nd
     return rng.standard_normal((batch,) + tuple(shape), dtype=np.float32)
 
 
+def synthetic_image(batch: int = 1, shape=(224, 224, 3), seed: int = 0) -> np.ndarray:
+    """Seeded stand-in for ``img_to_array(load_img(...)).astype(np.uint8)``: uniform uint8 RGB, 0..255."""
+    rng = np.random.default_rng(seed)
+    return rng.integers(0, 256, (batch,) + tuple(shape), dtype=np.uint8)
+
+
+#: ImageNet channel means of Keras' caffe mode, in BGR order (keras_applications.imagenet_utils)
+CAFFE_MEAN_BGR = (103.939, 116.779, 123.68)
+PREPROCESS_MODES = ("caffe",)
+
+
+def preprocess_input(x: np.ndarray, mode: str = "caffe") -> np.ndarray:
+    """Keras ``preprocess_input`` of ResNet50 / ResNet101 / ResNet152 / VGG16 (caffe mode), channels-last, as the
+    reference applies it before queueing an image (``test/test.py:23``).
+
+    Restates ``keras_applications.imagenet_utils._preprocess_numpy_input``: non-float input becomes float32, the channel
+    axis is reversed (RGB -> BGR) and the ImageNet mean is subtracted per channel in float32.  Returns a new float32
+    array; ``x`` is not modified.  ``DEFER(..., preprocess="caffe")`` applies the same transform on the GPU.
+    """
+    check_preprocess(mode)
+    x = np.asarray(x)
+    if x.shape[-1] != 3:
+        raise ValueError(f"preprocess_input: expected channels-last RGB (last axis 3), got shape {x.shape}")
+    y = x[..., ::-1].astype(np.float32)          # astype copies: the caller's array is never touched
+    y -= np.asarray(CAFFE_MEAN_BGR, np.float32)
+    return y
+
+
+def caffe_shift() -> np.ndarray:
+    """The per-channel shift the device applies after the channel flip: ``-float32(mean)``, BGR order."""
+    return -np.asarray(CAFFE_MEAN_BGR, np.float32)
+
+
+def check_preprocess(mode) -> None:
+    if mode not in PREPROCESS_MODES:
+        raise ValueError(f"preprocess={mode!r}: the supported mode is 'caffe' (Keras' preprocess_input of ResNet and VGG)")
+
+
 def _finish(model: Model, weights: Optional[str], seed: int) -> Model:
     if weights in ("synthetic", "imagenet"):
         # 'imagenet' is accepted for script compatibility (test/test.py:14) but cannot be

@@ -107,4 +107,11 @@ int defer_k_decode(int fmt, const void* x_act, float* y_f32, uint64_t n_elems, v
   return launch_decode(fmt, x_act, y_f32, n_elems, (cudaStream_t)stream);
 }
 
+int defer_k_preprocess(const uint8_t* x, const float* shift, float* y, int n, int h, int w, int c, void* stream) {
+  DEFER_CHECK(x && shift && y, "k_preprocess: null pointer");
+  DEFER_CHECK(n >= 1 && h >= 1 && w >= 1, "k_preprocess: empty image (%d,%d,%d)", n, h, w);
+  DEFER_CHECK(c == 3, "k_preprocess: caffe preprocessing needs 3 channels (RGB), got %d", c);
+  return launch_preprocess(x, shift, y, (size_t)n * h * w, (cudaStream_t)stream);
+}
+
 }  // extern "C"

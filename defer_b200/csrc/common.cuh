@@ -174,6 +174,8 @@ int launch_encode(int fmt, const float* x, void* y, size_t n_elems, cudaStream_t
 int launch_decode(int fmt, const void* x, float* y, size_t n_elems, cudaStream_t st);
 int launch_copy_act(int fmt, const void* x, void* y, size_t n_elems, cudaStream_t st);
 int launch_f32_to_bf16(const float* x, void* y, size_t n, cudaStream_t st);
+// Keras caffe preprocess_input: uint8 RGB (n_pix pixels x 3) -> fp32 BGR + shift (DEFER_OP_PREPROCESS)
+int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_pix, cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

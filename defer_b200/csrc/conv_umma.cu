@@ -27,6 +27,8 @@
 #include <cuda.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include <vector>
 
 #include "common.cuh"
@@ -80,6 +82,10 @@ struct alignas(128) MegaOp {
   // fused stem: the fp32 NHWC image the patch rows are built from, and the real conv geometry
   const float* stem_x;
   int stem_h, stem_w, stem_cin, stem_kh, stem_kw, stem_sh, stem_sw, stem_pad_t, stem_pad_l, stem_K;
+  // fused stem over a uint8 RGB image instead (conv_stem_u8_kernel): Keras caffe preprocessing on the fly,
+  // value[c] = float(image[2 - c]) + stem_shift[c]
+  const uint8_t* stem_u8;
+  float stem_shift[3];
 };
 
 template <int NPLANES, int BN>
@@ -299,32 +305,69 @@ __device__ __forceinline__ void epi_pair(const KParams& p, size_t pix, int c, fl
 // Fused RGB stem: the producer warpgroup writes one k-block of the A operand (128 patch rows x 64 k, bf16 hi / lo
 // planes) in the SWIZZLE_128B layout TMA would have produced.  In NHWC a patch is kh runs of kw*cin contiguous floats,
 // so k -> (kernel row a, offset jj) and one range check on the flat column index covers the left / right padding.
-template <int NPLANES>
+// U8: the image is uint8 RGB (cin == 3, checked by the stage) and each tap is preprocessed as it is read: channel c
+// <- image channel 2 - c, plus stem_shift[c].  The padding belongs to the preprocessed tensor, so an out-of-range tap
+// stays 0.  All eight byte loads of a chunk are issued before any of them is converted (a load whose conversion sits
+// next to it in a branch would wait out its latency before the next load issues), and as a run is whole pixels, tap k
+// has channel k % 3: the eight taps of a chunk see a rotation of (0, 1, 2), so the mirrored-channel offset and the shift
+// are chosen once per chunk.  float(byte) is exact via the 2^23 magic number, then one rounded add: the same value the
+// standalone preprocess_kernel writes.
+template <int NPLANES, bool U8>
 __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int m0, int kb, int r) {
+  using In = std::conditional_t<U8, uint8_t, float>;
   const KParams& p = op.p;
   const int m = m0 + r;
   const int run = op.stem_kw * op.stem_cin, wc = op.stem_w * op.stem_cin;
-  const float* img = nullptr;
+  const In* img = nullptr;
   int ih0 = 0, col0 = 0;
   if (m < p.m_total) {
     const int hw = p.ho * p.wo;
     const int im = m / hw, rem = m - im * hw, oh = rem / p.wo, ow = rem - oh * p.wo;
-    img = op.stem_x + (size_t)im * op.stem_h * wc;
+    if constexpr (U8) img = op.stem_u8 + (size_t)im * op.stem_h * wc;
+    else img = op.stem_x + (size_t)im * op.stem_h * wc;
     ih0 = oh * op.stem_sh - op.stem_pad_t;
     col0 = (ow * op.stem_sw - op.stem_pad_l) * op.stem_cin;
   }
   int k = kb * BK;
   int a = k / run, jj = k - a * run;
+  int c0 = 0, K = 0, H = 0;         // U8: channel of the chunk's first tap; stem_K and stem_h kept in registers
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  if constexpr (U8) {
+    c0 = k % 3;
+    K = op.stem_K;
+    H = op.stem_h;
+    s0 = op.stem_shift[0]; s1 = op.stem_shift[1]; s2 = op.stem_shift[2];
+  }
 #pragma unroll 1
   for (int ch = 0; ch < 8; ++ch) {
     float v[8];
+    if constexpr (U8) {
+      const float sr[3] = {c0 == 0 ? s0 : (c0 == 1 ? s1 : s2), c0 == 0 ? s1 : (c0 == 1 ? s2 : s0),
+                           c0 == 0 ? s2 : (c0 == 1 ? s0 : s1)};
+      const int mr[3] = {2 - 2 * c0, c0 == 2 ? 2 : -2 * c0, c0 == 0 ? -2 : 4 - 2 * c0};   // 2 - 2 * ((c0 + i) % 3)
+      uint32_t raw[8];
+      bool in[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int ih = ih0 + a, col = col0 + jj;
-      v[e] = (img && k < op.stem_K && ih >= 0 && ih < op.stem_h && col >= 0 && col < wc) ? __ldg(img + (size_t)ih * wc + col)
-                                                                                        : 0.f;
-      ++k;
-      if (++jj == run) { jj = 0; ++a; }
+      for (int e = 0; e < 8; ++e) {
+        const int ih = ih0 + a, col = col0 + jj;
+        in[e] = img && k < K && ih >= 0 && ih < H && col >= 0 && col < wc;
+        raw[e] = in[e] ? (uint32_t)__ldg(img + (size_t)ih * wc + col + mr[e % 3]) : 0u;
+        ++k;
+        if (++jj == run) { jj = 0; ++a; }
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        v[e] = in[e] ? __fadd_rn(__fsub_rn(__uint_as_float(0x4B000000u | raw[e]), 8388608.f), sr[e % 3]) : 0.f;
+      c0 = c0 == 0 ? 2 : c0 - 1;    // (c0 + 8) % 3
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int ih = ih0 + a, col = col0 + jj;
+        v[e] = (img && k < op.stem_K && ih >= 0 && ih < op.stem_h && col >= 0 && col < wc) ? __ldg(img + (size_t)ih * wc + col)
+                                                                                          : 0.f;
+        ++k;
+        if (++jj == run) { jj = 0; ++a; }
+      }
     }
     const uint32_t off = (uint32_t)r * 128u + ((uint32_t)(ch ^ (r & 7)) << 4);
     uint32_t h[4], l[4];
@@ -346,7 +389,7 @@ __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int
 // MODE 0: one (tile, split) per CTA: tile = (blockIdx.x, blockIdx.y), split = blockIdx.z (grid split-K or cluster split-K)
 // MODE 1: persistent grid: CTA b walks tiles b, b + gridDim.x, ... of one op
 // MODE 2: one cluster walks a run of ops; tiles are dealt round-robin to its CTAs, a cluster barrier separates ops
-template <int NPLANES, int BN, int MODE>
+template <int NPLANES, int BN, int MODE, bool U8 = false>
 __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stages, int pdl) {
   using L = Smem<NPLANES, BN>;
   constexpr int R = BN / 2;   // accumulator registers per consumer thread
@@ -394,7 +437,7 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
     const int split = MODE == 0 ? (int)blockIdx.z : 0;
     const int kb_begin = (split * p.k_blocks) / p.splits;   // balanced ranges; host guarantees k_blocks >= splits
     const int kb_end = ((split + 1) * p.k_blocks) / p.splits;
-    const bool stem = op.stem_x != nullptr;
+    const bool stem = U8 || op.stem_x != nullptr;
 
     for (int t = t_first; t < total; t += t_step) {
       const int m_tile = t % op.m_tiles;
@@ -430,7 +473,7 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
                 tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
                 if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
               }
-              stem_build<NPLANES>(op, a_dst, w0, kb, ptid);
+              stem_build<NPLANES, U8>(op, a_dst, w0, kb, ptid);
               asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
               prod_bar_sync();
               if (ptid == 0) mbar_arrive(full_bar(stage));
@@ -601,6 +644,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_kernel(const MegaO
   conv_body<NPLANES, BN, 1>(ops, 1, stages, pdl);
 }
 
+// the fused stem reading a uint8 RGB image (Keras caffe preprocessing applied while the patch rows are built)
+template <int NPLANES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  conv_body<NPLANES, 64, 1, true>(ops, 1, stages, pdl);
+}
+
 template <int NPLANES>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_mega_kernel(const MegaOp* __restrict__ ops, int n_ops, int stages) {
   conv_body<NPLANES, MEGA_BN, 2>(ops, n_ops, stages, 0);
@@ -754,10 +803,12 @@ int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t s
 // persistent grid over the tiles of one op in device memory: every CTA walks ceil(n_tiles / grid) tiles, so the launch
 // lasts `rounds` tile-times whatever the grid is; take the SMALLEST grid that still finishes in the minimum number of
 // rounds and leave the other SMs to the lanes running next to this one
-template <int NPLANES, int BN>
+template <int NPLANES, int BN, bool U8 = false>
 int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
   using L = Smem<NPLANES, BN>;
-  DEFER_TRY((set_smem_attr<conv_stream_kernel<NPLANES, BN>>()));
+  static_assert(!U8 || BN == 64, "the uint8 stem runs with 64-wide N tiles");
+  constexpr auto kernel = U8 ? &conv_stem_u8_kernel<NPLANES> : &conv_stream_kernel<NPLANES, BN>;
+  DEFER_TRY((set_smem_attr<kernel>()));
   if (stages > L::max_stages()) stages = L::max_stages();
   if (stages < 2) stages = 2;
   const int sms = sm_count();
@@ -778,10 +829,10 @@ int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t s
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_stream_kernel<NPLANES, BN>, reinterpret_cast<const MegaOp*>(dev_op), stages, 1));
+    DEFER_CUDA(cudaLaunchKernelEx(&cfg, kernel, reinterpret_cast<const MegaOp*>(dev_op), stages, 1));
     return DEFER_OK;
   }
-  conv_stream_kernel<NPLANES, BN><<<grid, NUM_THREADS, smem, st>>>(reinterpret_cast<const MegaOp*>(dev_op), stages, 0);
+  kernel<<<grid, NUM_THREADS, smem, st>>>(reinterpret_cast<const MegaOp*>(dev_op), stages, 0);
   DEFER_CUDA(cudaGetLastError());
   return DEFER_OK;
 }
@@ -1057,8 +1108,18 @@ void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, in
   op->stem_K = kh * kw * cin;
 }
 
-int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st) {
+void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]) {
+  MegaOp* op = reinterpret_cast<MegaOp*>(host_op);
+  op->stem_x = nullptr;
+  op->stem_u8 = x;
+  for (int c = 0; c < 3; ++c) op->stem_shift[c] = shift[c];
+}
+
+int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, cudaStream_t st) {
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
+  if (u8)
+    return nplanes == 2 ? launch_persist_t<2, 64, true>(dev_op, n_tiles, stages, st)
+                        : launch_persist_t<1, 64, true>(dev_op, n_tiles, stages, st);
   return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 

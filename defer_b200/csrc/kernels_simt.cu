@@ -1116,6 +1116,59 @@ int launch_copy_act(int fmt, const void* x, void* y, size_t n, cudaStream_t st) 
   return DEFER_OK;
 }
 
+// Keras caffe-mode preprocess_input on a uint8 RGB image: y[p, c] = float(x[p, 2 - c]) + shift[c], one exactly rounded
+// fp32 add per element (shift = -mean, so this is the host's float32(x) - mean bit for bit).  VEC: a thread reads four
+// pixels as three 32-bit words and writes them as three float4; the last n_pix % 4 pixels go one per thread.
+template <bool VEC>
+__global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restrict__ x, const float* __restrict__ shift,
+                                                         float* __restrict__ y, size_t n_pix) {
+  const float s0 = __ldg(shift), s1 = __ldg(shift + 1), s2 = __ldg(shift + 2);
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (VEC) {
+    const size_t groups = n_pix / 4;
+    if (i < groups) {
+      const uint32_t* xv = reinterpret_cast<const uint32_t*>(x) + 3 * i;
+      const uint32_t wd[3] = {__ldg(xv), __ldg(xv + 1), __ldg(xv + 2)};
+      float b[12], o[12];
+#pragma unroll
+      for (int j = 0; j < 12; ++j) b[j] = (float)((wd[j >> 2] >> (8 * (j & 3))) & 0xffu);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        o[3 * q] = __fadd_rn(b[3 * q + 2], s0);
+        o[3 * q + 1] = __fadd_rn(b[3 * q + 1], s1);
+        o[3 * q + 2] = __fadd_rn(b[3 * q], s2);
+      }
+      float4* yv = reinterpret_cast<float4*>(y) + 3 * i;
+      yv[0] = make_float4(o[0], o[1], o[2], o[3]);
+      yv[1] = make_float4(o[4], o[5], o[6], o[7]);
+      yv[2] = make_float4(o[8], o[9], o[10], o[11]);
+      return;
+    }
+    i = groups * 4 + (i - groups);
+  }
+  if (i >= n_pix) return;
+  const uint8_t* px = x + 3 * i;
+  float* py = y + 3 * i;
+  py[0] = __fadd_rn((float)px[2], s0);
+  py[1] = __fadd_rn((float)px[1], s1);
+  py[2] = __fadd_rn((float)px[0], s2);
+}
+int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_pix, cudaStream_t st) {
+  if (n_pix == 0) return DEFER_OK;
+  const bool vec = reinterpret_cast<uintptr_t>(x) % 4 == 0 && reinterpret_cast<uintptr_t>(y) % 16 == 0;
+  const size_t threads = vec ? n_pix / 4 + n_pix % 4 : n_pix;
+  const unsigned grid = (unsigned)((threads + 255) / 256);
+  if (vec) {
+    prefer_max_smem(preprocess_kernel<true>);
+    preprocess_kernel<true><<<grid, 256, 0, st>>>(x, shift, y, n_pix);
+  } else {
+    prefer_max_smem(preprocess_kernel<false>);
+    preprocess_kernel<false><<<grid, 256, 0, st>>>(x, shift, y, n_pix);
+  }
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
 __global__ void __launch_bounds__(256) f32_to_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) y[i] = __float2bfloat16_rn(x[i]);

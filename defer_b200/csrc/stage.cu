@@ -91,6 +91,11 @@ struct OpRt {
   std::string kname;
   double alg_bytes = 0, alg_flops = 0;
   int n_kernels = 1;
+  // Keras caffe preprocessing (DEFER_OP_PREPROCESS).  It is folded into the fused stem conv that reads its output when
+  // that conv is its only reader; the op then launches nothing and its F32 image is never written.
+  float pre_shift[3] = {0.f, 0.f, 0.f};   // PREPROCESS: host copy of the shift weights
+  int folded_into = -1;                   // PREPROCESS: index of the conv that applies it, -1 = runs preprocess_kernel
+  int u8_pre = -1;                        // fused stem conv: index of the PREPROCESS op folded into it, -1 = none
 };
 
 struct Lane {
@@ -169,9 +174,11 @@ struct defer_stage_s {
 
 namespace defer {
 
-static size_t buf_bytes(const Buf& b, int fmt) {
-  return b.elems * (b.elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt));
+static size_t elem_bytes(int elem, int fmt) {
+  return elem == DEFER_BUF_U8 ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
 }
+
+static size_t buf_bytes(const Buf& b, int fmt) { return b.elems * elem_bytes(b.elem, fmt); }
 
 static int set_device(const defer_stage_s* s) {
   DEFER_CUDA(cudaSetDevice(s->cfg.device));
@@ -192,7 +199,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
   switch (d.kind) {
     case DEFER_OP_CONV: {
       if (op.backend == 4 && op.stem_fused)
-        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w, st);
+        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w,
+                                op.u8_pre >= 0, st);
       if (op.backend == 4)
         DEFER_TRY(launch_stem_im2col(fmt, (const float*)x, L.im2col[oi], nb, bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t,
                                      d.pad_l, bo.h, bo.w, op.k_pad, st));
@@ -244,6 +252,9 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       }
       if (bi.elem == DEFER_BUF_F32) return launch_encode(fmt, (const float*)x, y, bi.elems, st);
       return launch_decode(fmt, x, (float*)y, bi.elems, st);
+    case DEFER_OP_PREPROCESS:
+      if (op.folded_into >= 0) return DEFER_OK;   // applied by the stem conv as it reads the image
+      return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
   }
   set_error("launch_op: unknown op kind %d", d.kind);
   return DEFER_ERR_INVALID;
@@ -297,7 +308,7 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
   const double nb = s->cfg.batch;
   const Buf& bi = s->bufs[d.in0];
   const Buf& bo = s->bufs[d.out];
-  auto ab = [&](const Buf& b) { return (double)(b.elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt)); };
+  auto ab = [&](const Buf& b) { return (double)elem_bytes(b.elem, fmt); };
   double in_b = nb * bi.h * bi.w * bi.c * ab(bi), out_b = nb * bo.h * bo.w * bo.c * ab(bo);
   switch (d.kind) {
     case DEFER_OP_CONV: {
@@ -398,16 +409,20 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
   for (int i = 0; i < n_bufs; ++i) {
     Buf b;
     b.h = bufs[i].h; b.w = bufs[i].w; b.c = bufs[i].c; b.elem = bufs[i].elem;
-    if (b.h < 1 || b.w < 1 || b.c < 1 || (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32)) {
+    if (b.h < 1 || b.w < 1 || b.c < 1 || (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8)) {
       set_error("buffer %d: bad descriptor (%d,%d,%d,elem %d)", i, b.h, b.w, b.c, b.elem);
+      return fail(DEFER_ERR_INVALID);
+    }
+    if (b.elem == DEFER_BUF_U8 && !(cfg->is_first && i == cfg->input_buf)) {
+      set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer", i);
       return fail(DEFER_ERR_INVALID);
     }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;
     b.bytes = buf_bytes(b, cfg->fmt);
     s->bufs.push_back(b);
   }
-  if (cfg->is_first && s->bufs[cfg->input_buf].elem != DEFER_BUF_F32) {
-    set_error("first stage input must be an F32 buffer");
+  if (cfg->is_first && s->bufs[cfg->input_buf].elem == DEFER_BUF_ACT) {
+    set_error("first stage input must be an F32 or U8 buffer");
     return fail(DEFER_ERR_INVALID);
   }
   if (cfg->is_last && s->bufs[cfg->output_buf].elem != DEFER_BUF_F32) {
@@ -465,6 +480,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     const Buf& bi = s->bufs[d.in0];
     const Buf& bo = s->bufs[d.out];
+    if ((bi.elem == DEFER_BUF_U8 && d.kind != DEFER_OP_PREPROCESS) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_U8)) {
+      set_error("op %d: only a PREPROCESS op may read the U8 input buffer (as in0)", i);
+      return fail(DEFER_ERR_INVALID);
+    }
     switch (d.kind) {
       case DEFER_OP_CONV: {
         int ho = (bi.h + d.pad_t + d.pad_b - d.kh) / d.sh + 1, wo = (bi.w + d.pad_l + d.pad_r - d.kw) / d.sw + 1;
@@ -551,6 +570,22 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
           set_error("op %d (copy): size mismatch", i);
           return fail(DEFER_ERR_INVALID);
         }
+        break;
+      case DEFER_OP_PREPROCESS:
+        op.kname = "preprocess_kernel";
+        if (bi.elem != DEFER_BUF_U8 || bi.c != 3) {
+          set_error("op %d (preprocess): input must be a U8 buffer with 3 channels (elem %d, c %d)", i, bi.elem, bi.c);
+          return fail(DEFER_ERR_INVALID);
+        }
+        if (bo.elem != DEFER_BUF_F32 || bo.h != bi.h || bo.w != bi.w || bo.c != bi.c) {
+          set_error("op %d (preprocess): output must be an F32 buffer of the input's shape", i);
+          return fail(DEFER_ERR_INVALID);
+        }
+        if (d.w_shift < 0 || s->weight_bytes[d.w_shift] != 3 * sizeof(float)) {
+          set_error("op %d (preprocess): w_shift must hold 3 fp32 values", i);
+          return fail(DEFER_ERR_INVALID);
+        }
+        memcpy(op.pre_shift, weight_ptrs[d.w_shift], sizeof op.pre_shift);
         break;
       default:
         set_error("op %d: unknown kind %d", i, d.kind);
@@ -949,6 +984,28 @@ int defer_stage_finalize(defer_stage_t s) {
                                (d.flags & DEFER_FLAG_RESIDUAL) ? L.buf[d.in1] : nullptr, L.buf[d.out]));
     }
   }
+  // Fold a PREPROCESS op into the fused stem conv when that conv is the only reader of its (non-output) F32 image:
+  // the stem then reads the uint8 image and preprocesses each tap itself.  Every other path runs preprocess_kernel.
+  for (int pi = 0; pi < (int)s->ops.size(); ++pi) {
+    OpRt& pre = s->ops[pi];
+    if (pre.d.kind != DEFER_OP_PREPROCESS || pre.d.out == s->cfg.output_buf) continue;
+    int reader = -1, n_reads = 0;
+    for (int oi = 0; oi < (int)s->ops.size(); ++oi) {
+      const defer_op_desc& d = s->ops[oi].d;
+      const int r = (d.in0 == pre.d.out) + (d.in1 == pre.d.out);
+      if (r) reader = oi;
+      n_reads += r;
+    }
+    if (n_reads != 1 || s->ops[reader].d.kind != DEFER_OP_CONV || !s->ops[reader].stem_fused) continue;
+    OpRt& conv = s->ops[reader];
+    pre.folded_into = reader;
+    pre.n_kernels = 0;
+    pre.alg_bytes = 0;
+    conv.u8_pre = pi;
+    conv.kname = "conv_stem_u8_kernel";
+    pre.kname = "preprocess (fused into " + conv.kname + ")";
+    conv.alg_bytes -= (double)s->bufs[pre.d.in0].elems * 3.0;   // the image is read at 1 B/elem instead of 4
+  }
   for (int oi = 0; oi < (int)s->ops.size(); ++oi) {
     OpRt& op = s->ops[oi];
     if ((op.backend != 2 && op.backend != 4) || !op.persist) continue;
@@ -962,6 +1019,10 @@ int defer_stage_finalize(defer_stage_t s) {
         const defer_op_desc& d = op.d;
         const Buf& bi = s->bufs[d.in0];
         umma_mega_set_stem(host.data(), (const float*)L.buf[d.in0], bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t, d.pad_l);
+        if (op.u8_pre >= 0) {
+          const OpRt& pre = s->ops[op.u8_pre];
+          umma_mega_set_stem_u8(host.data(), (const uint8_t*)L.buf[pre.d.in0], pre.pre_shift);
+        }
       }
       DEFER_CUDA(cudaMalloc(&L.persist_op[oi], ob));
       s->workspace.push_back(L.persist_op[oi]);
@@ -1194,7 +1255,17 @@ int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_o
   DEFER_TRY(set_device(s));
   void* src = s->lanes[lane].buf[buf_id];
   DEFER_CHECK(src, "read_buffer: buffer %d is not bound yet", buf_id);
+  for (size_t i = 0; i < s->ops.size(); ++i)
+    DEFER_CHECK(!(s->ops[i].d.out == buf_id && s->ops[i].folded_into >= 0),
+                "read_buffer: buffer %d is never written: op %zu (preprocess) is folded into op %d (%s)", buf_id, i,
+                s->ops[i].folded_into, s->ops[s->ops[i].folded_into].kname.c_str());
   DEFER_CUDA(cudaStreamSynchronize(s->lanes[lane].stream));
+  if (b.elem == DEFER_BUF_U8) {
+    std::vector<uint8_t> raw(b.elems);
+    DEFER_CUDA(cudaMemcpy(raw.data(), src, b.elems, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < b.elems; ++i) host_out[i] = (float)raw[i];
+    return DEFER_OK;
+  }
   if (b.elem == DEFER_BUF_F32 || s->cfg.fmt == DEFER_FMT_F32) {
     DEFER_CUDA(cudaMemcpy(host_out, src, b.elems * 4, cudaMemcpyDeviceToHost));
     return DEFER_OK;
@@ -1222,6 +1293,8 @@ int defer_stage_time_op(defer_stage_t s, int op_index, int iters, int flush_l2, 
   Lane& L = s->lanes[0];
   const defer_op_desc& d = s->ops[op_index].d;
   DEFER_CHECK(L.buf[d.out] && L.buf[d.in0], "time_op: op buffers not bound");
+  DEFER_CHECK(s->ops[op_index].folded_into < 0, "time_op: op %d launches nothing, it is folded into op %d (%s)", op_index,
+              s->ops[op_index].folded_into, s->ops[op_index].folded_into >= 0 ? s->ops[s->ops[op_index].folded_into].kname.c_str() : "");
   if (flush_l2 && !s->flush_buf) {
     s->flush_bytes = 256ull << 20;  // > 126 MB L2
     DEFER_CUDA(cudaMalloc(&s->flush_buf, s->flush_bytes));

@@ -13,8 +13,14 @@ What changed underneath:
   pinned-memory DMA instead of ZFP+LZ4+TCP.
 
 Non-reference additions: ``close()`` / context manager (the reference can only be killed), keyword-only
-``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1) and
-``coalesce``.
+``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1),
+``coalesce`` and ``preprocess``.
+
+Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the host before every ``input_q.put``
+(``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
+(``img_to_array(img).astype(np.uint8)``, shape ``(batch, h, w, 3)``) and the first stage applies the transform on its
+GPU, bit for bit what ``applications.preprocess_input`` gives on the host; an image crosses PCIe at 1 B per value
+instead of 4.  Other item dtypes are refused.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -33,6 +39,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import keras_like as K
+from .applications import check_preprocess
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
 
@@ -40,8 +47,11 @@ from .node import DTYPE_TO_FMT, StageRunner, parse_device
 class DEFER:
     def __init__(self, computeNodes, *, dtype: str = "float32", depth: int = 4, batch: Optional[int] = None,
                  coalesce: int = 1, linger_us: float = 200.0, conv_backend: int = 0, dist=None,
-                 wait_timeout_ms: int = 0, max_inflight: int = 0) -> None:
+                 wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None) -> None:
+        if preprocess is not None:
+            check_preprocess(preprocess)
         self.computeNodes = list(computeNodes)
+        self.preprocess = preprocess        # None | "caffe": uint8 queue items, preprocessed on stage 0's GPU
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -100,7 +110,8 @@ class DEFER:
                 self.dist.send_stage(i, {"json": models[i].to_json(), "weights": models[i].get_weights(),
                                          "next_node": str(next_node), "fmt": self.dtype, "batch": batch,
                                          "depth": self.depth, "conv_backend": self.conv_backend,
-                                         "wait_timeout_ms": self.wait_timeout_ms})
+                                         "wait_timeout_ms": self.wait_timeout_ms,
+                                         "preprocess": self.preprocess if i == 0 else None})
             self.dist.wait_all_ready()      # the 1-byte ACK of dispatcher.py:64-65
             return
         runners = []
@@ -110,7 +121,8 @@ class DEFER:
             r = StageRunner.from_wire(model_json, weights, device=parse_device(nodeIPs[i]), dtype=self.dtype,
                                       max_batch=batch, depth=self.depth, is_first=(i == 0), is_last=(i == n - 1),
                                       finalize=False, conv_backend=self.conv_backend,
-                                      wait_timeout_ms=self.wait_timeout_ms)
+                                      wait_timeout_ms=self.wait_timeout_ms,
+                                      preprocess=self.preprocess if i == 0 else None)
             r.name = f"part{i+1}"
             runners.append(r)
         for i in range(n - 1):              # next hop = nodeIPs[i+1] (dispatcher.py:51-55)
@@ -123,6 +135,7 @@ class DEFER:
     def _startDistEdgeInference(self, input: queue.Queue):
         first = self.stages[0] if self.stages else self.dist.local_runner()
         G, B = self.coalesce, self.batch or 1
+        u8 = self.preprocess is not None
         hold, nh = self._hold, len(self._hold)
         get_nowait = input.get_nowait
         submit_items = first.submit_items if hasattr(first, "submit_items") else None
@@ -146,7 +159,13 @@ class DEFER:
                 in_shape = None
                 while True:
                     x = model_input
-                    if not (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]):
+                    if u8:
+                        if not (isinstance(x, np.ndarray) and x.dtype == np.uint8):
+                            raise TypeError(f"DEFER(preprocess={self.preprocess!r}) takes uint8 RGB images "
+                                            "(img_to_array(img).astype(np.uint8)), got "
+                                            f"{getattr(x, 'dtype', type(x).__name__)}; do not preprocess them on the host")
+                        x = np.ascontiguousarray(x)
+                    elif not (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]):
                         x = np.ascontiguousarray(x, dtype=np.float32)
                     if x.shape[0] != B:
                         raise ValueError(f"queue item has batch {x.shape[0]}, DEFER was built for batch {B}")

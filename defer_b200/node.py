@@ -74,6 +74,8 @@ class StageRunner:
                     f"device {self.device}: {used} lane streams already live, {self.depth} more would exceed "
                     f"{MAX_STREAMS_PER_DEVICE} hardware work queues - flag-waiting lanes could block their own "
                     "producer.  Use fewer stages per GPU or a smaller depth.")
+        # a stage planned with preprocess= takes uint8 images (Keras caffe preprocessing runs on the GPU)
+        self.in_dtype = np.uint8 if plan.bufs[plan.input_buf][3] == A.BUF_U8 else np.float32
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
         self.out_elems = int(np.prod(self.out_shape))
@@ -101,8 +103,11 @@ class StageRunner:
     # ---- construction helpers
     @classmethod
     def from_model(cls, model: K.Model, device=0, dtype: str = "float32", max_batch: int = 1, depth: int = 1,
-                   is_first: bool = True, is_last: bool = True, finalize: bool = True, **kw) -> "StageRunner":
-        plan = plan_stage(model, is_first=is_first, is_last=is_last)
+                   is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
+                   **kw) -> "StageRunner":
+        """``preprocess="caffe"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the stage
+        applies Keras' caffe ``preprocess_input`` on the GPU."""
+        plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
                 is_last=is_last, name=model.name, **kw)
@@ -138,12 +143,31 @@ class StageRunner:
         A.check(self.lib.defer_stage_unlink(self.handle))
 
     # ---- steady state
+    def _host_input(self, x) -> np.ndarray:
+        """``x`` as the C-contiguous array the stage copies from.  A stage without preprocessing converts to float32.
+        A preprocessing stage takes uint8 only: a float array may be ``img_to_array`` output or already preprocessed,
+        and neither can be told apart from the other."""
+        if self.in_dtype == np.uint8:
+            if getattr(x, "dtype", None) != np.uint8:
+                raise TypeError(f"{self.name}: this stage preprocesses uint8 RGB images on the GPU (preprocess='caffe') "
+                                f"and got dtype {getattr(x, 'dtype', type(x).__name__)}; pass the image as "
+                                "img_to_array(img).astype(np.uint8), not preprocessed or float data")
+            if x.ndim != 4 or tuple(x.shape[1:]) != self.in_shape[1:]:   # e.g. channels-first: same bytes, wrong image
+                raise ValueError(f"{self.name}: image shape {tuple(x.shape)} is not (k,) + {self.in_shape[1:]} "
+                                 "(channels-last RGB)")
+            if not x.flags["C_CONTIGUOUS"]:
+                x = np.ascontiguousarray(x)
+                self._keep = x
+            return x
+        if not (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]):
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            self._keep = x
+        return x
+
     def submit(self, seq: int, x: np.ndarray) -> None:
         """Enqueue the H2D copy of microbatch ``seq``.  ``x`` must stay alive and unmodified until the
         step has consumed it; arrays registered with ``pin`` (or from ``pinned_empty``) copy asynchronously."""
-        if x.dtype != np.float32 or not x.flags["C_CONTIGUOUS"]:
-            x = np.ascontiguousarray(x, dtype=np.float32)
-            self._keep = x
+        x = self._host_input(x)
         if tuple(x.shape) != self.in_shape:
             raise ValueError(f"{self.name}: input shape {tuple(x.shape)} != stage input {self.in_shape}")
         A.check(self.lib.defer_stage_submit(self.handle, seq, x.ctypes.data, x.nbytes))
@@ -151,16 +175,19 @@ class StageRunner:
     def submit_part(self, seq: int, index: int, x: np.ndarray) -> None:
         """Coalesced ingress: copy the queue item ``x`` (``k`` samples, usually 1 - ``test/test.py:22``) into samples
         ``[index, index + k)`` of microbatch ``seq``.  Same lifetime rule as ``submit``."""
-        if x.dtype != np.float32 or not x.flags["C_CONTIGUOUS"]:
-            x = np.ascontiguousarray(x, dtype=np.float32)
-            self._keep = x
+        x = self._host_input(x)
         if tuple(x.shape[1:]) != self.in_shape[1:]:
             raise ValueError(f"{self.name}: item shape {tuple(x.shape)} does not match stage input {self.in_shape}")
         A.check(self.lib.defer_stage_submit_part(self.handle, seq, index, x.shape[0], x.ctypes.data, x.nbytes))
 
     def submit_items(self, seq: int, items) -> None:
-        """Coalesced ingress, one C call per group: ``items`` are C-contiguous float32 arrays of identical shape
-        ``(k,) + input_shape[1:]``; item i lands in samples ``[i*k, (i+1)*k)`` of microbatch ``seq``."""
+        """Coalesced ingress, one C call per group: ``items`` are C-contiguous arrays of the stage's input dtype (float32,
+        or uint8 on a preprocessing stage) and identical shape ``(k,) + input_shape[1:]``; item i lands in samples
+        ``[i*k, (i+1)*k)`` of microbatch ``seq``."""
+        if self.in_dtype == np.uint8:
+            for x in items:
+                if self._host_input(x) is not x:
+                    raise ValueError(f"{self.name}: submit_items needs C-contiguous items")
         n = len(items)
         ptrs = self._ptr_arrays.get(n)
         if ptrs is None:
@@ -194,7 +221,7 @@ class StageRunner:
 
     def predict(self, x: np.ndarray) -> np.ndarray:
         """Single-stage ``model.predict`` (reference ``test/local_infer.py:21``)."""
-        x = np.ascontiguousarray(x, dtype=np.float32)
+        x = self._host_input(x)
         out = np.empty(self.out_shape, np.float32)
         A.check(self.lib.defer_stage_predict(self.handle, x.ctypes.data, x.nbytes, out.ctypes.data, out.nbytes))
         return out
@@ -349,7 +376,8 @@ class Node:
         runner = StageRunner.from_wire(msg["json"], ns.weights, device=dev, dtype=msg["fmt"], max_batch=msg["batch"],
                                        depth=msg["depth"], is_first=(rank == 0), is_last=(rank == world - 1),
                                        finalize=False, conv_backend=msg.get("conv_backend", 0),
-                                       wait_timeout_ms=msg.get("wait_timeout_ms", 0))
+                                       wait_timeout_ms=msg.get("wait_timeout_ms", 0),
+                                       preprocess=msg.get("preprocess") if rank == 0 else None)
         ns.model = runner                               # src/node.py:38
         self.runner = runner
         # wire the hop: my consumer gives me its input-side token, I give it my output-side token

@@ -14,6 +14,10 @@ executable form is a short list of fused ops (``include/defer_b200.h``):
 
 A follower is absorbed only when the tensor between the two layers has exactly one consumer and is
 not the stage output - otherwise that tensor must exist in memory.
+
+With ``preprocess="caffe"`` (first stage only) the stage input is a uint8 RGB image and a ``PREPROCESS`` op
+(Keras' caffe ``preprocess_input``) writes the fp32 tensor the rest of the plan reads; the library folds it
+into the fused RGB stem when it can.
 """
 from __future__ import annotations
 
@@ -24,6 +28,7 @@ import numpy as np
 
 from . import _cabi as A
 from . import keras_like as K
+from .applications import caffe_shift, check_preprocess
 
 
 def same_pad(size: int, k: int, s: int) -> Tuple[int, int]:
@@ -82,7 +87,11 @@ def _hwc(shape) -> Tuple[int, int, int]:
     raise ValueError(f"unsupported tensor rank {shape}")
 
 
-def plan_stage(model: K.Model, is_first: bool, is_last: bool) -> Plan:
+def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None) -> Plan:
+    if preprocess is not None:
+        check_preprocess(preprocess)
+        if not is_first:
+            raise ValueError(f"preprocess={preprocess!r}: only the first stage takes images")
     nodes = list(model.iter_nodes())
     # names as recorded at map time (tensor histories may be re-tagged later by Input(tensor=...))
     order = [l.name for l, _ in nodes]
@@ -165,9 +174,18 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool) -> Plan:
         return materialise(t), (0, 0, 0, 0), []
 
     # stage input
-    tensor_buf[in_name] = new_buf(shapes[in_name], A.BUF_F32 if is_first else A.BUF_ACT)
+    if preprocess is None:
+        tensor_buf[in_name] = new_buf(shapes[in_name], A.BUF_F32 if is_first else A.BUF_ACT)
+        input_buf = tensor_buf[in_name]
+    else:
+        if _hwc(shapes[in_name])[2] != 3 or len(shapes[in_name]) != 4:
+            raise ValueError(f"preprocess={preprocess!r}: the input must be an RGB image (h, w, 3), got {shapes[in_name][1:]}")
+        input_buf = new_buf(shapes[in_name], A.BUF_U8)
+        op = emit(PlanOp(A.OP_PREPROCESS, input_buf, new_buf(shapes[in_name], A.BUF_F32),
+                         layers=[f"preprocess_input({preprocess})"]))
+        op.w_shift = add_weight(caffe_shift())
+        tensor_buf[in_name] = op.out
     producer[in_name] = None
-    input_buf = tensor_buf[in_name]
 
     for name in order:
         if name == in_name:

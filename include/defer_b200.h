@@ -62,7 +62,10 @@ typedef enum defer_op_kind {
   DEFER_OP_RELU = 7,     /* standalone Activation('relu')                                                     */
   DEFER_OP_ADD = 8,      /* standalone Add of two tensors [+ relu]                                            */
   DEFER_OP_PAD = 9,      /* standalone ZeroPadding2D                                                          */
-  DEFER_OP_COPY = 10     /* identity / Flatten / format cast                                                  */
+  DEFER_OP_COPY = 10,    /* identity / Flatten / format cast                                                  */
+  DEFER_OP_PREPROCESS = 11 /* Keras caffe-mode preprocess_input: in0 = U8 image (c == 3), out = F32 of the same    */
+                         /* shape, w_shift = 3 fp32 values in output-channel order;                              */
+                         /* y[..., c] = float(x[..., 2 - c]) + shift[c]  (RGB -> BGR, minus the ImageNet mean)   */
 } defer_op_kind;
 
 #define DEFER_FLAG_RELU      1u   /* apply relu at the end of the op                 */
@@ -71,11 +74,12 @@ typedef enum defer_op_kind {
 /* Buffer element type. */
 #define DEFER_BUF_ACT 0   /* stage activation format (defer_fmt of the stage) */
 #define DEFER_BUF_F32 1   /* plain fp32 regardless of the stage format (image in, probabilities out) */
+#define DEFER_BUF_U8  2   /* uint8 NHWC, 1 B/elem: only the first stage's input buffer, read only by DEFER_OP_PREPROCESS */
 
 /* One logical tensor of the plan.  Shapes are per sample, NHWC; vectors use h = w = 1. */
 typedef struct defer_buf_desc {
   int32_t h, w, c;
-  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 */
+  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 */
 } defer_buf_desc;
 
 /* One fused op of the plan.  Buffer ids index the defer_buf_desc array; weight ids index the
@@ -88,7 +92,7 @@ typedef struct defer_op_desc {
   uint32_t flags;          /* DEFER_FLAG_* */
   int32_t w_kernel;        /* CONV: fp32 HWIO kernel;  DENSE: fp32 (in,out) kernel */
   int32_t w_scale;         /* CONV / AFFINE: fp32 per-channel scale (NULL id -1 = ones) */
-  int32_t w_shift;         /* CONV / AFFINE: fp32 per-channel shift;  DENSE: bias */
+  int32_t w_shift;         /* CONV / AFFINE / PREPROCESS: fp32 per-channel shift;  DENSE: bias */
   int32_t reserved;
 } defer_op_desc;
 
@@ -187,7 +191,8 @@ DEFER_API int defer_stage_mark_elapsed(defer_stage_t s, float* ms);
 
 /* ---- introspection for tests and benches --------------------------------------------------- */
 DEFER_API int defer_stage_num_kernels(defer_stage_t s, int* per_step);           /* kernel launches per step */
-/* copy any plan buffer of `lane` to host as fp32 NHWC (decodes the stage format) */
+/* copy any plan buffer of `lane` to host as fp32 NHWC (decodes the stage format; a U8 buffer reads as its values
+ * 0..255).  Fails for the F32 image of a PREPROCESS op folded into the stem conv: that buffer is never written. */
 DEFER_API int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_out, uint64_t n_floats);
 /* stream / event handles for external timing (cudaStream_t as void*) */
 DEFER_API int defer_stage_stream(defer_stage_t s, int lane, void** stream);
@@ -227,6 +232,9 @@ DEFER_API int defer_k_eltwise(int fmt, int kind /* AFFINE | RELU | ADD */, const
 /* fp32 <-> stage-format conversion of a whole tensor (device pointers) */
 DEFER_API int defer_k_encode(int fmt, const float* x_f32, void* y_act, uint64_t n_elems, void* stream);
 DEFER_API int defer_k_decode(int fmt, const void* x_act, float* y_f32, uint64_t n_elems, void* stream);
+/* Keras caffe-mode preprocess_input (DEFER_OP_PREPROCESS): uint8 NHWC image (c == 3) -> fp32,
+ * y[..., c] = float(x[..., 2 - c]) + shift[c]; shift: 3 fp32 values on the device */
+DEFER_API int defer_k_preprocess(const uint8_t* x, const float* shift, float* y, int n, int h, int w, int c, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,165 @@
+"""Ingress cost of Keras caffe preprocessing: host fp32 items vs uint8 items preprocessed on the GPU.
+
+One GPU, ResNet50 (224 x 224, synthetic weights, fp32 parity), DEFER.run_defer with coalesce=32 and depth=4.  Three arms,
+each a live pipeline, timed in alternation (--reps rounds after one warm-up round):
+
+  a  fp32 items, already preprocessed before the clock starts, put on a full input queue
+  b  uint8 items, applications.preprocess_input in the feeding thread (what a reference-style driver does)
+  c  uint8 items on a full input queue, DEFER(preprocess="caffe"): the first stage preprocesses on the GPU
+
+It prints one JSON line: end-to-end inferences/s per arm (median, min, max over the rounds), H2D bytes per item, the
+device time of the fp32 fused stem, the uint8 fused stem and the standalone preprocess_kernel (time_op, L2 flushed), the
+host time of one preprocess_input call, and the card's name and power limit (read-only nvidia-smi query).
+
+    python tools/ingress_bench.py [--items 640] [--reps 3]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import queue
+import statistics
+import subprocess
+import sys
+import threading
+import time
+from pathlib import Path
+
+import numpy as np
+
+sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+
+from defer_b200 import applications  # noqa: E402
+from defer_b200.dispatcher import DEFER  # noqa: E402
+from defer_b200.node import StageRunner  # noqa: E402
+
+G, DEPTH = 32, 4
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                             text=True, timeout=30).stdout.strip().splitlines()
+        name, power = out[0].rsplit(",", 1)
+        return {"gpu": name.strip(), "power_limit": power.strip()}
+    except Exception as e:  # noqa: BLE001
+        return {"gpu": "unknown", "power_limit": f"unknown ({e})"}
+
+
+class Arm:
+    def __init__(self, model, preprocess):
+        self.defer = DEFER([0], depth=DEPTH, coalesce=G, linger_us=2000, preprocess=preprocess)
+        self.in_q, self.out_q = queue.Queue(), queue.Queue()
+        self.err = []
+        self.thread = threading.Thread(target=self._run, args=(model,), daemon=True)
+        self.thread.start()
+        if not self.defer.wait_ready(600) or self.err:
+            raise RuntimeError(f"pipeline did not come up: {self.err}")
+        st = self.defer.stages[0]
+        self.h2d_per_item = st.io_bytes()[0] // st.batch
+
+    def _run(self, model):
+        try:
+            self.defer.run_defer(model, [], self.in_q, self.out_q)
+        except BaseException as e:  # noqa: BLE001
+            self.err.append(e)
+
+    def rate(self, items, host_preprocess=False):
+        """Inferences/s from the first put to the last result."""
+        t0 = time.perf_counter()
+        if host_preprocess:
+            def feed():
+                for x in items:
+                    self.in_q.put(applications.preprocess_input(x))
+            f = threading.Thread(target=feed, daemon=True)
+            f.start()
+        else:
+            for x in items:
+                self.in_q.put(x)
+        for _ in items:
+            self.out_q.get(timeout=300)
+        dt = time.perf_counter() - t0
+        if host_preprocess:
+            f.join()
+        if self.err:
+            raise RuntimeError(self.err)
+        return len(items) / dt
+
+    def close(self):
+        self.defer.close()
+        self.thread.join(timeout=60)
+
+
+def stem_times(model, iters):
+    """time_op (us) of the three stem kernels at the benchmarked microbatch (32 images)."""
+    out = {}
+    for key, env, pre, op in (("conv_stem_kernel_f32_us", None, None, 0), ("conv_stem_u8_kernel_us", None, "caffe", 1),
+                              ("preprocess_kernel_us", "0", "caffe", 0)):
+        old = os.environ.pop("DEFER_STEM_FUSED", None)
+        if env is not None:
+            os.environ["DEFER_STEM_FUSED"] = env
+        try:
+            r = StageRunner.from_model(model, device=0, dtype="float32", max_batch=G, depth=1, preprocess=pre)
+        finally:
+            os.environ.pop("DEFER_STEM_FUSED", None)
+            if old is not None:
+                os.environ["DEFER_STEM_FUSED"] = old
+        try:
+            kernel = r.op_info(op)["kernel"]
+            r.predict(applications.synthetic_image(G, seed=1) if pre else applications.synthetic_input(G, seed=1))
+            ts = [r.time_op(op, iters=iters, flush_l2=True) for _ in range(3)]
+            out[key] = {"kernel": kernel, "us": round(statistics.median(ts), 2), "spread_us": round(max(ts) - min(ts), 2)}
+        finally:
+            r.close()
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--items", type=int, default=640, help="queue items per timed round (batch-1 images)")
+    ap.add_argument("--reps", type=int, default=3, help="timed rounds per arm (alternated), >= 3")
+    ap.add_argument("--op-iters", type=int, default=50)
+    args = ap.parse_args()
+    if args.reps < 3:
+        ap.error("--reps must be >= 3")
+
+    model = applications.ResNet50()
+    imgs = [applications.synthetic_image(1, seed=i) for i in range(args.items)]
+    pre = [applications.preprocess_input(x) for x in imgs]
+
+    t0 = time.perf_counter()
+    n_host = 200
+    for i in range(n_host):
+        applications.preprocess_input(imgs[i % len(imgs)])
+    host_us = (time.perf_counter() - t0) / n_host * 1e6
+
+    arms = {"a_f32_items": Arm(model, None), "b_u8_host_preprocess": Arm(model, None), "c_u8_gpu_preprocess": Arm(model, "caffe")}
+    feeds = {"a_f32_items": (pre, False), "b_u8_host_preprocess": (imgs, True), "c_u8_gpu_preprocess": (imgs, False)}
+    rates = {k: [] for k in arms}
+    try:
+        for rnd in range(args.reps + 1):
+            for k, arm in arms.items():
+                items, host = feeds[k]
+                r = arm.rate(items, host_preprocess=host)
+                if rnd > 0:                                   # round 0 warms every shape up
+                    rates[k].append(r)
+        h2d = {k: arm.h2d_per_item for k, arm in arms.items()}
+    finally:
+        for arm in arms.values():
+            arm.close()
+
+    res = {
+        "metric": "resnet50_ingress_inferences_per_s",
+        "coalesce": G, "depth": DEPTH, "items_per_round": args.items, "rounds": args.reps,
+        "arms": {k: {"median": round(statistics.median(v), 1), "min": round(min(v), 1), "max": round(max(v), 1),
+                     "all": [round(x, 1) for x in v], "h2d_bytes_per_item": h2d[k]} for k, v in rates.items()},
+        "host_preprocess_input_us": round(host_us, 1),
+        "stem_time_op": stem_times(model, args.op_iters),
+    }
+    res.update(card())
+    print(json.dumps(res), flush=True)
+
+
+if __name__ == "__main__":
+    main()
