@@ -8,6 +8,10 @@ The reference imports these from ``tensorflow.python.keras.applications``
   shortcut, conv biases, BN eps 1e-3, auto-named ``Add``/``Activation`` layers (tf.keras
   zero-based: ``add, add_1, ... add_15``), so the cut list of ``test/test.py:18`` applies verbatim.
 * ``ResNet152``: ``resnet_common.py`` (``conv{s}_block{b}_{1,2,3}_conv``, ``_add``, ``_out``, eps 1.001e-5).
+* ``ResNet50V2`` / ``ResNet101V2`` / ``ResNet152V2``: ``resnet_common.py``'s pre-activation blocks
+  (``_preact_bn``, ``_preact_relu``, ``_0_conv`` in the first block of a stack, bias-free ``_1_conv`` / ``_2_conv``,
+  the stride in the last block with an auto-named ``MaxPooling2D(1, strides=2)`` identity shortcut, ``_out`` Adds,
+  ``post_bn``, ``post_relu``).
 * ``VGG16``: ``block{i}_conv{j}`` (relu inside the conv), ``block{i}_pool``, ``flatten``, ``fc1``, ``fc2``,
   ``predictions``.
 
@@ -27,13 +31,20 @@ from .keras_like import (Activation, Add, BatchNormalization, Conv2D, Dense, Fla
 
 # --------------------------------------------------------------------------- synthetic weights
 
+#: ResNet V2 residual-branch gain: the conv that feeds an ``Add`` directly is scaled by this over sqrt(number of Adds).
+#: Chosen on the CPU oracle at seed 1: top-1 probability 0.84 / 0.08 / 0.11 for 50V2 / 101V2 / 152V2, with 10+ classes
+#: above 1e-3 and every ``_out`` sum of RMS 0.5-6; 2.5 already pushes 50V2 to 0.97.
+V2_BRANCH_GAIN = 2.2
+
+
 def synthetic_weights(model: Model, seed: int = 1, logit_std: float = 2.0) -> None:
     """Fill ``model`` with deterministic weights (see DESIGN.md "Synthetic data").
 
     conv / dense kernels: He-normal; biases N(0, 0.1); BN gamma U(0.8, 1.2), beta N(0, 0.1),
     mean N(0, 0.1), var U(0.8, 1.2).  The BN that feeds the main branch of a residual ``Add``
-    gets gamma x 0.25 so the variance stays O(1) over 16-50 blocks; the last Dense is scaled so
-    logits have std ~``logit_std`` (softmax not saturated).
+    gets gamma x 0.25 so the variance stays O(1) over 16-50 blocks; a conv that feeds an ``Add``
+    directly (ResNet V2) gets its kernel x ``V2_BRANCH_GAIN / sqrt(#Adds)``; the last Dense is scaled
+    so logits have std ~``logit_std`` (softmax not saturated).
     """
     rng = np.random.default_rng(seed)
     # BN layers directly feeding an Add together with a deeper path get damped
@@ -50,6 +61,13 @@ def synthetic_weights(model: Model, seed: int = 1, logit_std: float = 2.0) -> No
             src = model.get_layer(ins[0])
             if isinstance(src, Conv2D) and (layer.name.endswith("branch1") or layer.name.endswith("_0_bn")):
                 damp.discard(layer.name)
+    # ResNet V2: a residual branch ends in a conv feeding the Add directly (no BN to damp), and the pre-activation BN that
+    # reads the sum does not normalise it, so the sum grows geometrically with depth (top-1 probability 1.0 unscaled).
+    # No V1 model or VGG has such a conv, so their weights are unchanged.
+    n_adds = sum(isinstance(l, Add) for l, _ in model.iter_nodes())
+    res_convs = {n for l, ins in model.iter_nodes() if isinstance(l, Add) for n in ins
+                 if isinstance(model.get_layer(n), Conv2D)}
+    res_scale = np.float32(V2_BRANCH_GAIN / np.sqrt(max(n_adds, 1)))
     last_dense = None
     for layer, _ in model.iter_nodes():
         if isinstance(layer, Dense):
@@ -62,6 +80,8 @@ def synthetic_weights(model: Model, seed: int = 1, logit_std: float = 2.0) -> No
                  * np.float32(np.sqrt(2.0 / fan_in))]
             if layer.use_bias:
                 w.append((rng.standard_normal(layer.filters, dtype=np.float32) * np.float32(0.1)))
+            if layer.name in res_convs:
+                w[0] = w[0] * res_scale     # after drawing: the RNG stream is the same with or without it
             layer.set_weights(w)
         elif isinstance(layer, Dense):
             fan_in = layer.in_features
@@ -264,6 +284,68 @@ def ResNet152(weights: Optional[str] = "synthetic", include_top: bool = True, in
 def ResNet101(weights: Optional[str] = "synthetic", include_top: bool = True, input_shape=(224, 224, 3),
               classes: int = 1000, seed: int = 1, fresh_names: bool = True) -> Model:
     return _resnet_common([3, 4, 23, 3], "resnet101", weights, input_shape, classes, seed, fresh_names)
+
+
+# --------------------------------------------------------------------------- ResNet V2 (resnet_common, pre-activation)
+
+def _block2(x, filters, kernel_size=3, stride=1, conv_shortcut=False, name=""):
+    eps = 1.001e-5
+    preact = BatchNormalization(epsilon=eps, name=name + "_preact_bn")(x)
+    preact = Activation("relu", name=name + "_preact_relu")(preact)
+    if conv_shortcut:
+        sc = Conv2D(4 * filters, 1, strides=stride, name=name + "_0_conv")(preact)
+    else:
+        sc = MaxPooling2D(1, strides=stride)(x) if stride > 1 else x
+    y = Conv2D(filters, 1, strides=1, use_bias=False, name=name + "_1_conv")(preact)
+    y = BatchNormalization(epsilon=eps, name=name + "_1_bn")(y)
+    y = Activation("relu", name=name + "_1_relu")(y)
+    y = ZeroPadding2D(padding=((1, 1), (1, 1)), name=name + "_2_pad")(y)
+    y = Conv2D(filters, kernel_size, strides=stride, use_bias=False, name=name + "_2_conv")(y)
+    y = BatchNormalization(epsilon=eps, name=name + "_2_bn")(y)
+    y = Activation("relu", name=name + "_2_relu")(y)
+    y = Conv2D(4 * filters, 1, name=name + "_3_conv")(y)
+    return Add(name=name + "_out")([sc, y])
+
+
+def _stack2(x, filters, blocks, stride1=2, name=""):
+    x = _block2(x, filters, conv_shortcut=True, name=name + "_block1")
+    for i in range(2, blocks):
+        x = _block2(x, filters, name=f"{name}_block{i}")
+    return _block2(x, filters, stride=stride1, name=f"{name}_block{blocks}")
+
+
+def _resnet_v2(blocks, model_name, weights, input_shape, classes, seed, fresh_names):
+    if fresh_names:
+        K.clear_session()
+    img = Input(shape=input_shape)
+    x = ZeroPadding2D(padding=((3, 3), (3, 3)), name="conv1_pad")(img)
+    x = Conv2D(64, 7, strides=2, name="conv1_conv")(x)
+    x = ZeroPadding2D(padding=((1, 1), (1, 1)), name="pool1_pad")(x)
+    x = MaxPooling2D(3, strides=2, name="pool1_pool")(x)
+    x = _stack2(x, 64, blocks[0], name="conv2")
+    x = _stack2(x, 128, blocks[1], name="conv3")
+    x = _stack2(x, 256, blocks[2], name="conv4")
+    x = _stack2(x, 512, blocks[3], stride1=1, name="conv5")
+    x = BatchNormalization(epsilon=1.001e-5, name="post_bn")(x)
+    x = Activation("relu", name="post_relu")(x)
+    x = GlobalAveragePooling2D(name="avg_pool")(x)
+    x = Dense(classes, activation="softmax", name="predictions")(x)
+    return _finish(Model(img, x, name=model_name), weights, seed)
+
+
+def ResNet50V2(weights: Optional[str] = "synthetic", include_top: bool = True, input_shape=(224, 224, 3),
+               classes: int = 1000, seed: int = 1, fresh_names: bool = True) -> Model:
+    return _resnet_v2([3, 4, 6, 3], "resnet50v2", weights, input_shape, classes, seed, fresh_names)
+
+
+def ResNet101V2(weights: Optional[str] = "synthetic", include_top: bool = True, input_shape=(224, 224, 3),
+                classes: int = 1000, seed: int = 1, fresh_names: bool = True) -> Model:
+    return _resnet_v2([3, 4, 23, 3], "resnet101v2", weights, input_shape, classes, seed, fresh_names)
+
+
+def ResNet152V2(weights: Optional[str] = "synthetic", include_top: bool = True, input_shape=(224, 224, 3),
+                classes: int = 1000, seed: int = 1, fresh_names: bool = True) -> Model:
+    return _resnet_v2([3, 8, 36, 3], "resnet152v2", weights, input_shape, classes, seed, fresh_names)
 
 
 # --------------------------------------------------------------------------- VGG16

@@ -40,8 +40,8 @@ int defer_k_conv(int fmt, int backend, const void* x, int x_is_f32, const float*
       if (rc == DEFER_OK && cudaMalloc(&dev_op, host.size()) != cudaSuccess) rc = DEFER_ERR_CUDA;
       if (rc == DEFER_OK) cudaMemcpy(dev_op, host.data(), host.size(), cudaMemcpyHostToDevice);
       if (rc == DEFER_OK)
-        rc = backend == 3 ? launch_conv_persistent(plan.nplanes, dev_op, n_tiles, st)
-                          : launch_conv_stream(plan.nplanes, plan.bn, dev_op, n_tiles, plan.k_blocks, st);
+        rc = backend == 3 ? launch_conv_persistent(plan.nplanes, dev_op, n_tiles, false, st)
+                          : launch_conv_stream(plan.nplanes, plan.bn, dev_op, n_tiles, plan.k_blocks, false, st);
     }
     cudaError_t e = cudaStreamSynchronize(st);
     if (dev_op) cudaFree(dev_op);

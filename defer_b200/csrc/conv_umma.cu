@@ -86,6 +86,14 @@ struct alignas(128) MegaOp {
   // value[c] = float(image[2 - c]) + stem_shift[c]
   const uint8_t* stem_u8;
   float stem_shift[3];
+  // second epilogue output (conv_umma_aff_kernel / conv_stream_aff_kernel): a standalone per-channel affine(+ReLU) of
+  // the stored result, y2 = [relu](fmaf(stored, scale2[c], shift2[c])).  Appended last: the fields above keep their
+  // offsets and sizeof(MegaOp) stays 768 B.
+  const float* scale2;
+  const float* shift2;
+  void* y2;
+  int relu2;
+  int store_first;           // 0: only y2 is written (nothing else reads the conv's own output)
 };
 
 template <int NPLANES, int BN>
@@ -268,9 +276,12 @@ __device__ __forceinline__ void row_to_pixel(const KParams& p, int r, int n0, in
   }
 }
 
-// bias/BN, residual, ReLU and the store of two adjacent channels (c, c + 1) of one output pixel
-template <int NPLANES>
-__device__ __forceinline__ void epi_pair(const KParams& p, size_t pix, int c, float v0, float v1) {
+// bias/BN, residual, ReLU and the store of two adjacent channels (c, c + 1) of one output pixel.
+// AFF: then the folded affine op of MegaOp::scale2 etc. on the value as stored - hi + lo (BF16X2) or the bf16 (BF16),
+// exactly what eltwise_kernel<FMT, DEFER_OP_AFFINE> reads back - with the same fmaf, ReLU and split, into y2.  The folded
+// result is therefore bit-identical to the conv followed by the standalone affine op.
+template <int NPLANES, bool AFF = false>
+__device__ __forceinline__ void epi_pair(const KParams& p, const MegaOp& op, size_t pix, int c, float v0, float v1) {
   const float2 sc = p.scale ? __ldg(reinterpret_cast<const float2*>(p.scale + c)) : make_float2(1.f, 1.f);
   const float2 sf = p.shift ? __ldg(reinterpret_cast<const float2*>(p.shift + c)) : make_float2(0.f, 0.f);
   v0 = fmaf(v0, sc.x, sf.x);
@@ -291,14 +302,46 @@ __device__ __forceinline__ void epi_pair(const KParams& p, size_t pix, int c, fl
     v0 = fmaxf(v0, 0.f);
     v1 = fmaxf(v1, 0.f);
   }
-  uint32_t* y = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o);
-  if (NPLANES == 2) {
-    uint32_t hi, lo;
-    split_bf16x2(v0, v1, hi, lo);
-    y[0] = hi;
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
+  if constexpr (!AFF) {
+    uint32_t* y = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o);
+    if (NPLANES == 2) {
+      uint32_t hi, lo;
+      split_bf16x2(v0, v1, hi, lo);
+      y[0] = hi;
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
+    } else {
+      y[0] = pack_bf16x2(v0, v1);
+    }
   } else {
-    y[0] = pack_bf16x2(v0, v1);
+    uint32_t hi, lo = 0;
+    if (NPLANES == 2) split_bf16x2(v0, v1, hi, lo);
+    else hi = pack_bf16x2(v0, v1);
+    if (op.store_first) {
+      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o) = hi;
+      if (NPLANES == 2) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
+    }
+    float u0 = __uint_as_float(hi << 16), u1 = __uint_as_float(hi & 0xffff0000u);
+    if (NPLANES == 2) {
+      u0 = u0 + __uint_as_float(lo << 16);
+      u1 = u1 + __uint_as_float(lo & 0xffff0000u);
+    }
+    const float2 s2 = __ldg(reinterpret_cast<const float2*>(op.scale2 + c));
+    const float2 t2 = __ldg(reinterpret_cast<const float2*>(op.shift2 + c));
+    u0 = fmaf(u0, s2.x, t2.x);
+    u1 = fmaf(u1, s2.y, t2.y);
+    if (op.relu2) {
+      u0 = fmaxf(u0, 0.f);
+      u1 = fmaxf(u1, 0.f);
+    }
+    __nv_bfloat16* y2 = reinterpret_cast<__nv_bfloat16*>(op.y2) + o;
+    if (NPLANES == 2) {
+      uint32_t h2, l2;
+      split_bf16x2(u0, u1, h2, l2);
+      *reinterpret_cast<uint32_t*>(y2) = h2;
+      *reinterpret_cast<uint32_t*>(y2 + p.plane_out) = l2;
+    } else {
+      *reinterpret_cast<uint32_t*>(y2) = pack_bf16x2(u0, u1);
+    }
   }
 }
 
@@ -389,7 +432,7 @@ __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int
 // MODE 0: one (tile, split) per CTA: tile = (blockIdx.x, blockIdx.y), split = blockIdx.z (grid split-K or cluster split-K)
 // MODE 1: persistent grid: CTA b walks tiles b, b + gridDim.x, ... of one op
 // MODE 2: one cluster walks a run of ops; tiles are dealt round-robin to its CTAs, a cluster barrier separates ops
-template <int NPLANES, int BN, int MODE, bool U8 = false>
+template <int NPLANES, int BN, int MODE, bool U8 = false, bool AFF = false>
 __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stages, int pdl) {
   using L = Smem<NPLANES, BN>;
   constexpr int R = BN / 2;   // accumulator registers per consumer thread
@@ -586,8 +629,8 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
 #pragma unroll
       for (int q = 0; q < R / 4; ++q) {
         const int c = c_base + 8 * q + col_l;
-        if (valid0) epi_pair<NPLANES>(p, pix0, c, acc[4 * q], acc[4 * q + 1]);
-        if (valid1) epi_pair<NPLANES>(p, pix1, c, acc[4 * q + 2], acc[4 * q + 3]);
+        if (valid0) epi_pair<NPLANES, AFF>(p, op, pix0, c, acc[4 * q], acc[4 * q + 1]);
+        if (valid1) epi_pair<NPLANES, AFF>(p, op, pix1, c, acc[4 * q + 2], acc[4 * q + 3]);
       }
     }
 
@@ -620,8 +663,8 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
             a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
           }
           const int c = blockIdx.y * BN + 8 * q + 2 * (lane & 3);
-          if (valid0) epi_pair<NPLANES>(p, pix0, c, a.x, a.y);
-          if (valid1) epi_pair<NPLANES>(p, pix1, c, a.z, a.w);
+          if (valid0) epi_pair<NPLANES, AFF>(p, op, pix0, c, a.x, a.y);
+          if (valid1) epi_pair<NPLANES, AFF>(p, op, pix1, c, a.z, a.w);
         }
       }
       cluster_sync_all();   // no CTA may leave (and free its shared memory) while a peer still reads it
@@ -642,6 +685,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_umma_kernel(const __grid_
 template <int NPLANES, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
   conv_body<NPLANES, BN, 1>(ops, 1, stages, pdl);
+}
+
+// the same two executors with a folded affine op as a second epilogue output (MegaOp::y2)
+template <int NPLANES, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_umma_aff_kernel(const __grid_constant__ MegaOp op, int stages, int pdl) {
+  conv_body<NPLANES, BN, 0, false, true>(&op, 1, stages, pdl);
+}
+
+template <int NPLANES, int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_aff_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  conv_body<NPLANES, BN, 1, false, true>(ops, 1, stages, pdl);
 }
 
 // the fused stem reading a uint8 RGB image (Keras caffe preprocessing applied while the patch rows are built)
@@ -756,12 +810,18 @@ void fill_op(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, MegaOp* out) {
   kp.plane_out = (size_t)P.n * P.ho * P.wo * P.cout;
   op.m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
   op.n_tiles = P.cout / P.bn;
+  op.scale2 = P.scale2;
+  op.shift2 = P.shift2;
+  op.y2 = a.y2;
+  op.relu2 = P.relu2;
+  op.store_first = P.aff ? P.store_first : 1;
 }
 
-template <int NPLANES, int BN>
+template <int NPLANES, int BN, bool AFF = false>
 int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t st) {
   using L = Smem<NPLANES, BN>;
-  DEFER_TRY((set_smem_attr<conv_umma_kernel<NPLANES, BN>>()));
+  constexpr auto kernel = AFF ? &conv_umma_aff_kernel<NPLANES, BN> : &conv_umma_kernel<NPLANES, BN>;
+  DEFER_TRY((set_smem_attr<kernel>()));
   MegaOp op;
   fill_op(P, a, &op);
   // >= 2: a consumer releases a stage only once the NEXT k-block's wgmmas are issued (wgmma.wait_group 1)
@@ -792,10 +852,10 @@ int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t s
     }
     cfg.attrs = attr;
     cfg.numAttrs = na;
-    DEFER_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<NPLANES, BN>, op, stages, pdl));
+    DEFER_CUDA(cudaLaunchKernelEx(&cfg, kernel, op, stages, pdl));
     return DEFER_OK;
   }
-  conv_umma_kernel<NPLANES, BN><<<grid, NUM_THREADS, smem, st>>>(op, stages, 0);
+  kernel<<<grid, NUM_THREADS, smem, st>>>(op, stages, 0);
   DEFER_CUDA(cudaGetLastError());
   return DEFER_OK;
 }
@@ -803,11 +863,13 @@ int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t s
 // persistent grid over the tiles of one op in device memory: every CTA walks ceil(n_tiles / grid) tiles, so the launch
 // lasts `rounds` tile-times whatever the grid is; take the SMALLEST grid that still finishes in the minimum number of
 // rounds and leave the other SMs to the lanes running next to this one
-template <int NPLANES, int BN, bool U8 = false>
+template <int NPLANES, int BN, bool U8 = false, bool AFF = false>
 int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
   using L = Smem<NPLANES, BN>;
   static_assert(!U8 || BN == 64, "the uint8 stem runs with 64-wide N tiles");
-  constexpr auto kernel = U8 ? &conv_stem_u8_kernel<NPLANES> : &conv_stream_kernel<NPLANES, BN>;
+  static_assert(!(U8 && AFF), "no folded affine op on the stem");
+  constexpr auto kernel = U8 ? &conv_stem_u8_kernel<NPLANES>
+                             : (AFF ? &conv_stream_aff_kernel<NPLANES, BN> : &conv_stream_kernel<NPLANES, BN>);
   DEFER_TRY((set_smem_attr<kernel>()));
   if (stages > L::max_stages()) stages = L::max_stages();
   if (stages < 2) stages = 2;
@@ -1046,6 +1108,10 @@ void umma_conv_unbind(UmmaConvLaneArgs* a) {
 }
 
 int launch_conv_umma(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t st) {
+  if (P.aff) {
+    if (P.nplanes == 2) return P.bn == 128 ? launch_op_t<2, 128, true>(P, a, st) : launch_op_t<2, 64, true>(P, a, st);
+    return P.bn == 128 ? launch_op_t<1, 128, true>(P, a, st) : launch_op_t<1, 64, true>(P, a, st);
+  }
   if (P.nplanes == 2) return P.bn == 128 ? launch_op_t<2, 128>(P, a, st) : launch_op_t<2, 64>(P, a, st);
   return P.bn == 128 ? launch_op_t<1, 128>(P, a, st) : launch_op_t<1, 64>(P, a, st);
 }
@@ -1076,16 +1142,25 @@ int umma_mega_cluster_size() {
 }
 
 // ONE op on a persistent grid (many tiles: batched microbatches / large feature maps), 64-wide N tiles
-int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st) {
+int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, bool aff, cudaStream_t st) {
   const int stages = env_int("DEFER_PERSIST_STAGES", MAX_STAGES);
+  if (aff)
+    return nplanes == 2 ? launch_persist_t<2, 64, false, true>(dev_op, n_tiles, stages, st)
+                        : launch_persist_t<1, 64, false, true>(dev_op, n_tiles, stages, st);
   return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 
 // ONE op on the streaming persistent grid: every byte of shared memory goes to the operand ring (the epilogue runs from
 // the accumulator registers), so the producer keeps the next tile's operands in flight during this tile's epilogue
-int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, cudaStream_t st) {
+int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, bool aff, cudaStream_t st) {
   (void)k_blocks;
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
+  if (aff) {
+    if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128, false, true>(dev_op, n_tiles, stages, st)
+                                       : launch_persist_t<1, 128, false, true>(dev_op, n_tiles, stages, st);
+    if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64, false, true>(dev_op, n_tiles, stages, st)
+                                      : launch_persist_t<1, 64, false, true>(dev_op, n_tiles, stages, st);
+  }
   if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 128>(dev_op, n_tiles, stages, st);
   if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
   set_error("conv_stream: unsupported N tile %d", bn);

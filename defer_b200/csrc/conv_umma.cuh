@@ -25,6 +25,12 @@ struct UmmaConvPlan {
   void* w_dev = nullptr;   // transformed weights
   const float* scale = nullptr;
   const float* shift = nullptr;
+  // a standalone affine op folded into the epilogue (set by the caller after umma_conv_prepare): y2 = [relu](fmaf(stored, scale2, shift2))
+  bool aff = false;
+  const float* scale2 = nullptr;
+  const float* shift2 = nullptr;
+  int relu2 = 0;
+  int store_first = 1;     // 0: the conv's own output is not written (only the affine op's)
   CUtensorMap tmap_w[2];   // hi, lo
   bool ready = false;
 };
@@ -35,6 +41,7 @@ struct UmmaConvLaneArgs {
   bool direct_out = false;           // output lives in a peer GPU's slot (the epilogue's plain stores reach it)
   const void* res = nullptr;
   void* y = nullptr;
+  void* y2 = nullptr;                // output of the folded affine op (UmmaConvPlan::aff)
   float* partial = nullptr;          // split-K partial tiles (per lane: lanes run concurrently)
   unsigned int* counters = nullptr;  // split-K arrival counters, one per output tile
 };
@@ -55,7 +62,7 @@ int umma_mega_fill(void* host_dst, const UmmaConvPlan& plan, const UmmaConvLaneA
 int umma_mega_cluster_size();
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st);
 // one op on the streaming persistent kernel (deep operand ring, epilogue from the accumulator registers)
-int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, cudaStream_t st);
+int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, bool aff, cudaStream_t st);
 // fused stem: conv over a few-channel fp32 image with the im2col done inside the persistent kernel
 bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags);
 void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l);
@@ -64,6 +71,6 @@ void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, in
 void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]);
 int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, cudaStream_t st);
 // one op on a persistent grid (64-wide N tiles): for ops with many tiles
-int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, cudaStream_t st);
+int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, bool aff, cudaStream_t st);
 
 }  // namespace defer

@@ -94,8 +94,12 @@ struct OpRt {
   // Keras caffe preprocessing (DEFER_OP_PREPROCESS).  It is folded into the fused stem conv that reads its output when
   // that conv is its only reader; the op then launches nothing and its F32 image is never written.
   float pre_shift[3] = {0.f, 0.f, 0.f};   // PREPROCESS: host copy of the shift weights
-  int folded_into = -1;                   // PREPROCESS: index of the conv that applies it, -1 = runs preprocess_kernel
+  int folded_into = -1;                   // PREPROCESS / AFFINE: index of the conv that applies it, -1 = runs its own kernel
   int u8_pre = -1;                        // fused stem conv: index of the PREPROCESS op folded into it, -1 = none
+  // A standalone AFFINE(+ReLU) that reads a wgmma conv's output is folded into that conv's epilogue (DEFER_FOLD_AFFINE=1):
+  // the conv writes the affine op's output too, and its own output only when something else reads it.
+  int aff_op = -1;                        // wgmma conv: index of the AFFINE op folded into it, -1 = none
+  bool store_out = true;                  // ... false: the conv's own output buffer is never written
 };
 
 struct Lane {
@@ -208,8 +212,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
         if (op.stream)
           return launch_conv_stream(op.umma.nplanes, op.umma.bn, L.persist_op[oi],
                                     op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w * (op.umma.cout / op.umma.bn),
-                                    op.umma.k_blocks, st);
-        if (op.persist) return launch_conv_persistent(op.umma.nplanes, L.persist_op[oi], op.n_tiles64, st);
+                                    op.umma.k_blocks, op.aff_op >= 0, st);
+        if (op.persist) return launch_conv_persistent(op.umma.nplanes, L.persist_op[oi], op.n_tiles64, op.aff_op >= 0, st);
         return launch_conv_umma(op.umma, L.umma[oi], st);
       }
       ConvParams p;
@@ -236,6 +240,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
     case DEFER_OP_SOFTMAX:
       return launch_softmax((const float*)x, (float*)y, nb, bo.c, st);
     case DEFER_OP_AFFINE:
+      if (op.folded_into >= 0) return DEFER_OK;   // written by the conv's epilogue
+      [[fallthrough]];
     case DEFER_OP_RELU:
     case DEFER_OP_ADD:
       return launch_eltwise(fmt, d.kind, x, d.in1 >= 0 ? L.buf[d.in1] : nullptr, wptr(d.w_scale), wptr(d.w_shift), y,
@@ -605,6 +611,35 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     return fail(DEFER_ERR_INVALID);
   }
   for (auto& op : s->ops) op_costs(s, op);
+  // DEFER_FOLD_AFFINE=1: fold each AFFINE op whose input a wgmma conv of this stage writes into that conv (one per conv).
+  // The conv keeps its own store only when another op reads that buffer or it is the stage output.  The SIMT / F32 path
+  // keeps the standalone op, and so does the RGB stem.  Opt-in: measured on H100 the folded ResNet V2 step is slower
+  // (the epilogue's pair-wise stores are less coalesced than eltwise_kernel's float4 pass; BASELINE.md section 4).
+  {
+    const char* fe = getenv("DEFER_FOLD_AFFINE");
+    const bool fold = fe != nullptr && atoi(fe) != 0;
+    for (int ai = 0; fold && ai < n_ops; ++ai) {
+      OpRt& aff = s->ops[ai];
+      const defer_op_desc& d = aff.d;
+      if (d.kind != DEFER_OP_AFFINE || d.w_scale < 0 || d.w_shift < 0) continue;
+      const int ci = writer[d.in0];
+      if (ci < 0 || s->ops[ci].d.kind != DEFER_OP_CONV || s->ops[ci].backend != 2 || s->ops[ci].aff_op >= 0) continue;
+      OpRt& conv = s->ops[ci];
+      bool needed = d.in0 == cfg->output_buf;
+      for (int oi = 0; oi < n_ops; ++oi)
+        if (oi != ai && (ops[oi].in0 == d.in0 || ops[oi].in1 == d.in0)) needed = true;
+      aff.folded_into = ci;
+      aff.n_kernels = 0;
+      conv.aff_op = ai;
+      conv.store_out = needed;
+      conv.kname = "conv_umma_aff_kernel";
+      aff.kname = "affine (fused into " + conv.kname + ")";
+      conv.alg_bytes += aff.alg_bytes / 2;     // + the affine op's output (op_costs counted its input and output)
+      if (!needed) conv.alg_bytes -= aff.alg_bytes / 2;
+      aff.alg_bytes = 0;
+      if (s->output_writer == ai) s->output_writer = ci;   // HOP_TMA / HOP_DIRECT: wait for the slot before the conv
+    }
+  }
 
   // ---- arena: ctrl + input slots (exported to the upstream stage)
   size_t in_bytes = s->bufs[cfg->input_buf].bytes;
@@ -880,9 +915,10 @@ int defer_stage_finalize(defer_stage_t s) {
     const bool mega_on = e && atoi(e) != 0;   // cluster-chain megakernel: opt-in (wins only when launch-bound)
     int i = 0, n = (int)s->ops.size();
     while (mega_on && i < n) {
-      if (s->ops[i].backend != 2) { ++i; continue; }
+      // a conv carrying a folded AFFINE op ends a run and runs on its own (conv_mega_kernel has no second output)
+      if (s->ops[i].backend != 2 || s->ops[i].aff_op >= 0) { ++i; continue; }
       int j = i;
-      while (j + 1 < n && s->ops[j + 1].backend == 2) ++j;
+      while (j + 1 < n && s->ops[j + 1].backend == 2 && s->ops[j + 1].aff_op < 0) ++j;
       if (j > i) {
         defer_stage_s::MegaGroup g;
         g.first = i;
@@ -954,7 +990,17 @@ int defer_stage_finalize(defer_stage_t s) {
       break;
     }
     op.stream = op.persist && stream_bn > 0;
-    if (op.persist) op.kname = std::string(stem ? "stem_im2col+" : "") + (op.stream ? "conv_stream_kernel" : "conv_mega_kernel(grid)");
+    if (op.persist && op.aff_op >= 0) op.kname = op.stream ? "conv_stream_aff_kernel" : "conv_stream_aff_kernel(grid)";
+    else if (op.persist) op.kname = std::string(stem ? "stem_im2col+" : "") + (op.stream ? "conv_stream_kernel" : "conv_mega_kernel(grid)");
+    if (op.aff_op >= 0) {
+      const defer_op_desc& a = s->ops[op.aff_op].d;
+      op.umma.aff = true;
+      op.umma.scale2 = (const float*)s->d_weights[a.w_scale];
+      op.umma.shift2 = (const float*)s->d_weights[a.w_shift];
+      op.umma.relu2 = (a.flags & DEFER_FLAG_RELU) ? 1 : 0;
+      op.umma.store_first = op.store_out ? 1 : 0;
+      s->ops[op.aff_op].kname = "affine (fused into " + op.kname + ")";
+    }
     // fused stem: no patch matrix at all when the tile geometry allows it and the output stays on this GPU
     {
       const int fuse = getenv("DEFER_STEM_FUSED") ? atoi(getenv("DEFER_STEM_FUSED")) : 1;
@@ -982,6 +1028,7 @@ int defer_stage_finalize(defer_stage_t s) {
       }
       DEFER_TRY(umma_conv_bind(op.umma, &L.umma[oi], conv_in,
                                (d.flags & DEFER_FLAG_RESIDUAL) ? L.buf[d.in1] : nullptr, L.buf[d.out]));
+      if (op.aff_op >= 0) L.umma[oi].y2 = L.buf[s->ops[op.aff_op].d.out];
     }
   }
   // Fold a PREPROCESS op into the fused stem conv when that conv is the only reader of its (non-output) F32 image:
@@ -1255,10 +1302,16 @@ int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_o
   DEFER_TRY(set_device(s));
   void* src = s->lanes[lane].buf[buf_id];
   DEFER_CHECK(src, "read_buffer: buffer %d is not bound yet", buf_id);
-  for (size_t i = 0; i < s->ops.size(); ++i)
-    DEFER_CHECK(!(s->ops[i].d.out == buf_id && s->ops[i].folded_into >= 0),
+  for (size_t i = 0; i < s->ops.size(); ++i) {
+    const OpRt& op = s->ops[i];
+    if (op.d.out != buf_id) continue;
+    DEFER_CHECK(!(op.d.kind == DEFER_OP_PREPROCESS && op.folded_into >= 0),
                 "read_buffer: buffer %d is never written: op %zu (preprocess) is folded into op %d (%s)", buf_id, i,
-                s->ops[i].folded_into, s->ops[s->ops[i].folded_into].kname.c_str());
+                op.folded_into, op.folded_into >= 0 ? s->ops[op.folded_into].kname.c_str() : "");
+    DEFER_CHECK(op.store_out, "read_buffer: buffer %d is never written: op %zu (%s) stores only the output of the affine op %d "
+                "folded into it (no other op reads buffer %d; without DEFER_FOLD_AFFINE=1 it is written)", buf_id, i, op.kname.c_str(),
+                op.aff_op, buf_id);
+  }
   DEFER_CUDA(cudaStreamSynchronize(s->lanes[lane].stream));
   if (b.elem == DEFER_BUF_U8) {
     std::vector<uint8_t> raw(b.elems);
