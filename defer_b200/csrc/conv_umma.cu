@@ -13,9 +13,10 @@
 //     the fp32 accumulator lives in their registers.
 //   * BF16X2 format (fp32 parity path): activations and weights are (hi, lo) bf16 planes and each
 //     K = 16 step issues hi*hi + lo*hi + hi*lo (bf16x3, ~2^-16 relative) into the same accumulator.
-//   * Epilogue (the consumer warpgroups, straight from the accumulator registers): per-channel
-//     scale/shift (bias + BN) -> + residual -> relu -> re-split to bf16 planes -> st.global (plain
-//     stores, so the output may be a peer GPU's input slot: the hop is fused into the kernel).
+//   * Epilogue (the consumer warpgroups): the accumulator tile goes through a 32 KB shared-memory staging tile
+//     (after the operand ring) into whole rows; per-channel scale/shift (bias + BN) -> + residual -> relu ->
+//     re-split to bf16 planes -> 16-byte st.global (plain stores, so the output may be a peer GPU's input slot:
+//     the hop is fused into the kernel).
 //   * Split-K for weight-heavy small-M layers (7x7, 14x14 maps at batch 1): either partial tiles in an
 //     fp32 workspace reduced by the last-arriving CTA, or (DEFER_UMMA_CLUSTER=1) the splits of a tile as
 //     one thread-block cluster reducing through distributed shared memory.  Both sum in a fixed order.
@@ -51,6 +52,8 @@ constexpr int SMEM_CAP = 227 * 1024 - 256;   // opt-in shared memory per block o
 constexpr int CTL_BYTES = 256;         // mbarriers
 constexpr int MAX_STAGES = 8;
 constexpr int MEGA_BN = 64;
+constexpr int STG_COLS = 64;                    // epilogue staging tile: BM rows x 64 fp32 columns (a BN = 128 tile takes two passes)
+constexpr int STG_BYTES = BM * STG_COLS * 4;   // 32 KB, after the operand ring
 
 struct KParams {
   // geometry
@@ -105,12 +108,17 @@ struct Smem {
   __host__ __device__ static constexpr int ring(int stages, bool red) {
     return (red && stages * STAGE < RED) ? RED : stages * STAGE;
   }
-  // + slack for the manual 1024-B alignment of the dynamic smem base
-  __host__ __device__ static constexpr int total(int stages, bool red) { return ring(stages, red) + CTL_BYTES + 1024; }
+  // ring | epilogue staging tile | mbarriers, + slack for the manual 1024-B alignment of the dynamic smem base
+  __host__ __device__ static constexpr int total(int stages, bool red) {
+    return ring(stages, red) + STG_BYTES + CTL_BYTES + 1024;
+  }
   __host__ __device__ static constexpr int max_stages() {
-    return (SMEM_CAP - CTL_BYTES - 1024) / STAGE > MAX_STAGES ? MAX_STAGES : (SMEM_CAP - CTL_BYTES - 1024) / STAGE;
+    return (SMEM_CAP - STG_BYTES - CTL_BYTES - 1024) / STAGE > MAX_STAGES ? MAX_STAGES
+                                                                          : (SMEM_CAP - STG_BYTES - CTL_BYTES - 1024) / STAGE;
   }
 };
+static_assert(Smem<2, 128>::max_stages() == 3 && Smem<2, 64>::max_stages() == 4, "BF16X2 ring depths");
+static_assert(Smem<1, 64>::max_stages() == 8 && Smem<1, 128>::max_stages() == 6, "BF16 ring depths");
 
 // ---------------------------------------------------------------------------------------------- PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -276,71 +284,204 @@ __device__ __forceinline__ void row_to_pixel(const KParams& p, int r, int n0, in
   }
 }
 
-// bias/BN, residual, ReLU and the store of two adjacent channels (c, c + 1) of one output pixel.
-// AFF: then the folded affine op of MegaOp::scale2 etc. on the value as stored - hi + lo (BF16X2) or the bf16 (BF16),
-// exactly what eltwise_kernel<FMT, DEFER_OP_AFFINE> reads back - with the same fmaf, ReLU and split, into y2.  The folded
-// result is therefore bit-identical to the conv followed by the standalone affine op.
-template <int NPLANES, bool AFF = false>
-__device__ __forceinline__ void epi_pair(const KParams& p, const MegaOp& op, size_t pix, int c, float v0, float v1) {
-  const float2 sc = p.scale ? __ldg(reinterpret_cast<const float2*>(p.scale + c)) : make_float2(1.f, 1.f);
-  const float2 sf = p.shift ? __ldg(reinterpret_cast<const float2*>(p.shift + c)) : make_float2(0.f, 0.f);
-  v0 = fmaf(v0, sc.x, sf.x);
-  v1 = fmaf(v1, sc.y, sf.y);
-  const size_t o = pix * p.cout + c;
-  if (p.res) {
-    const __nv_bfloat16* r = reinterpret_cast<const __nv_bfloat16*>(p.res) + o;
-    const __nv_bfloat162 h = *reinterpret_cast<const __nv_bfloat162*>(r);
-    v0 += __low2float(h);
-    v1 += __high2float(h);
-    if (NPLANES == 2) {
-      const __nv_bfloat162 l = *reinterpret_cast<const __nv_bfloat162*>(r + p.plane_out);
-      v0 += __low2float(l);
-      v1 += __high2float(l);
-    }
+// ---- the epilogue: per-channel scale/shift (bias + BN) -> + residual -> ReLU -> split to the bf16 planes -> st.global
+// The operands it needs, read from the op once per tile.  MODE 1 / 2 read their op from device memory; a field read inside
+// the store loop would be re-read after every store (a generic store may alias the op), and each residual load would wait
+// for that re-read.
+struct EpiArgs {
+  const float* scale;
+  const float* shift;
+  const __nv_bfloat16* res;
+  __nv_bfloat16* y;
+  size_t plane;          // element offset of the lo plane (output and residual have the same shape)
+  int cout;
+  bool relu;
+  bool store_first;      // AFF: 0 = only y2 is written
+  bool relu2;
+  const float* scale2;   // AFF: folded affine op
+  const float* shift2;
+  __nv_bfloat16* y2;
+};
+
+__device__ __forceinline__ EpiArgs epi_args(const MegaOp& op) {
+  const KParams& p = op.p;
+  EpiArgs e;
+  e.scale = p.scale;
+  e.shift = p.shift;
+  e.res = reinterpret_cast<const __nv_bfloat16*>(p.res);
+  e.y = reinterpret_cast<__nv_bfloat16*>(p.y);
+  e.plane = p.plane_out;
+  e.cout = p.cout;
+  e.relu = (p.flags & DEFER_FLAG_RELU) != 0;
+  e.store_first = op.store_first != 0;
+  e.relu2 = op.relu2 != 0;
+  e.scale2 = op.scale2;
+  e.shift2 = op.shift2;
+  e.y2 = reinterpret_cast<__nv_bfloat16*>(op.y2);
+  return e;
+}
+
+// fp32 staging tile, 128 rows x 64 columns (256 B per row).  The 16-B chunk j of row r sits at chunk j ^ 2 (r & 7): the
+// fragment writes (a half-warp writes 4 rows x 8 columns, one float2 per lane) and the row reads (a quarter-warp reads
+// 8 chunks of one row, one float4 per lane) are then free of bank conflicts.
+__device__ __forceinline__ uint32_t stg_off(int r, int c) {
+  return (uint32_t)(r * STG_COLS + (((c >> 2) ^ ((r & 7) << 1)) << 2) + (c & 3)) * 4u;
+}
+__device__ __forceinline__ void sts2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b));
+}
+__device__ __forceinline__ float4 lds4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+// plain st.global (no cache hint, no TMA): the output may be a peer GPU's input slot (DEFER_HOP=direct|tma)
+__device__ __forceinline__ void stg4(void* p, uint4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
+}
+
+__device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+
+// The epilogue of one output tile, staged through shared memory in passes of 64 columns.
+//   phase 1: the consumers write their accumulator fragments into the staging tile;
+//   phase 2: thread t owns the 8 channels 8 (t % 8) .. + 7 of rows t / 8 + 32 k (k = 0..3).  It issues all of its residual
+//   loads (16 B per plane per row) before the barrier and uses them after it, and stores 16 B per plane per row, so a warp
+//   writes four whole 128-B row segments per plane.
+// Per element the arithmetic and its order are those of the conv's definition: fmaf(acc, scale, shift), + res_hi, + res_lo,
+// ReLU, split.  AFF then applies the folded affine op to the value as stored - hi + lo (BF16X2) or the bf16 (BF16), exactly
+// what eltwise_kernel<FMT, DEFER_OP_AFFINE> reads back - with the same fmaf, ReLU and split, into y2.  The folded result is
+// therefore bit-identical to the conv followed by the standalone affine op.
+// qmask: the 8-column groups q (acc[4q .. 4q + 3]) this CTA stores (cluster split-K: those it reduced; otherwise all).
+template <int NPLANES, int BN, bool AFF>
+__device__ __forceinline__ void epi_tile(const KParams& p, const EpiArgs& e, uint32_t stg, const float (&acc)[BN / 2],
+                                         uint32_t qmask, int c_base, int n0, int h0, int w0) {
+  const int tid = threadIdx.x;
+  const int lane = tid & 31;
+  const int row0 = (tid >> 7) * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);   // fragment rows row0, row0 + 8
+  const int col_l = 2 * (lane & 3);
+  const int jg = tid & 7;                                                   // phase-2 channel group
+  const int rb = tid >> 3;                                                  // phase-2 rows rb + 32 k
+  // the two chunks of a channel group, read in the order that spreads a quarter-warp over all 32 banks
+  const int ca = 2 * jg + ((jg >> 2) & 1), cb = ca ^ 1;
+  const bool swap = (jg >> 2) & 1;
+  size_t orow[4];
+  uint32_t vmask = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    bool v;
+    size_t pix;
+    row_to_pixel(p, rb + 32 * k, n0, h0, w0, v, pix);
+    orow[k] = pix * (size_t)e.cout;
+    vmask |= (uint32_t)v << k;
   }
-  if (p.flags & DEFER_FLAG_RELU) {
-    v0 = fmaxf(v0, 0.f);
-    v1 = fmaxf(v1, 0.f);
-  }
-  if constexpr (!AFF) {
-    uint32_t* y = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o);
-    if (NPLANES == 2) {
-      uint32_t hi, lo;
-      split_bf16x2(v0, v1, hi, lo);
-      y[0] = hi;
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
-    } else {
-      y[0] = pack_bf16x2(v0, v1);
+#pragma unroll
+  for (int P = 0; P < BN / STG_COLS; ++P) {
+    const bool mine = (qmask >> (8 * P + jg)) & 1u;
+    const int c = c_base + STG_COLS * P + 8 * jg;
+    cons_bar_sync();   // every consumer is done reading the staging tile (previous pass or previous tile)
+#pragma unroll
+    for (int qq = 0; qq < 8; ++qq) {
+      const int q = 8 * P + qq;
+      if (!((qmask >> q) & 1u)) continue;
+      sts2(stg + stg_off(row0, 8 * qq + col_l), acc[4 * q], acc[4 * q + 1]);
+      sts2(stg + stg_off(row0 + 8, 8 * qq + col_l), acc[4 * q + 2], acc[4 * q + 3]);
     }
-  } else {
-    uint32_t hi, lo = 0;
-    if (NPLANES == 2) split_bf16x2(v0, v1, hi, lo);
-    else hi = pack_bf16x2(v0, v1);
-    if (op.store_first) {
-      *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o) = hi;
-      if (NPLANES == 2) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.y) + o + p.plane_out) = lo;
+    // the residual and the per-channel operands: all loads of the pass are in flight across the barrier, before any is
+    // used (issued after the fragment writes, whose registers are free by then)
+    uint4 rh[4], rl[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      rh[k] = rl[k] = make_uint4(0u, 0u, 0u, 0u);
+      if (e.res && mine && ((vmask >> k) & 1u)) {
+        rh[k] = __ldcg(reinterpret_cast<const uint4*>(e.res + orow[k] + c));
+        if (NPLANES == 2) rl[k] = __ldcg(reinterpret_cast<const uint4*>(e.res + e.plane + orow[k] + c));
+      }
     }
-    float u0 = __uint_as_float(hi << 16), u1 = __uint_as_float(hi & 0xffff0000u);
-    if (NPLANES == 2) {
-      u0 = u0 + __uint_as_float(lo << 16);
-      u1 = u1 + __uint_as_float(lo & 0xffff0000u);
+    float sc[8], sf[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { sc[i] = 1.f; sf[i] = 0.f; }
+    if (mine) {
+      if (e.scale) {
+        const float4 a = __ldg(reinterpret_cast<const float4*>(e.scale + c));
+        const float4 b = __ldg(reinterpret_cast<const float4*>(e.scale + c + 4));
+        sc[0] = a.x; sc[1] = a.y; sc[2] = a.z; sc[3] = a.w; sc[4] = b.x; sc[5] = b.y; sc[6] = b.z; sc[7] = b.w;
+      }
+      if (e.shift) {
+        const float4 a = __ldg(reinterpret_cast<const float4*>(e.shift + c));
+        const float4 b = __ldg(reinterpret_cast<const float4*>(e.shift + c + 4));
+        sf[0] = a.x; sf[1] = a.y; sf[2] = a.z; sf[3] = a.w; sf[4] = b.x; sf[5] = b.y; sf[6] = b.z; sf[7] = b.w;
+      }
     }
-    const float2 s2 = __ldg(reinterpret_cast<const float2*>(op.scale2 + c));
-    const float2 t2 = __ldg(reinterpret_cast<const float2*>(op.shift2 + c));
-    u0 = fmaf(u0, s2.x, t2.x);
-    u1 = fmaf(u1, s2.y, t2.y);
-    if (op.relu2) {
-      u0 = fmaxf(u0, 0.f);
-      u1 = fmaxf(u1, 0.f);
-    }
-    __nv_bfloat16* y2 = reinterpret_cast<__nv_bfloat16*>(op.y2) + o;
-    if (NPLANES == 2) {
-      uint32_t h2, l2;
-      split_bf16x2(u0, u1, h2, l2);
-      *reinterpret_cast<uint32_t*>(y2) = h2;
-      *reinterpret_cast<uint32_t*>(y2 + p.plane_out) = l2;
-    } else {
-      *reinterpret_cast<uint32_t*>(y2) = pack_bf16x2(u0, u1);
+    cons_bar_sync();
+    if (!mine) continue;
+
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (!((vmask >> k) & 1u)) continue;
+      const int r = rb + 32 * k;
+      const float4 xa = lds4(stg + stg_off(r, 4 * ca));
+      const float4 xb = lds4(stg + stg_off(r, 4 * cb));
+      const float4 x0 = swap ? xb : xa, x1 = swap ? xa : xb;
+      float v[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+      const uint32_t hw[4] = {rh[k].x, rh[k].y, rh[k].z, rh[k].w};
+      const uint32_t lw[4] = {rl[k].x, rl[k].y, rl[k].z, rl[k].w};
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        v[i] = fmaf(v[i], sc[i], sf[i]);
+        if (e.res) {
+          v[i] += (i & 1) ? bf_hi(hw[i >> 1]) : bf_lo(hw[i >> 1]);
+          if (NPLANES == 2) v[i] += (i & 1) ? bf_hi(lw[i >> 1]) : bf_lo(lw[i >> 1]);
+        }
+        if (e.relu) v[i] = fmaxf(v[i], 0.f);
+      }
+      uint4 hi, lo = make_uint4(0u, 0u, 0u, 0u);
+      if (NPLANES == 2) {
+        split_bf16x2(v[0], v[1], hi.x, lo.x);
+        split_bf16x2(v[2], v[3], hi.y, lo.y);
+        split_bf16x2(v[4], v[5], hi.z, lo.z);
+        split_bf16x2(v[6], v[7], hi.w, lo.w);
+      } else {
+        hi = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+      }
+      const size_t o = orow[k] + c;
+      if (!AFF || e.store_first) {
+        stg4(e.y + o, hi);
+        if (NPLANES == 2) stg4(e.y + e.plane + o, lo);
+      }
+      if constexpr (AFF) {
+        float s2[8], t2[8];
+        {
+          const float4 a = __ldg(reinterpret_cast<const float4*>(e.scale2 + c));
+          const float4 b = __ldg(reinterpret_cast<const float4*>(e.scale2 + c + 4));
+          const float4 d = __ldg(reinterpret_cast<const float4*>(e.shift2 + c));
+          const float4 f = __ldg(reinterpret_cast<const float4*>(e.shift2 + c + 4));
+          s2[0] = a.x; s2[1] = a.y; s2[2] = a.z; s2[3] = a.w; s2[4] = b.x; s2[5] = b.y; s2[6] = b.z; s2[7] = b.w;
+          t2[0] = d.x; t2[1] = d.y; t2[2] = d.z; t2[3] = d.w; t2[4] = f.x; t2[5] = f.y; t2[6] = f.z; t2[7] = f.w;
+        }
+        const uint32_t sh[4] = {hi.x, hi.y, hi.z, hi.w};
+        const uint32_t sl[4] = {lo.x, lo.y, lo.z, lo.w};
+        float u[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          u[i] = (i & 1) ? bf_hi(sh[i >> 1]) : bf_lo(sh[i >> 1]);
+          if (NPLANES == 2) u[i] = u[i] + ((i & 1) ? bf_hi(sl[i >> 1]) : bf_lo(sl[i >> 1]));
+          u[i] = fmaf(u[i], s2[i], t2[i]);
+          if (e.relu2) u[i] = fmaxf(u[i], 0.f);
+        }
+        uint4 h2, l2;
+        if (NPLANES == 2) {
+          split_bf16x2(u[0], u[1], h2.x, l2.x);
+          split_bf16x2(u[2], u[3], h2.y, l2.y);
+          split_bf16x2(u[4], u[5], h2.z, l2.z);
+          split_bf16x2(u[6], u[7], h2.w, l2.w);
+          stg4(e.y2 + o, h2);
+          stg4(e.y2 + e.plane + o, l2);
+        } else {
+          h2 = make_uint4(pack_bf16x2(u[0], u[1]), pack_bf16x2(u[2], u[3]), pack_bf16x2(u[4], u[5]), pack_bf16x2(u[6], u[7]));
+          stg4(e.y2 + o, h2);
+        }
+      }
     }
   }
 }
@@ -440,7 +581,8 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const uint32_t ring = smem_u32(smem);
   const bool red = MODE == 0 && ops[0].p.cluster;
-  const uint32_t bar_base = ring + L::ring(stages, red);
+  const uint32_t stg = ring + L::ring(stages, red);   // epilogue staging tile, outside the ring
+  const uint32_t bar_base = stg + STG_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
   __shared__ int s_is_last;
@@ -579,12 +721,6 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
       // ===================================================================== consumers: epilogue
       // wgmma m64nN accumulator layout: register i of thread (warp w, lane l) of warpgroup g holds row
       // 64g + 16w + l/4 + 8*((i/2)&1), column 8*(i/4) + 2*(l%4) + (i&1)
-      const int row0 = wg * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);
-      const int col_l = 2 * (lane & 3);
-      bool valid0, valid1;
-      size_t pix0, pix1;
-      row_to_pixel(p, row0, n0, h0, w0, valid0, pix0);
-      row_to_pixel(p, row0 + 8, n0, h0, w0, valid1, pix1);
 
       if (MODE == 0 && p.cluster) {
         // ---- cluster split-K: the S CTAs of the cluster hold the S partial tiles of ONE output tile.  Each parks its
@@ -626,19 +762,12 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
           }
         }
       }
-#pragma unroll
-      for (int q = 0; q < R / 4; ++q) {
-        const int c = c_base + 8 * q + col_l;
-        if (valid0) epi_pair<NPLANES, AFF>(p, op, pix0, c, acc[4 * q], acc[4 * q + 1]);
-        if (valid1) epi_pair<NPLANES, AFF>(p, op, pix1, c, acc[4 * q + 2], acc[4 * q + 3]);
-      }
+      epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, 0xffffu, c_base, n0, h0, w0);
     }
 
     if (MODE == 0 && p.cluster) {
       cluster_sync_all();
       if (tid < CONS_THREADS) {
-        const int lane = tid & 31;
-        const int row0 = (tid >> 7) * 64 + ((tid >> 5) & 3) * 16 + (lane >> 2);
         const int m_tile = blockIdx.x;
         int n0 = 0, h0 = 0, w0 = 0;
         if (p.flat) {
@@ -649,23 +778,27 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
           h0 = (t2 % p.tiles_h) * p.tile_h;
           w0 = (m_tile % p.tiles_w) * p.tile_w;
         }
-        bool valid0, valid1;
-        size_t pix0, pix1;
-        row_to_pixel(p, row0, n0, h0, w0, valid0, pix0);
-        row_to_pixel(p, row0 + 8, n0, h0, w0, valid1, pix1);
+        // this CTA reduces and stores the column groups q = rank, rank + S, ...; the partials it reads over DSMEM sit at
+        // the start of each peer's ring, the staging tile after it, so peers may still be reading while this CTA stages
         const int S = p.splits;
+        const int rank = (int)cluster_ctarank();
         const uint32_t mine = ring + (uint32_t)tid * 16u;
-        for (int q = (int)cluster_ctarank(); q < R / 4; q += S) {
+        float acc[R];
+        uint32_t qmask = 0;
+#pragma unroll
+        for (int q = 0; q < R / 4; ++q) {
+          acc[4 * q] = acc[4 * q + 1] = acc[4 * q + 2] = acc[4 * q + 3] = 0.f;
+          if (q % S != rank) continue;
+          qmask |= 1u << q;
           const uint32_t addr = mine + (uint32_t)(q * CONS_THREADS) * 16u;
           float4 a = dsmem_ld4(dsmem_map(addr, 0));
           for (int s = 1; s < S; ++s) {
             const float4 v = dsmem_ld4(dsmem_map(addr, (uint32_t)s));
             a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
           }
-          const int c = blockIdx.y * BN + 8 * q + 2 * (lane & 3);
-          if (valid0) epi_pair<NPLANES, AFF>(p, op, pix0, c, a.x, a.y);
-          if (valid1) epi_pair<NPLANES, AFF>(p, op, pix1, c, a.z, a.w);
+          acc[4 * q] = a.x; acc[4 * q + 1] = a.y; acc[4 * q + 2] = a.z; acc[4 * q + 3] = a.w;
         }
+        epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, qmask, (int)blockIdx.y * BN, n0, h0, w0);
       }
       cluster_sync_all();   // no CTA may leave (and free its shared memory) while a peer still reads it
     }
@@ -1150,8 +1283,8 @@ int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, bool af
   return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 
-// ONE op on the streaming persistent grid: every byte of shared memory goes to the operand ring (the epilogue runs from
-// the accumulator registers), so the producer keeps the next tile's operands in flight during this tile's epilogue
+// ONE op on the streaming persistent grid: the epilogue stages through its own shared-memory tile, outside the operand
+// ring, so the producer keeps the next tile's operands in flight during this tile's epilogue
 int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, bool aff, cudaStream_t st) {
   (void)k_blocks;
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);

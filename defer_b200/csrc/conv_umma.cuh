@@ -61,7 +61,7 @@ size_t umma_mega_op_bytes();
 int umma_mega_fill(void* host_dst, const UmmaConvPlan& plan, const UmmaConvLaneArgs& args);   // one op descriptor
 int umma_mega_cluster_size();
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st);
-// one op on the streaming persistent kernel (deep operand ring, epilogue from the accumulator registers)
+// one op on the streaming persistent kernel (deep operand ring, epilogue staged outside it)
 int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, bool aff, cudaStream_t st);
 // fused stem: conv over a few-channel fp32 image with the im2col done inside the persistent kernel
 bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags);
