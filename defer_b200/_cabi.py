@@ -20,6 +20,8 @@ FMT_F32, FMT_BF16X2, FMT_BF16 = 0, 1, 2
 OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS = range(1, 12)
 FLAG_RELU, FLAG_RESIDUAL = 1, 2
 BUF_ACT, BUF_F32, BUF_U8 = 0, 1, 2
+PRE_CAFFE, PRE_TF = 0, 1
+PRE_MODES = {"caffe": PRE_CAFFE, "tf": PRE_TF}
 OK, ERR_INVALID, ERR_CUDA, ERR_TIMEOUT, ERR_STATE = 0, -1, -2, -3, -4
 
 FMT_NAMES = {FMT_F32: "f32", FMT_BF16X2: "bf16x2", FMT_BF16: "bf16"}
@@ -37,7 +39,7 @@ class OpDesc(C.Structure):
                 ("kh", C.c_int32), ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32),
                 ("pad_t", C.c_int32), ("pad_l", C.c_int32), ("pad_b", C.c_int32), ("pad_r", C.c_int32),
                 ("flags", C.c_uint32), ("w_kernel", C.c_int32), ("w_scale", C.c_int32), ("w_shift", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("mode", C.c_int32)]
 
 
 class StageConfig(C.Structure):
@@ -96,6 +98,7 @@ PROTOTYPES = {
     "defer_k_encode": (_i, [_i, _vp, _vp, _u64, _vp]),
     "defer_k_decode": (_i, [_i, _vp, _vp, _u64, _vp]),
     "defer_k_preprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "defer_k_preprocess_tf": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
 }
 
 _LIB = None

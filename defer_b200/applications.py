@@ -120,7 +120,9 @@ def synthetic_image(batch: int = 1, shape=(224, 224, 3), seed: int = 0) -> np.nd
 
 #: ImageNet channel means of Keras' caffe mode, in BGR order (keras_applications.imagenet_utils)
 CAFFE_MEAN_BGR = (103.939, 116.779, 123.68)
-PREPROCESS_MODES = ("caffe",)
+#: the ``preprocess=`` modes of DEFER / StageRunner / plan_stage: Keras' ``preprocess_input`` of ResNet50 / 101 / 152 and
+#: VGG16 ('caffe'), and of ResNet50V2 / 101V2 / 152V2 ('tf')
+PREPROCESS_MODES = ("caffe", "tf")
 
 
 def preprocess_input(x: np.ndarray, mode: str = "caffe") -> np.ndarray:
@@ -131,12 +133,27 @@ def preprocess_input(x: np.ndarray, mode: str = "caffe") -> np.ndarray:
     axis is reversed (RGB -> BGR) and the ImageNet mean is subtracted per channel in float32.  Returns a new float32
     array; ``x`` is not modified.  ``DEFER(..., preprocess="caffe")`` applies the same transform on the GPU.
     """
-    check_preprocess(mode)
+    if mode != "caffe":
+        raise ValueError(f"preprocess_input(mode={mode!r}): this function applies 'caffe' mode only; "
+                         "use resnet_v2_preprocess_input for 'tf' mode")
     x = np.asarray(x)
     if x.shape[-1] != 3:
         raise ValueError(f"preprocess_input: expected channels-last RGB (last axis 3), got shape {x.shape}")
     y = x[..., ::-1].astype(np.float32)          # astype copies: the caller's array is never touched
     y -= np.asarray(CAFFE_MEAN_BGR, np.float32)
+    return y
+
+
+def resnet_v2_preprocess_input(x: np.ndarray) -> np.ndarray:
+    """Keras ``preprocess_input`` of ResNet50V2 / ResNet101V2 / ResNet152V2 (tf mode).
+
+    Restates ``keras_applications.imagenet_utils._preprocess_numpy_input(x, mode='tf')``: non-float input becomes
+    float32, then ``x /= 127.5; x -= 1.`` in float32 - no channel flip, no mean.  Returns a new float32 array; ``x`` is
+    not modified.  ``DEFER(..., preprocess="tf")`` applies the same transform on the GPU, bit for bit.
+    """
+    y = np.asarray(x).astype(np.float32)        # astype copies: the caller's array is never touched
+    y /= np.float32(127.5)
+    y -= np.float32(1.0)
     return y
 
 
@@ -147,10 +164,22 @@ def caffe_shift() -> np.ndarray:
 
 def check_preprocess(mode) -> None:
     if mode not in PREPROCESS_MODES:
-        raise ValueError(f"preprocess={mode!r}: the supported mode is 'caffe' (Keras' preprocess_input of ResNet and VGG)")
+        raise ValueError(f"preprocess={mode!r}: the supported modes are 'caffe' (Keras' preprocess_input of ResNet50/101/152 "
+                         "and VGG16) and 'tf' (ResNet50V2/101V2/152V2)")
 
 
-def _finish(model: Model, weights: Optional[str], seed: int) -> Model:
+def check_model_preprocess(model, mode) -> None:
+    """Refuse ``preprocess="tf"`` on a model whose Keras ``preprocess_input`` is caffe mode (``model.preprocess_mode``,
+    recorded by the builders here).  A model without the record - a partition or one rebuilt from JSON - is not checked,
+    and ``"caffe"`` stays accepted everywhere."""
+    recorded = getattr(model, "preprocess_mode", None)
+    if mode == "tf" and recorded == "caffe":
+        raise ValueError(f"preprocess='tf': {model.name} is preprocessed in Keras' 'caffe' mode (RGB -> BGR, minus the "
+                         "ImageNet mean); pass preprocess='caffe'")
+
+
+def _finish(model: Model, weights: Optional[str], seed: int, preprocess_mode: str = "caffe") -> Model:
+    model.preprocess_mode = preprocess_mode     # the mode of this model's Keras preprocess_input
     if weights in ("synthetic", "imagenet"):
         # 'imagenet' is accepted for script compatibility (test/test.py:14) but cannot be
         # downloaded offline: synthetic weights are used and flagged on the model.
@@ -330,7 +359,7 @@ def _resnet_v2(blocks, model_name, weights, input_shape, classes, seed, fresh_na
     x = Activation("relu", name="post_relu")(x)
     x = GlobalAveragePooling2D(name="avg_pool")(x)
     x = Dense(classes, activation="softmax", name="predictions")(x)
-    return _finish(Model(img, x, name=model_name), weights, seed)
+    return _finish(Model(img, x, name=model_name), weights, seed, preprocess_mode="tf")
 
 
 def ResNet50V2(weights: Optional[str] = "synthetic", include_top: bool = True, input_shape=(224, 224, 3),

@@ -114,4 +114,11 @@ int defer_k_preprocess(const uint8_t* x, const float* shift, float* y, int n, in
   return launch_preprocess(x, shift, y, (size_t)n * h * w, (cudaStream_t)stream);
 }
 
+int defer_k_preprocess_tf(const uint8_t* x, float* y, int n, int h, int w, int c, void* stream) {
+  DEFER_CHECK(x && y, "k_preprocess_tf: null pointer");
+  DEFER_CHECK(n >= 1 && h >= 1 && w >= 1, "k_preprocess_tf: empty image (%d,%d,%d)", n, h, w);
+  DEFER_CHECK(c == 3, "k_preprocess_tf: preprocessing needs 3 channels (RGB), got %d", c);
+  return launch_preprocess_tf(x, y, (size_t)n * h * w, (cudaStream_t)stream);
+}
+
 }  // extern "C"

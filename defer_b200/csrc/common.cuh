@@ -117,6 +117,19 @@ __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uin
   lo = pack_bf16x2(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
 }
 
+// Keras 'tf'-mode preprocess_input of one byte value b (0..255, exact in fp32): fl32(fl32(b / 127.5) - 1), bit for bit,
+// without a division (__fdiv_rn carries a called slow path, which the wgmma kernels must not contain).  q = b * r with
+// r = fl32(1 / 127.5) is off by one ulp for 111 of the 256 bytes; one exact remainder e = b - q * 127.5 (a single FMA)
+// and one correction q + e * r give the correctly rounded quotient for all 256.  Every step is an explicit _rn
+// intrinsic, so nvcc cannot contract or reorder it: FMUL, FFMA, FFMA, FADD.
+__device__ __forceinline__ float keras_tf_preprocess(float b) {
+  const float r = __uint_as_float(0x3C008081u);   // fl32(1 / 127.5)
+  float q = __fmul_rn(b, r);
+  const float e = __fmaf_rn(-q, 127.5f, b);
+  q = __fmaf_rn(e, r, q);
+  return __fsub_rn(q, 1.0f);
+}
+
 template <int FMT>
 __device__ __forceinline__ void act_store4(void* __restrict__ base, size_t plane, size_t i, float4 v) {
   if constexpr (FMT == FMT_F32) {
@@ -176,6 +189,8 @@ int launch_copy_act(int fmt, const void* x, void* y, size_t n_elems, cudaStream_
 int launch_f32_to_bf16(const float* x, void* y, size_t n, cudaStream_t st);
 // Keras caffe preprocess_input: uint8 RGB (n_pix pixels x 3) -> fp32 BGR + shift (DEFER_OP_PREPROCESS)
 int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_pix, cudaStream_t st);
+// Keras tf preprocess_input: uint8 RGB (n_pix pixels x 3) -> fp32 b / 127.5 - 1, channels kept (DEFER_PRE_TF)
+int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

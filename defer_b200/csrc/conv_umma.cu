@@ -86,7 +86,8 @@ struct alignas(128) MegaOp {
   const float* stem_x;
   int stem_h, stem_w, stem_cin, stem_kh, stem_kw, stem_sh, stem_sw, stem_pad_t, stem_pad_l, stem_K;
   // fused stem over a uint8 RGB image instead (conv_stem_u8_kernel): Keras caffe preprocessing on the fly,
-  // value[c] = float(image[2 - c]) + stem_shift[c]
+  // value[c] = float(image[2 - c]) + stem_shift[c]; or Keras tf preprocessing (conv_stem_u8tf_kernel, stem_shift unused),
+  // value[c] = float(image[c]) / 127.5 - 1
   const uint8_t* stem_u8;
   float stem_shift[3];
   // second epilogue output (conv_umma_aff_kernel / conv_stream_aff_kernel): a standalone per-channel affine(+ReLU) of
@@ -496,8 +497,11 @@ __device__ __forceinline__ void epi_tile(const KParams& p, const EpiArgs& e, uin
 // has channel k % 3: the eight taps of a chunk see a rotation of (0, 1, 2), so the mirrored-channel offset and the shift
 // are chosen once per chunk.  float(byte) is exact via the 2^23 magic number, then one rounded add: the same value the
 // standalone preprocess_kernel writes.
-template <int NPLANES, bool U8>
+// U8 && TF: Keras tf mode instead - channel c <- image channel c, keras_tf_preprocess(float(byte)), no shift: the same
+// value preprocess_tf_kernel writes.  The loads are issued the same way; there is no channel rotation to track.
+template <int NPLANES, bool U8, bool TF = false>
 __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int m0, int kb, int r) {
+  static_assert(U8 || !TF, "tf preprocessing reads a uint8 image");
   using In = std::conditional_t<U8, uint8_t, float>;
   const KParams& p = op.p;
   const int m = m0 + r;
@@ -525,7 +529,21 @@ __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int
 #pragma unroll 1
   for (int ch = 0; ch < 8; ++ch) {
     float v[8];
-    if constexpr (U8) {
+    if constexpr (TF) {
+      uint32_t raw[8];
+      bool in[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int ih = ih0 + a, col = col0 + jj;
+        in[e] = img && k < K && ih >= 0 && ih < H && col >= 0 && col < wc;
+        raw[e] = in[e] ? (uint32_t)__ldg(img + (size_t)ih * wc + col) : 0u;
+        ++k;
+        if (++jj == run) { jj = 0; ++a; }
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        v[e] = in[e] ? keras_tf_preprocess(__fsub_rn(__uint_as_float(0x4B000000u | raw[e]), 8388608.f)) : 0.f;
+    } else if constexpr (U8) {
       const float sr[3] = {c0 == 0 ? s0 : (c0 == 1 ? s1 : s2), c0 == 0 ? s1 : (c0 == 1 ? s2 : s0),
                            c0 == 0 ? s2 : (c0 == 1 ? s0 : s1)};
       const int mr[3] = {2 - 2 * c0, c0 == 2 ? 2 : -2 * c0, c0 == 0 ? -2 : 4 - 2 * c0};   // 2 - 2 * ((c0 + i) % 3)
@@ -573,7 +591,7 @@ __device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int
 // MODE 0: one (tile, split) per CTA: tile = (blockIdx.x, blockIdx.y), split = blockIdx.z (grid split-K or cluster split-K)
 // MODE 1: persistent grid: CTA b walks tiles b, b + gridDim.x, ... of one op
 // MODE 2: one cluster walks a run of ops; tiles are dealt round-robin to its CTAs, a cluster barrier separates ops
-template <int NPLANES, int BN, int MODE, bool U8 = false, bool AFF = false>
+template <int NPLANES, int BN, int MODE, bool U8 = false, bool AFF = false, bool TF = false>
 __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stages, int pdl) {
   using L = Smem<NPLANES, BN>;
   constexpr int R = BN / 2;   // accumulator registers per consumer thread
@@ -658,7 +676,7 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
                 tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
                 if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
               }
-              stem_build<NPLANES, U8>(op, a_dst, w0, kb, ptid);
+              stem_build<NPLANES, U8, TF>(op, a_dst, w0, kb, ptid);
               asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
               prod_bar_sync();
               if (ptid == 0) mbar_arrive(full_bar(stage));
@@ -837,6 +855,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8_kernel(const Mega
   conv_body<NPLANES, 64, 1, true>(ops, 1, stages, pdl);
 }
 
+// ... preprocessing it in Keras tf mode instead
+template <int NPLANES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8tf_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  conv_body<NPLANES, 64, 1, true, false, true>(ops, 1, stages, pdl);
+}
+
 template <int NPLANES>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_mega_kernel(const MegaOp* __restrict__ ops, int n_ops, int stages) {
   conv_body<NPLANES, MEGA_BN, 2>(ops, n_ops, stages, 0);
@@ -996,12 +1020,13 @@ int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t s
 // persistent grid over the tiles of one op in device memory: every CTA walks ceil(n_tiles / grid) tiles, so the launch
 // lasts `rounds` tile-times whatever the grid is; take the SMALLEST grid that still finishes in the minimum number of
 // rounds and leave the other SMs to the lanes running next to this one
-template <int NPLANES, int BN, bool U8 = false, bool AFF = false>
+template <int NPLANES, int BN, bool U8 = false, bool AFF = false, bool TF = false>
 int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
   using L = Smem<NPLANES, BN>;
   static_assert(!U8 || BN == 64, "the uint8 stem runs with 64-wide N tiles");
   static_assert(!(U8 && AFF), "no folded affine op on the stem");
-  constexpr auto kernel = U8 ? &conv_stem_u8_kernel<NPLANES>
+  static_assert(U8 || !TF, "tf preprocessing reads a uint8 image");
+  constexpr auto kernel = U8 ? (TF ? &conv_stem_u8tf_kernel<NPLANES> : &conv_stem_u8_kernel<NPLANES>)
                              : (AFF ? &conv_stream_aff_kernel<NPLANES, BN> : &conv_stream_kernel<NPLANES, BN>);
   DEFER_TRY((set_smem_attr<kernel>()));
   if (stages > L::max_stages()) stages = L::max_stages();
@@ -1323,8 +1348,11 @@ void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]
   for (int c = 0; c < 3; ++c) op->stem_shift[c] = shift[c];
 }
 
-int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, cudaStream_t st) {
+int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, bool tf, cudaStream_t st) {
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
+  if (u8 && tf)
+    return nplanes == 2 ? launch_persist_t<2, 64, true, false, true>(dev_op, n_tiles, stages, st)
+                        : launch_persist_t<1, 64, true, false, true>(dev_op, n_tiles, stages, st);
   if (u8)
     return nplanes == 2 ? launch_persist_t<2, 64, true>(dev_op, n_tiles, stages, st)
                         : launch_persist_t<1, 64, true>(dev_op, n_tiles, stages, st);

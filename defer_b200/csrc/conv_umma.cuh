@@ -67,9 +67,10 @@ int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int
 bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags);
 void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l);
 // ... reading a uint8 RGB image instead, preprocessed on the fly (after umma_mega_set_stem): channel c of the conv input
-// is float(image[.., 2 - c]) + shift[c]
+// is float(image[.., 2 - c]) + shift[c] (Keras caffe mode), or with tf float(image[.., c]) / 127.5 - 1 (Keras tf mode,
+// shift unused)
 void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]);
-int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, cudaStream_t st);
+int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, bool tf, cudaStream_t st);
 // one op on a persistent grid (64-wide N tiles): for ops with many tiles
 int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, bool aff, cudaStream_t st);
 

@@ -1116,13 +1116,18 @@ int launch_copy_act(int fmt, const void* x, void* y, size_t n, cudaStream_t st) 
   return DEFER_OK;
 }
 
-// Keras caffe-mode preprocess_input on a uint8 RGB image: y[p, c] = float(x[p, 2 - c]) + shift[c], one exactly rounded
-// fp32 add per element (shift = -mean, so this is the host's float32(x) - mean bit for bit).  VEC: a thread reads four
-// pixels as three 32-bit words and writes them as three float4; the last n_pix % 4 pixels go one per thread.
-template <bool VEC>
-__global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restrict__ x, const float* __restrict__ shift,
-                                                         float* __restrict__ y, size_t n_pix) {
-  const float s0 = __ldg(shift), s1 = __ldg(shift + 1), s2 = __ldg(shift + 2);
+// Keras preprocess_input on a uint8 RGB image.  Caffe mode (TF false): y[p, c] = float(x[p, 2 - c]) + shift[c], one
+// exactly rounded fp32 add per element (shift = -mean, so this is the host's float32(x) - mean bit for bit).  Tf mode
+// (TF true, shift unused): y[p, c] = keras_tf_preprocess(float(x[p, c])), the host's float32(x) / 127.5 - 1 bit for bit.
+// VEC: a thread reads four pixels as three 32-bit words and writes them as three float4; the last n_pix % 4 pixels go
+// one per thread.
+template <bool VEC, bool TF>
+__device__ __forceinline__ void preprocess_body(const uint8_t* __restrict__ x, const float* __restrict__ shift,
+                                                float* __restrict__ y, size_t n_pix) {
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  if constexpr (!TF) {
+    s0 = __ldg(shift); s1 = __ldg(shift + 1); s2 = __ldg(shift + 2);
+  }
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (VEC) {
     const size_t groups = n_pix / 4;
@@ -1132,11 +1137,16 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restri
       float b[12], o[12];
 #pragma unroll
       for (int j = 0; j < 12; ++j) b[j] = (float)((wd[j >> 2] >> (8 * (j & 3))) & 0xffu);
+      if constexpr (TF) {
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        o[3 * q] = __fadd_rn(b[3 * q + 2], s0);
-        o[3 * q + 1] = __fadd_rn(b[3 * q + 1], s1);
-        o[3 * q + 2] = __fadd_rn(b[3 * q], s2);
+        for (int j = 0; j < 12; ++j) o[j] = keras_tf_preprocess(b[j]);
+      } else {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          o[3 * q] = __fadd_rn(b[3 * q + 2], s0);
+          o[3 * q + 1] = __fadd_rn(b[3 * q + 1], s1);
+          o[3 * q + 2] = __fadd_rn(b[3 * q], s2);
+        }
       }
       float4* yv = reinterpret_cast<float4*>(y) + 3 * i;
       yv[0] = make_float4(o[0], o[1], o[2], o[3]);
@@ -1149,9 +1159,25 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restri
   if (i >= n_pix) return;
   const uint8_t* px = x + 3 * i;
   float* py = y + 3 * i;
-  py[0] = __fadd_rn((float)px[2], s0);
-  py[1] = __fadd_rn((float)px[1], s1);
-  py[2] = __fadd_rn((float)px[0], s2);
+  if constexpr (TF) {
+    py[0] = keras_tf_preprocess((float)px[0]);
+    py[1] = keras_tf_preprocess((float)px[1]);
+    py[2] = keras_tf_preprocess((float)px[2]);
+  } else {
+    py[0] = __fadd_rn((float)px[2], s0);
+    py[1] = __fadd_rn((float)px[1], s1);
+    py[2] = __fadd_rn((float)px[0], s2);
+  }
+}
+template <bool VEC>
+__global__ void __launch_bounds__(256) preprocess_kernel(const uint8_t* __restrict__ x, const float* __restrict__ shift,
+                                                         float* __restrict__ y, size_t n_pix) {
+  preprocess_body<VEC, false>(x, shift, y, n_pix);
+}
+template <bool VEC>
+__global__ void __launch_bounds__(256) preprocess_tf_kernel(const uint8_t* __restrict__ x, float* __restrict__ y,
+                                                            size_t n_pix) {
+  preprocess_body<VEC, true>(x, nullptr, y, n_pix);
 }
 int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_pix, cudaStream_t st) {
   if (n_pix == 0) return DEFER_OK;
@@ -1164,6 +1190,21 @@ int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_p
   } else {
     prefer_max_smem(preprocess_kernel<false>);
     preprocess_kernel<false><<<grid, 256, 0, st>>>(x, shift, y, n_pix);
+  }
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t st) {
+  if (n_pix == 0) return DEFER_OK;
+  const bool vec = reinterpret_cast<uintptr_t>(x) % 4 == 0 && reinterpret_cast<uintptr_t>(y) % 16 == 0;
+  const size_t threads = vec ? n_pix / 4 + n_pix % 4 : n_pix;
+  const unsigned grid = (unsigned)((threads + 255) / 256);
+  if (vec) {
+    prefer_max_smem(preprocess_tf_kernel<true>);
+    preprocess_tf_kernel<true><<<grid, 256, 0, st>>>(x, y, n_pix);
+  } else {
+    prefer_max_smem(preprocess_tf_kernel<false>);
+    preprocess_tf_kernel<false><<<grid, 256, 0, st>>>(x, y, n_pix);
   }
   DEFER_CUDA(cudaGetLastError());
   return DEFER_OK;

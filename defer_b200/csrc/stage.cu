@@ -91,9 +91,9 @@ struct OpRt {
   std::string kname;
   double alg_bytes = 0, alg_flops = 0;
   int n_kernels = 1;
-  // Keras caffe preprocessing (DEFER_OP_PREPROCESS).  It is folded into the fused stem conv that reads its output when
+  // Keras preprocessing (DEFER_OP_PREPROCESS, caffe or tf mode).  It is folded into the fused stem conv that reads its output when
   // that conv is its only reader; the op then launches nothing and its F32 image is never written.
-  float pre_shift[3] = {0.f, 0.f, 0.f};   // PREPROCESS: host copy of the shift weights
+  float pre_shift[3] = {0.f, 0.f, 0.f};   // PREPROCESS, caffe: host copy of the shift weights (tf has none)
   int folded_into = -1;                   // PREPROCESS / AFFINE: index of the conv that applies it, -1 = runs its own kernel
   int u8_pre = -1;                        // fused stem conv: index of the PREPROCESS op folded into it, -1 = none
   // A standalone AFFINE(+ReLU) that reads a wgmma conv's output is folded into that conv's epilogue (DEFER_FOLD_AFFINE=1):
@@ -204,7 +204,7 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
     case DEFER_OP_CONV: {
       if (op.backend == 4 && op.stem_fused)
         return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w,
-                                op.u8_pre >= 0, st);
+                                op.u8_pre >= 0, op.u8_pre >= 0 && s->ops[op.u8_pre].d.mode == DEFER_PRE_TF, st);
       if (op.backend == 4)
         DEFER_TRY(launch_stem_im2col(fmt, (const float*)x, L.im2col[oi], nb, bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t,
                                      d.pad_l, bo.h, bo.w, op.k_pad, st));
@@ -260,6 +260,7 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       return launch_decode(fmt, x, (float*)y, bi.elems, st);
     case DEFER_OP_PREPROCESS:
       if (op.folded_into >= 0) return DEFER_OK;   // applied by the stem conv as it reads the image
+      if (d.mode == DEFER_PRE_TF) return launch_preprocess_tf((const uint8_t*)x, (float*)y, (size_t)nb * bi.h * bi.w, st);
       return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
   }
   set_error("launch_op: unknown op kind %d", d.kind);
@@ -490,6 +491,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       set_error("op %d: only a PREPROCESS op may read the U8 input buffer (as in0)", i);
       return fail(DEFER_ERR_INVALID);
     }
+    if (d.kind != DEFER_OP_PREPROCESS && d.mode != 0) {
+      set_error("op %d: mode %d is meaningful only on a PREPROCESS op and must be 0 here", i, d.mode);
+      return fail(DEFER_ERR_INVALID);
+    }
     switch (d.kind) {
       case DEFER_OP_CONV: {
         int ho = (bi.h + d.pad_t + d.pad_b - d.kh) / d.sh + 1, wo = (bi.w + d.pad_l + d.pad_r - d.kw) / d.sw + 1;
@@ -578,7 +583,11 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         }
         break;
       case DEFER_OP_PREPROCESS:
-        op.kname = "preprocess_kernel";
+        if (d.mode != DEFER_PRE_CAFFE && d.mode != DEFER_PRE_TF) {
+          set_error("op %d (preprocess): unknown mode %d (caffe %d, tf %d)", i, d.mode, DEFER_PRE_CAFFE, DEFER_PRE_TF);
+          return fail(DEFER_ERR_INVALID);
+        }
+        op.kname = d.mode == DEFER_PRE_TF ? "preprocess_tf_kernel" : "preprocess_kernel";
         if (bi.elem != DEFER_BUF_U8 || bi.c != 3) {
           set_error("op %d (preprocess): input must be a U8 buffer with 3 channels (elem %d, c %d)", i, bi.elem, bi.c);
           return fail(DEFER_ERR_INVALID);
@@ -586,6 +595,14 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         if (bo.elem != DEFER_BUF_F32 || bo.h != bi.h || bo.w != bi.w || bo.c != bi.c) {
           set_error("op %d (preprocess): output must be an F32 buffer of the input's shape", i);
           return fail(DEFER_ERR_INVALID);
+        }
+        if (d.mode == DEFER_PRE_TF) {   // Keras hard-codes 127.5 and 1: nothing to upload
+          if (d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0) {
+            set_error("op %d (preprocess, tf): takes no weights (w_kernel %d, w_scale %d, w_shift %d)", i, d.w_kernel,
+                      d.w_scale, d.w_shift);
+            return fail(DEFER_ERR_INVALID);
+          }
+          break;
         }
         if (d.w_shift < 0 || s->weight_bytes[d.w_shift] != 3 * sizeof(float)) {
           set_error("op %d (preprocess): w_shift must hold 3 fp32 values", i);
@@ -1032,7 +1049,8 @@ int defer_stage_finalize(defer_stage_t s) {
     }
   }
   // Fold a PREPROCESS op into the fused stem conv when that conv is the only reader of its (non-output) F32 image:
-  // the stem then reads the uint8 image and preprocesses each tap itself.  Every other path runs preprocess_kernel.
+  // the stem then reads the uint8 image and preprocesses each tap itself.  Every other path runs preprocess_kernel
+  // (preprocess_tf_kernel in tf mode).
   for (int pi = 0; pi < (int)s->ops.size(); ++pi) {
     OpRt& pre = s->ops[pi];
     if (pre.d.kind != DEFER_OP_PREPROCESS || pre.d.out == s->cfg.output_buf) continue;
@@ -1049,7 +1067,7 @@ int defer_stage_finalize(defer_stage_t s) {
     pre.n_kernels = 0;
     pre.alg_bytes = 0;
     conv.u8_pre = pi;
-    conv.kname = "conv_stem_u8_kernel";
+    conv.kname = pre.d.mode == DEFER_PRE_TF ? "conv_stem_u8tf_kernel" : "conv_stem_u8_kernel";
     pre.kname = "preprocess (fused into " + conv.kname + ")";
     conv.alg_bytes -= (double)s->bufs[pre.d.in0].elems * 3.0;   // the image is read at 1 B/elem instead of 4
   }

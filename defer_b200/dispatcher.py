@@ -20,7 +20,9 @@ Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the ho
 (``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
 (``img_to_array(img).astype(np.uint8)``, shape ``(batch, h, w, 3)``) and the first stage applies the transform on its
 GPU, bit for bit what ``applications.preprocess_input`` gives on the host; an image crosses PCIe at 1 B per value
-instead of 4.  Other item dtypes are refused.
+instead of 4.  ``preprocess="tf"`` does the same with the ResNet V2 family's transform
+(``applications.resnet_v2_preprocess_input``), and is refused for a model whose Keras preprocessing is caffe mode.
+Other item dtypes are refused.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -39,7 +41,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import keras_like as K
-from .applications import check_preprocess
+from .applications import check_model_preprocess, check_preprocess
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
 
@@ -51,7 +53,7 @@ class DEFER:
         if preprocess is not None:
             check_preprocess(preprocess)
         self.computeNodes = list(computeNodes)
-        self.preprocess = preprocess        # None | "caffe": uint8 queue items, preprocessed on stage 0's GPU
+        self.preprocess = preprocess        # None | "caffe" | "tf": uint8 queue items, preprocessed on stage 0's GPU
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -243,6 +245,7 @@ class DEFER:
     def run_defer(self, model: K.Model, partition_layers, input_stream: queue.Queue, output_stream: queue.Queue):
         if self.batch is None:
             self.batch = 1
+        check_model_preprocess(model, self.preprocess)   # the partitions no longer know which model they came from
         models_to_dispatch = self._partition(model, partition_layers)
         # the last stage has `depth` result buffers (one process) / the result ring and every stage's lanes bound the
         # chain (one process per GPU): more microbatches in flight than that would overwrite a result before it is read

@@ -74,8 +74,11 @@ class StageRunner:
                     f"device {self.device}: {used} lane streams already live, {self.depth} more would exceed "
                     f"{MAX_STREAMS_PER_DEVICE} hardware work queues - flag-waiting lanes could block their own "
                     "producer.  Use fewer stages per GPU or a smaller depth.")
-        # a stage planned with preprocess= takes uint8 images (Keras caffe preprocessing runs on the GPU)
+        # a stage planned with preprocess= takes uint8 images (Keras preprocessing in that mode runs on the GPU)
         self.in_dtype = np.uint8 if plan.bufs[plan.input_buf][3] == A.BUF_U8 else np.float32
+        # the Keras mode of the stage's PREPROCESS op, for messages (None: no preprocessing; the library refuses a bad mode)
+        pre_modes = [o.mode for o in plan.ops if o.kind == A.OP_PREPROCESS]
+        self.preprocess = {v: k for k, v in A.PRE_MODES.items()}.get(pre_modes[0]) if pre_modes else None
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
         self.out_elems = int(np.prod(self.out_shape))
@@ -90,7 +93,7 @@ class StageRunner:
             t, l, b, r = o.pads
             ops[i] = A.OpDesc(kind=o.kind, in0=o.in0, in1=o.in1, out=o.out, kh=o.kh, kw=o.kw, sh=o.sh, sw=o.sw,
                               pad_t=t, pad_l=l, pad_b=b, pad_r=r, flags=o.flags, w_kernel=o.w_kernel,
-                              w_scale=o.w_scale, w_shift=o.w_shift, reserved=0)
+                              w_scale=o.w_scale, w_shift=o.w_shift, mode=o.mode)
         n_w = len(plan.weights)
         wptrs = (C.c_void_p * max(n_w, 1))(*[w.ctypes.data for w in plan.weights])
         wbytes = (C.c_uint64 * max(n_w, 1))(*[w.nbytes for w in plan.weights])
@@ -105,8 +108,8 @@ class StageRunner:
     def from_model(cls, model: K.Model, device=0, dtype: str = "float32", max_batch: int = 1, depth: int = 1,
                    is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
                    **kw) -> "StageRunner":
-        """``preprocess="caffe"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the stage
-        applies Keras' caffe ``preprocess_input`` on the GPU."""
+        """``preprocess="caffe"`` or ``"tf"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the
+        stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family)."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
@@ -149,7 +152,8 @@ class StageRunner:
         and neither can be told apart from the other."""
         if self.in_dtype == np.uint8:
             if getattr(x, "dtype", None) != np.uint8:
-                raise TypeError(f"{self.name}: this stage preprocesses uint8 RGB images on the GPU (preprocess='caffe') "
+                raise TypeError(f"{self.name}: this stage preprocesses uint8 RGB images on the GPU "
+                                f"(preprocess={self.preprocess!r}) "
                                 f"and got dtype {getattr(x, 'dtype', type(x).__name__)}; pass the image as "
                                 "img_to_array(img).astype(np.uint8), not preprocessed or float data")
             if x.ndim != 4 or tuple(x.shape[1:]) != self.in_shape[1:]:   # e.g. channels-first: same bytes, wrong image

@@ -15,9 +15,9 @@ executable form is a short list of fused ops (``include/defer_b200.h``):
 A follower is absorbed only when the tensor between the two layers has exactly one consumer and is
 not the stage output - otherwise that tensor must exist in memory.
 
-With ``preprocess="caffe"`` (first stage only) the stage input is a uint8 RGB image and a ``PREPROCESS`` op
-(Keras' caffe ``preprocess_input``) writes the fp32 tensor the rest of the plan reads; the library folds it
-into the fused RGB stem when it can.
+With ``preprocess="caffe"`` or ``"tf"`` (first stage only) the stage input is a uint8 RGB image and a
+``PREPROCESS`` op (Keras' ``preprocess_input`` in that mode) writes the fp32 tensor the rest of the plan reads;
+the library folds it into the fused RGB stem when it can.
 """
 from __future__ import annotations
 
@@ -28,7 +28,7 @@ import numpy as np
 
 from . import _cabi as A
 from . import keras_like as K
-from .applications import caffe_shift, check_preprocess
+from .applications import caffe_shift, check_model_preprocess, check_preprocess
 
 
 def same_pad(size: int, k: int, s: int) -> Tuple[int, int]:
@@ -53,6 +53,7 @@ class PlanOp:
     w_kernel: int = -1
     w_scale: int = -1
     w_shift: int = -1
+    mode: int = 0                                     # PREPROCESS: A.PRE_CAFFE | A.PRE_TF
     layers: List[str] = field(default_factory=list)   # reference layer names fused into this op
     # planner-only state
     scale: Optional[np.ndarray] = None                # float64 while folding
@@ -92,6 +93,7 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         check_preprocess(preprocess)
         if not is_first:
             raise ValueError(f"preprocess={preprocess!r}: only the first stage takes images")
+        check_model_preprocess(model, preprocess)
     nodes = list(model.iter_nodes())
     # names as recorded at map time (tensor histories may be re-tagged later by Input(tensor=...))
     order = [l.name for l, _ in nodes]
@@ -182,8 +184,9 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
             raise ValueError(f"preprocess={preprocess!r}: the input must be an RGB image (h, w, 3), got {shapes[in_name][1:]}")
         input_buf = new_buf(shapes[in_name], A.BUF_U8)
         op = emit(PlanOp(A.OP_PREPROCESS, input_buf, new_buf(shapes[in_name], A.BUF_F32),
-                         layers=[f"preprocess_input({preprocess})"]))
-        op.w_shift = add_weight(caffe_shift())
+                         mode=A.PRE_MODES[preprocess], layers=[f"preprocess_input({preprocess})"]))
+        if preprocess == "caffe":                     # tf: Keras hard-codes 127.5 and 1, no weights
+            op.w_shift = add_weight(caffe_shift())
         tensor_buf[in_name] = op.out
     producer[in_name] = None
 

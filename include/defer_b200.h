@@ -63,10 +63,15 @@ typedef enum defer_op_kind {
   DEFER_OP_ADD = 8,      /* standalone Add of two tensors [+ relu]                                            */
   DEFER_OP_PAD = 9,      /* standalone ZeroPadding2D                                                          */
   DEFER_OP_COPY = 10,    /* identity / Flatten / format cast                                                  */
-  DEFER_OP_PREPROCESS = 11 /* Keras caffe-mode preprocess_input: in0 = U8 image (c == 3), out = F32 of the same    */
-                         /* shape, w_shift = 3 fp32 values in output-channel order;                              */
-                         /* y[..., c] = float(x[..., 2 - c]) + shift[c]  (RGB -> BGR, minus the ImageNet mean)   */
+  DEFER_OP_PREPROCESS = 11 /* Keras preprocess_input: in0 = U8 image (c == 3), out = F32 of the same shape;     */
+                         /* `mode` DEFER_PRE_CAFFE: w_shift = 3 fp32 values in output-channel order,            */
+                         /*   y[..., c] = float(x[..., 2 - c]) + shift[c]  (RGB -> BGR, minus the ImageNet mean)  */
+                         /* `mode` DEFER_PRE_TF: no weights, y = float(x) / 127.5 - 1 in fp32 (ResNet V2)       */
 } defer_op_kind;
+
+/* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
+#define DEFER_PRE_CAFFE 0   /* keras_applications imagenet_utils mode='caffe' (ResNet50/101/152, VGG16) */
+#define DEFER_PRE_TF    1   /* mode='tf' (ResNet50V2/101V2/152V2): fl32(fl32(x / 127.5) - 1), bit for bit */
 
 #define DEFER_FLAG_RELU      1u   /* apply relu at the end of the op                 */
 #define DEFER_FLAG_RESIDUAL  2u   /* CONV: add buffer in1 before the (optional) relu */
@@ -93,7 +98,7 @@ typedef struct defer_op_desc {
   int32_t w_kernel;        /* CONV: fp32 HWIO kernel;  DENSE: fp32 (in,out) kernel */
   int32_t w_scale;         /* CONV / AFFINE: fp32 per-channel scale (NULL id -1 = ones) */
   int32_t w_shift;         /* CONV / AFFINE / PREPROCESS: fp32 per-channel shift;  DENSE: bias */
-  int32_t reserved;
+  int32_t mode;            /* PREPROCESS: DEFER_PRE_*;  every other kind: 0 */
 } defer_op_desc;
 
 typedef struct defer_stage_config {
@@ -235,6 +240,9 @@ DEFER_API int defer_k_decode(int fmt, const void* x_act, float* y_f32, uint64_t 
 /* Keras caffe-mode preprocess_input (DEFER_OP_PREPROCESS): uint8 NHWC image (c == 3) -> fp32,
  * y[..., c] = float(x[..., 2 - c]) + shift[c]; shift: 3 fp32 values on the device */
 DEFER_API int defer_k_preprocess(const uint8_t* x, const float* shift, float* y, int n, int h, int w, int c, void* stream);
+/* Keras tf-mode preprocess_input (DEFER_OP_PREPROCESS, DEFER_PRE_TF): uint8 NHWC image (c == 3) -> fp32,
+ * y = fl32(fl32(float(x) / 127.5) - 1), channels in place */
+DEFER_API int defer_k_preprocess_tf(const uint8_t* x, float* y, int n, int h, int w, int c, void* stream);
 
 #ifdef __cplusplus
 }

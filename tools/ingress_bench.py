@@ -1,17 +1,20 @@
-"""Ingress cost of Keras caffe preprocessing: host fp32 items vs uint8 items preprocessed on the GPU.
+"""Ingress cost of Keras preprocessing: host fp32 items vs uint8 items preprocessed on the GPU.
 
-One GPU, ResNet50 (224 x 224, synthetic weights, fp32 parity), DEFER.run_defer with coalesce=32 and depth=4.  Three arms,
-each a live pipeline, timed in alternation (--reps rounds after one warm-up round):
+One GPU, ResNet50 in caffe mode or ResNet50V2 in tf mode (224 x 224, synthetic weights, fp32 parity), DEFER.run_defer
+with coalesce=32 and depth=4.  Three arms, each a live pipeline, timed in alternation (--reps rounds after one warm-up
+round):
 
   a  fp32 items, already preprocessed before the clock starts, put on a full input queue
-  b  uint8 items, applications.preprocess_input in the feeding thread (what a reference-style driver does)
-  c  uint8 items on a full input queue, DEFER(preprocess="caffe"): the first stage preprocesses on the GPU
+  b  uint8 items, the host preprocessing function in the feeding thread (what a reference-style driver does):
+     applications.preprocess_input (caffe) or applications.resnet_v2_preprocess_input (tf)
+  c  uint8 items on a full input queue, DEFER(preprocess=mode): the first stage preprocesses on the GPU
 
 It prints one JSON line: end-to-end inferences/s per arm (median, min, max over the rounds), H2D bytes per item, the
-device time of the fp32 fused stem, the uint8 fused stem and the standalone preprocess_kernel (time_op, L2 flushed), the
-host time of one preprocess_input call, and the card's name and power limit (read-only nvidia-smi query).
+device time of the fp32 fused stem, the uint8 fused stem of the mode and its standalone preprocessing kernel (time_op,
+L2 flushed), the host time of one preprocessing call, and the card's name and power limit (read-only nvidia-smi query).
 
-    python tools/ingress_bench.py [--items 640] [--reps 3]
+    python tools/ingress_bench.py [--model resnet50 --preprocess caffe] [--items 640] [--reps 3]
+    python tools/ingress_bench.py --model resnet50v2 --preprocess tf
 """
 from __future__ import annotations
 
@@ -35,6 +38,10 @@ from defer_b200.dispatcher import DEFER  # noqa: E402
 from defer_b200.node import StageRunner  # noqa: E402
 
 G, DEPTH = 32, 4
+MODELS = {"resnet50": applications.ResNet50, "resnet50v2": applications.ResNet50V2}
+HOST_PREPROCESS = {"caffe": applications.preprocess_input, "tf": applications.resnet_v2_preprocess_input}
+# mode -> (fused uint8 stem kernel, standalone preprocessing kernel)
+KERNELS = {"caffe": ("conv_stem_u8_kernel", "preprocess_kernel"), "tf": ("conv_stem_u8tf_kernel", "preprocess_tf_kernel")}
 
 
 def card():
@@ -48,7 +55,8 @@ def card():
 
 
 class Arm:
-    def __init__(self, model, preprocess):
+    def __init__(self, model, preprocess, host_preprocess):
+        self.host_preprocess = host_preprocess
         self.defer = DEFER([0], depth=DEPTH, coalesce=G, linger_us=2000, preprocess=preprocess)
         self.in_q, self.out_q = queue.Queue(), queue.Queue()
         self.err = []
@@ -71,7 +79,7 @@ class Arm:
         if host_preprocess:
             def feed():
                 for x in items:
-                    self.in_q.put(applications.preprocess_input(x))
+                    self.in_q.put(self.host_preprocess(x))
             f = threading.Thread(target=feed, daemon=True)
             f.start()
         else:
@@ -91,11 +99,12 @@ class Arm:
         self.thread.join(timeout=60)
 
 
-def stem_times(model, iters):
+def stem_times(model, mode, iters):
     """time_op (us) of the three stem kernels at the benchmarked microbatch (32 images)."""
     out = {}
-    for key, env, pre, op in (("conv_stem_kernel_f32_us", None, None, 0), ("conv_stem_u8_kernel_us", None, "caffe", 1),
-                              ("preprocess_kernel_us", "0", "caffe", 0)):
+    stem_u8, pre_kernel = KERNELS[mode]
+    for key, env, pre, op in (("conv_stem_kernel_f32_us", None, None, 0), (f"{stem_u8}_us", None, mode, 1),
+                              (f"{pre_kernel}_us", "0", mode, 0)):
         old = os.environ.pop("DEFER_STEM_FUSED", None)
         if env is not None:
             os.environ["DEFER_STEM_FUSED"] = env
@@ -107,6 +116,8 @@ def stem_times(model, iters):
                 os.environ["DEFER_STEM_FUSED"] = old
         try:
             kernel = r.op_info(op)["kernel"]
+            if key != "conv_stem_kernel_f32_us" and kernel != key[:-3]:
+                raise RuntimeError(f"{key}: op {op} runs {kernel}")
             r.predict(applications.synthetic_image(G, seed=1) if pre else applications.synthetic_input(G, seed=1))
             ts = [r.time_op(op, iters=iters, flush_l2=True) for _ in range(3)]
             out[key] = {"kernel": kernel, "us": round(statistics.median(ts), 2), "spread_us": round(max(ts) - min(ts), 2)}
@@ -120,21 +131,26 @@ def main():
     ap.add_argument("--items", type=int, default=640, help="queue items per timed round (batch-1 images)")
     ap.add_argument("--reps", type=int, default=3, help="timed rounds per arm (alternated), >= 3")
     ap.add_argument("--op-iters", type=int, default=50)
+    ap.add_argument("--model", choices=sorted(MODELS), default="resnet50")
+    ap.add_argument("--preprocess", choices=sorted(HOST_PREPROCESS), default="caffe",
+                    help="Keras preprocessing mode (the model's own: caffe for resnet50, tf for resnet50v2)")
     args = ap.parse_args()
     if args.reps < 3:
         ap.error("--reps must be >= 3")
 
-    model = applications.ResNet50()
+    model = MODELS[args.model]()
+    host_fn = HOST_PREPROCESS[args.preprocess]
     imgs = [applications.synthetic_image(1, seed=i) for i in range(args.items)]
-    pre = [applications.preprocess_input(x) for x in imgs]
+    pre = [host_fn(x) for x in imgs]
 
     t0 = time.perf_counter()
     n_host = 200
     for i in range(n_host):
-        applications.preprocess_input(imgs[i % len(imgs)])
+        host_fn(imgs[i % len(imgs)])
     host_us = (time.perf_counter() - t0) / n_host * 1e6
 
-    arms = {"a_f32_items": Arm(model, None), "b_u8_host_preprocess": Arm(model, None), "c_u8_gpu_preprocess": Arm(model, "caffe")}
+    arms = {"a_f32_items": Arm(model, None, host_fn), "b_u8_host_preprocess": Arm(model, None, host_fn),
+            "c_u8_gpu_preprocess": Arm(model, args.preprocess, host_fn)}
     feeds = {"a_f32_items": (pre, False), "b_u8_host_preprocess": (imgs, True), "c_u8_gpu_preprocess": (imgs, False)}
     rates = {k: [] for k in arms}
     try:
@@ -150,12 +166,12 @@ def main():
             arm.close()
 
     res = {
-        "metric": "resnet50_ingress_inferences_per_s",
+        "metric": f"{args.model}_ingress_inferences_per_s", "preprocess": args.preprocess,
         "coalesce": G, "depth": DEPTH, "items_per_round": args.items, "rounds": args.reps,
         "arms": {k: {"median": round(statistics.median(v), 1), "min": round(min(v), 1), "max": round(max(v), 1),
                      "all": [round(x, 1) for x in v], "h2d_bytes_per_item": h2d[k]} for k, v in rates.items()},
         "host_preprocess_input_us": round(host_us, 1),
-        "stem_time_op": stem_times(model, args.op_iters),
+        "stem_time_op": stem_times(model, args.preprocess, args.op_iters),
     }
     res.update(card())
     print(json.dumps(res), flush=True)
