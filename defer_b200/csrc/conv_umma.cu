@@ -22,9 +22,10 @@
 //     one thread-block cluster reducing through distributed shared memory.  Both sum in a fixed order.
 //
 // Warp roles (384 threads): warpgroups 0-1 consume (wgmma + epilogue), warpgroup 2 produces (one thread
-// issues the TMA loads; for the fused RGB stem all 128 threads build the A operand from the fp32 image).
-// The same body runs one tile per CTA (conv_umma_kernel) or walks a tile list (conv_stream_kernel:
-// persistent grid, or one cluster walking a run of ops separated by cluster barriers).
+// issues the TMA loads).  The same body runs one tile per CTA (conv_umma_kernel) or walks a tile list
+// (conv_stream_kernel: persistent grid, or one cluster walking a run of ops separated by cluster barriers).
+// The fused RGB stem (conv_stem_kernel and its uint8 variants) has a body of its own: all 128 producer threads
+// build the A operand from an image window they stage in shared memory.
 #include <cuda.h>
 #include <string.h>
 
@@ -82,17 +83,18 @@ struct alignas(128) MegaOp {
   CUtensorMap tmw[2];
   KParams p;
   int m_tiles, n_tiles;     // tiles of this op: m fastest
-  // fused stem: the fp32 NHWC image the patch rows are built from, and the real conv geometry
+  // fused stem: the fp32 NHWC image the patch rows are built from, the real conv geometry and the image window of one
+  // M tile (stem_win_rows x stem_win_cols values, see stem_body)
   const float* stem_x;
   int stem_h, stem_w, stem_cin, stem_kh, stem_kw, stem_sh, stem_sw, stem_pad_t, stem_pad_l, stem_K;
+  int stem_win_rows, stem_win_cols;
   // fused stem over a uint8 RGB image instead (conv_stem_u8_kernel): Keras caffe preprocessing on the fly,
   // value[c] = float(image[2 - c]) + stem_shift[c]; or Keras tf preprocessing (conv_stem_u8tf_kernel, stem_shift unused),
   // value[c] = float(image[c]) / 127.5 - 1
   const uint8_t* stem_u8;
   float stem_shift[3];
   // second epilogue output (conv_umma_aff_kernel / conv_stream_aff_kernel): a standalone per-channel affine(+ReLU) of
-  // the stored result, y2 = [relu](fmaf(stored, scale2[c], shift2[c])).  Appended last: the fields above keep their
-  // offsets and sizeof(MegaOp) stays 768 B.
+  // the stored result, y2 = [relu](fmaf(stored, scale2[c], shift2[c])).
   const float* scale2;
   const float* shift2;
   void* y2;
@@ -487,111 +489,11 @@ __device__ __forceinline__ void epi_tile(const KParams& p, const EpiArgs& e, uin
   }
 }
 
-// Fused RGB stem: the producer warpgroup writes one k-block of the A operand (128 patch rows x 64 k, bf16 hi / lo
-// planes) in the SWIZZLE_128B layout TMA would have produced.  In NHWC a patch is kh runs of kw*cin contiguous floats,
-// so k -> (kernel row a, offset jj) and one range check on the flat column index covers the left / right padding.
-// U8: the image is uint8 RGB (cin == 3, checked by the stage) and each tap is preprocessed as it is read: channel c
-// <- image channel 2 - c, plus stem_shift[c].  The padding belongs to the preprocessed tensor, so an out-of-range tap
-// stays 0.  All eight byte loads of a chunk are issued before any of them is converted (a load whose conversion sits
-// next to it in a branch would wait out its latency before the next load issues), and as a run is whole pixels, tap k
-// has channel k % 3: the eight taps of a chunk see a rotation of (0, 1, 2), so the mirrored-channel offset and the shift
-// are chosen once per chunk.  float(byte) is exact via the 2^23 magic number, then one rounded add: the same value the
-// standalone preprocess_kernel writes.
-// U8 && TF: Keras tf mode instead - channel c <- image channel c, keras_tf_preprocess(float(byte)), no shift: the same
-// value preprocess_tf_kernel writes.  The loads are issued the same way; there is no channel rotation to track.
-template <int NPLANES, bool U8, bool TF = false>
-__device__ __forceinline__ void stem_build(const MegaOp& op, uint32_t a_dst, int m0, int kb, int r) {
-  static_assert(U8 || !TF, "tf preprocessing reads a uint8 image");
-  using In = std::conditional_t<U8, uint8_t, float>;
-  const KParams& p = op.p;
-  const int m = m0 + r;
-  const int run = op.stem_kw * op.stem_cin, wc = op.stem_w * op.stem_cin;
-  const In* img = nullptr;
-  int ih0 = 0, col0 = 0;
-  if (m < p.m_total) {
-    const int hw = p.ho * p.wo;
-    const int im = m / hw, rem = m - im * hw, oh = rem / p.wo, ow = rem - oh * p.wo;
-    if constexpr (U8) img = op.stem_u8 + (size_t)im * op.stem_h * wc;
-    else img = op.stem_x + (size_t)im * op.stem_h * wc;
-    ih0 = oh * op.stem_sh - op.stem_pad_t;
-    col0 = (ow * op.stem_sw - op.stem_pad_l) * op.stem_cin;
-  }
-  int k = kb * BK;
-  int a = k / run, jj = k - a * run;
-  int c0 = 0, K = 0, H = 0;         // U8: channel of the chunk's first tap; stem_K and stem_h kept in registers
-  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-  if constexpr (U8) {
-    c0 = k % 3;
-    K = op.stem_K;
-    H = op.stem_h;
-    s0 = op.stem_shift[0]; s1 = op.stem_shift[1]; s2 = op.stem_shift[2];
-  }
-#pragma unroll 1
-  for (int ch = 0; ch < 8; ++ch) {
-    float v[8];
-    if constexpr (TF) {
-      uint32_t raw[8];
-      bool in[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int ih = ih0 + a, col = col0 + jj;
-        in[e] = img && k < K && ih >= 0 && ih < H && col >= 0 && col < wc;
-        raw[e] = in[e] ? (uint32_t)__ldg(img + (size_t)ih * wc + col) : 0u;
-        ++k;
-        if (++jj == run) { jj = 0; ++a; }
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        v[e] = in[e] ? keras_tf_preprocess(__fsub_rn(__uint_as_float(0x4B000000u | raw[e]), 8388608.f)) : 0.f;
-    } else if constexpr (U8) {
-      const float sr[3] = {c0 == 0 ? s0 : (c0 == 1 ? s1 : s2), c0 == 0 ? s1 : (c0 == 1 ? s2 : s0),
-                           c0 == 0 ? s2 : (c0 == 1 ? s0 : s1)};
-      const int mr[3] = {2 - 2 * c0, c0 == 2 ? 2 : -2 * c0, c0 == 0 ? -2 : 4 - 2 * c0};   // 2 - 2 * ((c0 + i) % 3)
-      uint32_t raw[8];
-      bool in[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int ih = ih0 + a, col = col0 + jj;
-        in[e] = img && k < K && ih >= 0 && ih < H && col >= 0 && col < wc;
-        raw[e] = in[e] ? (uint32_t)__ldg(img + (size_t)ih * wc + col + mr[e % 3]) : 0u;
-        ++k;
-        if (++jj == run) { jj = 0; ++a; }
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e)
-        v[e] = in[e] ? __fadd_rn(__fsub_rn(__uint_as_float(0x4B000000u | raw[e]), 8388608.f), sr[e % 3]) : 0.f;
-      c0 = c0 == 0 ? 2 : c0 - 1;    // (c0 + 8) % 3
-    } else {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const int ih = ih0 + a, col = col0 + jj;
-        v[e] = (img && k < op.stem_K && ih >= 0 && ih < op.stem_h && col >= 0 && col < wc) ? __ldg(img + (size_t)ih * wc + col)
-                                                                                          : 0.f;
-        ++k;
-        if (++jj == run) { jj = 0; ++a; }
-      }
-    }
-    const uint32_t off = (uint32_t)r * 128u + ((uint32_t)(ch ^ (r & 7)) << 4);
-    uint32_t h[4], l[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      if (NPLANES == 2) split_bf16x2(v[2 * q], v[2 * q + 1], h[q], l[q]);
-      else h[q] = pack_bf16x2(v[2 * q], v[2 * q + 1]);
-    }
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + off), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3])
-                 : "memory");
-    if (NPLANES == 2)
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + Smem<NPLANES, 64>::A_PLANE + off), "r"(l[0]),
-                   "r"(l[1]), "r"(l[2]), "r"(l[3])
-                   : "memory");
-  }
-}
-
 // ---------------------------------------------------------------------------------------------- the kernel body
 // MODE 0: one (tile, split) per CTA: tile = (blockIdx.x, blockIdx.y), split = blockIdx.z (grid split-K or cluster split-K)
 // MODE 1: persistent grid: CTA b walks tiles b, b + gridDim.x, ... of one op
 // MODE 2: one cluster walks a run of ops; tiles are dealt round-robin to its CTAs, a cluster barrier separates ops
-template <int NPLANES, int BN, int MODE, bool U8 = false, bool AFF = false, bool TF = false>
+template <int NPLANES, int BN, int MODE, bool AFF = false>
 __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stages, int pdl) {
   using L = Smem<NPLANES, BN>;
   constexpr int R = BN / 2;   // accumulator registers per consumer thread
@@ -640,7 +542,6 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
     const int split = MODE == 0 ? (int)blockIdx.z : 0;
     const int kb_begin = (split * p.k_blocks) / p.splits;   // balanced ranges; host guarantees k_blocks >= splits
     const int kb_end = ((split + 1) * p.k_blocks) / p.splits;
-    const bool stem = U8 || op.stem_x != nullptr;
 
     for (int t = t_first; t < total; t += t_step) {
       const int m_tile = t % op.m_tiles;
@@ -658,8 +559,7 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
 
       if (tid >= CONS_THREADS) {
         // =================================================================== producer
-        const int ptid = tid - CONS_THREADS;
-        if (stem || ptid == 0) {
+        if (tid == CONS_THREADS) {
           const uint32_t a_rows = p.flat ? (uint32_t)BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
           uint32_t i2 = it;
           for (int kb = kb_begin; kb < kb_end; ++kb, ++i2) {
@@ -670,32 +570,20 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
             const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
             const int tap = kb / p.cblocks;
             const int cb = kb - tap * p.cblocks;
-            if (stem) {
-              if (ptid == 0) {
-                mbar_expect_tx(full_bar(stage), NPLANES * (uint32_t)L::B_PLANE);
-                tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
-                if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
-              }
-              stem_build<NPLANES, U8, TF>(op, a_dst, w0, kb, ptid);
-              asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
-              prod_bar_sync();
-              if (ptid == 0) mbar_arrive(full_bar(stage));
-            } else {
-              const int khi = tap / p.kw;
-              const int kwi = tap - khi * p.kw;
-              int cw = w0, ch = 0, cn = 0;
-              if (!p.flat) {
-                cw = w0 * p.sw + kwi - p.pad_l;
-                ch = h0 * p.sh + khi - p.pad_t;
-                cn = n0;
-              }
-              mbar_arrive_expect_tx(full_bar(stage), NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE));
-              tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
-              tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
-              if (NPLANES == 2) {
-                tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
-                tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
-              }
+            const int khi = tap / p.kw;
+            const int kwi = tap - khi * p.kw;
+            int cw = w0, ch = 0, cn = 0;
+            if (!p.flat) {
+              cw = w0 * p.sw + kwi - p.pad_l;
+              ch = h0 * p.sh + khi - p.pad_t;
+              cn = n0;
+            }
+            mbar_arrive_expect_tx(full_bar(stage), NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE));
+            tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
+            tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
+            if (NPLANES == 2) {
+              tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
+              tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
             }
           }
         }
@@ -841,29 +729,300 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_kernel(const MegaO
 // the same two executors with a folded affine op as a second epilogue output (MegaOp::y2)
 template <int NPLANES, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_umma_aff_kernel(const __grid_constant__ MegaOp op, int stages, int pdl) {
-  conv_body<NPLANES, BN, 0, false, true>(&op, 1, stages, pdl);
+  conv_body<NPLANES, BN, 0, true>(&op, 1, stages, pdl);
 }
 
 template <int NPLANES, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_stream_aff_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
-  conv_body<NPLANES, BN, 1, false, true>(ops, 1, stages, pdl);
-}
-
-// the fused stem reading a uint8 RGB image (Keras caffe preprocessing applied while the patch rows are built)
-template <int NPLANES>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
-  conv_body<NPLANES, 64, 1, true>(ops, 1, stages, pdl);
-}
-
-// ... preprocessing it in Keras tf mode instead
-template <int NPLANES>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8tf_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
-  conv_body<NPLANES, 64, 1, true, false, true>(ops, 1, stages, pdl);
+  conv_body<NPLANES, BN, 1, true>(ops, 1, stages, pdl);
 }
 
 template <int NPLANES>
 __global__ void __launch_bounds__(NUM_THREADS, 1) conv_mega_kernel(const MegaOp* __restrict__ ops, int n_ops, int stages) {
   conv_body<NPLANES, MEGA_BN, 2>(ops, n_ops, stages, 0);
+}
+
+// ---------------------------------------------------------------------------------------------- the fused RGB stem
+// conv_stem_kernel, conv_stem_u8_kernel, conv_stem_u8tf_kernel: a persistent grid over the tiles of a conv whose input has
+// a few channels (K = kh * kw * cin <= 256, zero-padded to whole k-blocks; C_out = 64), with no patch matrix in memory.
+// The M tile is tile_h x tile_w output pixels of one image, so its input footprint is a window of
+//   stem_win_rows = (tile_h - 1) * sh + kh rows  x  stem_win_cols = ((tile_w - 1) * sw + kw) * cin values.
+// For each tile the producer warpgroup fills that window in shared memory with the conv input's fp32 values: the fp32 image
+// itself, or the uint8 image preprocessed (Keras caffe: channel c <- float(image[2 - c]) + stem_shift[c]; Keras tf:
+// keras_tf_preprocess(float(image[c])) - bit for bit what preprocess_kernel / preprocess_tf_kernel write), and zeros
+// outside the image, since the padding belongs to the preprocessed tensor.  Consecutive threads load consecutive values of
+// a window row, and every load of a window is issued before any is converted.  The window is double-buffered: the loads of
+// the next tile are in flight while the k-blocks of this one are built.
+// The builder writes patch row r (pixel th = r / tile_w, tw = r % tile_w of the tile) of k-block kb in the SWIZZLE_128B
+// layout TMA would have produced: k = a * kw * cin + jj is window value (th * sh + a) * stem_win_cols + tw * sw * cin + jj
+// for k < K, and 0 beyond.  Same values, same split and same K order as the patch matrix of stem_im2col_kernel, so the
+// fused stem and the im2col path agree bitwise.
+enum StemIn { STEM_F32, STEM_U8_CAFFE, STEM_U8_TF };
+constexpr int PROD_THREADS = NUM_THREADS - CONS_THREADS;
+constexpr int STEM_WIN_BYTES = 24 * 1024;                         // one window buffer; two are resident
+constexpr int STEM_WIN_VALS = STEM_WIN_BYTES / 4;
+constexpr int STEM_FILL = STEM_WIN_VALS / PROD_THREADS;           // window values per producer thread, held in registers
+constexpr int STEM_TILE_W = 16;                                   // 8 x 16 output pixels per M tile (fewer columns on a narrow map)
+
+template <int NPLANES>
+struct StemSmem {
+  static constexpr int STAGE = Smem<NPLANES, 64>::STAGE;
+  // ring | epilogue staging tile | two window buffers | mbarriers, + slack for the 1024-B alignment of the base
+  __host__ __device__ static constexpr int total(int stages) {
+    return stages * STAGE + STG_BYTES + 2 * STEM_WIN_BYTES + CTL_BYTES + 1024;
+  }
+  __host__ __device__ static constexpr int max_stages() {
+    return (SMEM_CAP - STG_BYTES - 2 * STEM_WIN_BYTES - CTL_BYTES - 1024) / STAGE > MAX_STAGES
+               ? MAX_STAGES
+               : (SMEM_CAP - STG_BYTES - 2 * STEM_WIN_BYTES - CTL_BYTES - 1024) / STAGE;
+  }
+};
+// BF16X2: 3 stages of 48 KB hold the whole K loop of a tile (K <= 256: at most 4 k-blocks) next to the two windows
+static_assert(StemSmem<2>::max_stages() == 3 && StemSmem<1>::max_stages() == 6, "stem ring depths with two image windows");
+static_assert(STEM_FILL * PROD_THREADS == STEM_WIN_VALS, "the producer threads cover a whole window");
+
+// the stem's operands, read from the op once per kernel (a field read after a shared-memory store would be re-read)
+struct StemGeo {
+  const float* x;
+  const uint8_t* u8;
+  float s0, s1, s2;
+  int H, rowlen;        // image rows, values per image row (w * cin)
+  int cin, sh, sw, pad_t, pad_l;
+  int wcols, nwin;      // window: values per row, values in all
+  int run, K;           // kw * cin, kh * kw * cin
+};
+
+__device__ __forceinline__ StemGeo stem_geo(const MegaOp& op) {
+  StemGeo g;
+  g.x = op.stem_x;
+  g.u8 = op.stem_u8;
+  g.s0 = op.stem_shift[0]; g.s1 = op.stem_shift[1]; g.s2 = op.stem_shift[2];
+  g.H = op.stem_h;
+  g.rowlen = op.stem_w * op.stem_cin;
+  g.cin = op.stem_cin; g.sh = op.stem_sh; g.sw = op.stem_sw; g.pad_t = op.stem_pad_t; g.pad_l = op.stem_pad_l;
+  g.wcols = op.stem_win_cols;
+  g.nwin = op.stem_win_rows * op.stem_win_cols;
+  g.run = op.stem_kw * op.stem_cin;
+  g.K = op.stem_K;
+  return g;
+}
+
+// output pixel of row 0 of stem tile m_tile (tile_n = 1: a tile never spans two images)
+__device__ __forceinline__ void stem_tile_origin(const KParams& p, int m_tile, int& n0, int& h0, int& w0) {
+  const int t2 = m_tile / p.tiles_w;
+  n0 = t2 / p.tiles_h;
+  h0 = (t2 - n0 * p.tiles_h) * p.tile_h;
+  w0 = (m_tile - t2 * p.tiles_w) * p.tile_w;
+}
+
+// This thread's values of the window of the tile at (n0, h0, w0): value e = ptid + 128 j (row e / wcols, column e % wcols).
+// Out-of-image values are marked: 0 (fp32: +0.f) or 0x100 (uint8).
+template <int IN>
+__device__ __forceinline__ void stem_fill_load(const StemGeo& g, int ptid, int n0, int h0, int w0, uint32_t (&raw)[STEM_FILL]) {
+  const int ih0 = h0 * g.sh - g.pad_t, col0 = (w0 * g.sw - g.pad_l) * g.cin;
+  const size_t img = (size_t)n0 * g.H * g.rowlen;
+  const int dq = PROD_THREADS / g.wcols, dm = PROD_THREADS - dq * g.wcols;
+  int wr = ptid / g.wcols, wc = ptid - wr * g.wcols;
+  int c = wc % 3;   // uint8 images: channel of the value (a window row is whole 3-channel pixels)
+#pragma unroll
+  for (int j = 0; j < STEM_FILL; ++j) {
+    const int ih = ih0 + wr, col = col0 + wc;
+    const bool in = ptid + PROD_THREADS * j < g.nwin && ih >= 0 && ih < g.H && col >= 0 && col < g.rowlen;
+    const size_t off = img + (size_t)(ih * g.rowlen + col);
+    if constexpr (IN == STEM_F32) raw[j] = in ? __float_as_uint(__ldg(g.x + off)) : 0u;
+    else raw[j] = in ? (uint32_t)__ldg(g.u8 + off + (IN == STEM_U8_CAFFE ? 2 - 2 * c : 0)) : 0x100u;
+    wr += dq;
+    wc += dm;
+    if (wc >= g.wcols) { wc -= g.wcols; ++wr; }
+    c = c == 0 ? 2 : c - 1;   // (c + 128) % 3
+  }
+}
+
+// ... converted to the conv input's values and stored at window[e].  float(byte) is exact via the 2^23 magic number; then
+// the one rounded add (caffe) or keras_tf_preprocess (tf).
+template <int IN>
+__device__ __forceinline__ void stem_fill_store(const StemGeo& g, uint32_t win, int ptid, const uint32_t (&raw)[STEM_FILL]) {
+  int c = (ptid % g.wcols) % 3;
+#pragma unroll
+  for (int j = 0; j < STEM_FILL; ++j) {
+    const int e = ptid + PROD_THREADS * j;
+    if (e < g.nwin) {
+      const float b = __fsub_rn(__uint_as_float(0x4B000000u | raw[j]), 8388608.f);
+      float v;
+      if constexpr (IN == STEM_F32) v = __uint_as_float(raw[j]);
+      else if constexpr (IN == STEM_U8_CAFFE) v = raw[j] > 255u ? 0.f : __fadd_rn(b, c == 0 ? g.s0 : (c == 1 ? g.s1 : g.s2));
+      else v = raw[j] > 255u ? 0.f : keras_tf_preprocess(b);
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(win + 4u * (uint32_t)e), "f"(v) : "memory");
+    }
+    c = c == 0 ? 2 : c - 1;
+  }
+}
+
+// patch row r of k-block kb (128 rows x 64 k, bf16 hi / lo planes) from the window; row_base = th * sh * wcols + tw * sw * cin
+template <int NPLANES>
+__device__ __forceinline__ void stem_build(const StemGeo& g, uint32_t win, uint32_t a_dst, int r, int row_base, int kb) {
+  int k = kb * BK;
+  int a = k / g.run, jj = k - a * g.run;
+  uint32_t src = win + 4u * (uint32_t)(row_base + a * g.wcols + jj);
+  const uint32_t wrap = 4u * (uint32_t)(g.wcols - g.run);   // end of a kernel row's run -> start of the next one
+#pragma unroll 1
+  for (int ch = 0; ch < 8; ++ch) {
+    float v[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      v[e] = 0.f;
+      if (k < g.K) asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v[e]) : "r"(src));
+      ++k;
+      src += 4u;
+      if (++jj == g.run) { jj = 0; src += wrap; }
+    }
+    const uint32_t off = (uint32_t)r * 128u + ((uint32_t)(ch ^ (r & 7)) << 4);
+    uint32_t h[4], l[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (NPLANES == 2) split_bf16x2(v[2 * q], v[2 * q + 1], h[q], l[q]);
+      else h[q] = pack_bf16x2(v[2 * q], v[2 * q + 1]);
+    }
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + off), "r"(h[0]), "r"(h[1]), "r"(h[2]), "r"(h[3])
+                 : "memory");
+    if (NPLANES == 2)
+      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_dst + Smem<NPLANES, 64>::A_PLANE + off), "r"(l[0]),
+                   "r"(l[1]), "r"(l[2]), "r"(l[3])
+                   : "memory");
+  }
+}
+
+template <int NPLANES, int IN>
+__device__ __forceinline__ void stem_body(const MegaOp* ops, int stages, int pdl) {
+  using L = Smem<NPLANES, 64>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const uint32_t ring = smem_u32(smem);
+  const uint32_t stg = ring + stages * L::STAGE;
+  const uint32_t win0 = stg + STG_BYTES;
+  const uint32_t bar_base = win0 + 2 * STEM_WIN_BYTES;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (stages + s); };
+
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), CONS_THREADS / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (pdl) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  }
+
+  const MegaOp& op = ops[0];
+  const KParams& p = op.p;
+  const int total = op.m_tiles * op.n_tiles;
+  const int k_blocks = p.k_blocks;
+  uint32_t it = 0;   // k-blocks through the ring so far (same sequence in both roles)
+
+  if (tid >= CONS_THREADS) {
+    // =================================================================== producer: window fill + patch rows
+    const int ptid = tid - CONS_THREADS;
+    const StemGeo g = stem_geo(op);
+    // rows past tile_h x tile_w (a map narrower than the tile) build pixel (0, 0): the epilogue stores no such row
+    int th = ptid / p.tile_w, tw = ptid - th * p.tile_w;
+    if (th >= p.tile_h) th = tw = 0;
+    const int row_base = th * g.sh * g.wcols + tw * g.sw * g.cin;
+    uint32_t raw[STEM_FILL];
+    int n0, h0, w0;
+    if ((int)blockIdx.x < total) {
+      stem_tile_origin(p, (int)blockIdx.x % op.m_tiles, n0, h0, w0);
+      stem_fill_load<IN>(g, ptid, n0, h0, w0, raw);
+      stem_fill_store<IN>(g, win0, ptid, raw);
+    }
+    int wb = 0;
+    for (int t = blockIdx.x; t < total; t += gridDim.x, wb ^= 1) {
+      const int t_next = t + (int)gridDim.x;
+      if (t_next < total) {   // the next tile's window: in flight while this tile is built
+        stem_tile_origin(p, t_next % op.m_tiles, n0, h0, w0);
+        stem_fill_load<IN>(g, ptid, n0, h0, w0, raw);
+      }
+      prod_bar_sync();   // window wb is complete
+      const uint32_t win = win0 + (uint32_t)wb * STEM_WIN_BYTES;
+      const int c_base = (t / op.m_tiles) * 64;
+      for (int kb = 0; kb < k_blocks; ++kb, ++it) {
+        const int stage = (int)(it % (uint32_t)stages);
+        mbar_wait(empty_bar(stage), ((it / (uint32_t)stages) & 1u) ^ 1u, 1);
+        const uint32_t a_dst = ring + stage * L::STAGE;
+        const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
+        if (ptid == 0) {
+          mbar_expect_tx(full_bar(stage), NPLANES * (uint32_t)L::B_PLANE);
+          tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), kb * BK, c_base, 0);
+          if (NPLANES == 2) tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), kb * BK, c_base, 0);
+        }
+        stem_build<NPLANES>(g, win, a_dst, ptid, row_base, kb);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
+        prod_bar_sync();   // also: every producer is done reading window wb ^ 1 (built by the previous tile)
+        if (ptid == 0) mbar_arrive(full_bar(stage));
+      }
+      if (t_next < total) stem_fill_store<IN>(g, win0 + (uint32_t)(wb ^ 1) * STEM_WIN_BYTES, ptid, raw);
+    }
+    return;
+  }
+
+  // ===================================================================== consumers
+  const int wg = tid >> 7;
+  const int lane = tid & 31;
+  for (int t = blockIdx.x; t < total; t += gridDim.x) {
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    int prev_stage = -1;
+    for (int kb = 0; kb < k_blocks; ++kb, ++it) {
+      const int stage = (int)(it % (uint32_t)stages);
+      mbar_wait(full_bar(stage), (it / (uint32_t)stages) & 1u, 2);
+      const uint32_t a_addr = ring + stage * L::STAGE + wg * (64 * 128);
+      const uint32_t b_addr = ring + stage * L::STAGE + NPLANES * L::A_PLANE;
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t a_hi = make_sw128_desc(a_addr + k * 32);
+        const uint64_t b_hi = make_sw128_desc(b_addr + k * 32);
+        wgmma_bf16<64>(acc, a_hi, b_hi);
+        if (NPLANES == 2) {
+          wgmma_bf16<64>(acc, make_sw128_desc(a_addr + L::A_PLANE + k * 32), b_hi);
+          wgmma_bf16<64>(acc, a_hi, make_sw128_desc(b_addr + L::B_PLANE + k * 32));
+        }
+      }
+      wg_commit();
+      wg_wait<1>();   // the previous k-block's wgmmas are done: its stage may be refilled
+      acc_fence(acc);
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+      prev_stage = stage;
+    }
+    wg_wait<0>();
+    acc_fence(acc);
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+    int n0, h0, w0;
+    stem_tile_origin(p, t % op.m_tiles, n0, h0, w0);
+    epi_tile<NPLANES, 64, false>(p, epi_args(op), stg, acc, 0xffffu, (t / op.m_tiles) * 64, n0, h0, w0);
+  }
+}
+
+template <int NPLANES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  stem_body<NPLANES, STEM_F32>(ops, stages, pdl);
+}
+
+// the fused stem reading a uint8 RGB image: Keras caffe preprocessing applied as the window is filled
+template <int NPLANES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  stem_body<NPLANES, STEM_U8_CAFFE>(ops, stages, pdl);
+}
+
+// ... preprocessing it in Keras tf mode instead
+template <int NPLANES>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_stem_u8tf_kernel(const MegaOp* __restrict__ ops, int stages, int pdl) {
+  stem_body<NPLANES, STEM_U8_TF>(ops, stages, pdl);
 }
 
 // weights: fp32 HWIO [tap][cin][cout]  ->  bf16 [plane][tap][cout][cin]
@@ -1020,22 +1179,13 @@ int launch_op_t(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, cudaStream_t s
 // persistent grid over the tiles of one op in device memory: every CTA walks ceil(n_tiles / grid) tiles, so the launch
 // lasts `rounds` tile-times whatever the grid is; take the SMALLEST grid that still finishes in the minimum number of
 // rounds and leave the other SMs to the lanes running next to this one
-template <int NPLANES, int BN, bool U8 = false, bool AFF = false, bool TF = false>
-int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
-  using L = Smem<NPLANES, BN>;
-  static_assert(!U8 || BN == 64, "the uint8 stem runs with 64-wide N tiles");
-  static_assert(!(U8 && AFF), "no folded affine op on the stem");
-  static_assert(U8 || !TF, "tf preprocessing reads a uint8 image");
-  constexpr auto kernel = U8 ? (TF ? &conv_stem_u8tf_kernel<NPLANES> : &conv_stem_u8_kernel<NPLANES>)
-                             : (AFF ? &conv_stream_aff_kernel<NPLANES, BN> : &conv_stream_kernel<NPLANES, BN>);
+template <auto kernel>
+int launch_grid(const void* dev_op, int n_tiles, int stages, size_t smem, cudaStream_t st) {
   DEFER_TRY((set_smem_attr<kernel>()));
-  if (stages > L::max_stages()) stages = L::max_stages();
-  if (stages < 2) stages = 2;
   const int sms = sm_count();
   int grid = sms < n_tiles ? sms : n_tiles;
   const int rounds = (n_tiles + grid - 1) / grid;
   grid = (n_tiles + rounds - 1) / rounds;
-  const size_t smem = (size_t)L::total(stages, false);
   static const int pdl = env_int("DEFER_PDL", 0);
   if (pdl) {
     cudaLaunchConfig_t cfg;
@@ -1055,6 +1205,26 @@ int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t s
   kernel<<<grid, NUM_THREADS, smem, st>>>(reinterpret_cast<const MegaOp*>(dev_op), stages, 0);
   DEFER_CUDA(cudaGetLastError());
   return DEFER_OK;
+}
+
+template <int NPLANES, int BN, bool AFF = false>
+int launch_persist_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
+  using L = Smem<NPLANES, BN>;
+  constexpr auto kernel = AFF ? &conv_stream_aff_kernel<NPLANES, BN> : &conv_stream_kernel<NPLANES, BN>;
+  if (stages > L::max_stages()) stages = L::max_stages();
+  if (stages < 2) stages = 2;
+  return launch_grid<kernel>(dev_op, n_tiles, stages, (size_t)L::total(stages, false), st);
+}
+
+template <int NPLANES, int IN>
+int launch_stem_t(const void* dev_op, int n_tiles, int stages, cudaStream_t st) {
+  using L = StemSmem<NPLANES>;
+  constexpr auto kernel = IN == STEM_U8_TF      ? &conv_stem_u8tf_kernel<NPLANES>
+                          : IN == STEM_U8_CAFFE ? &conv_stem_u8_kernel<NPLANES>
+                                                : &conv_stem_kernel<NPLANES>;
+  if (stages > L::max_stages()) stages = L::max_stages();
+  if (stages < 2) stages = 2;
+  return launch_grid<kernel>(dev_op, n_tiles, stages, (size_t)L::total(stages), st);
 }
 
 template <int NPLANES>
@@ -1303,8 +1473,8 @@ int umma_mega_cluster_size() {
 int launch_conv_persistent(int nplanes, const void* dev_op, int n_tiles, bool aff, cudaStream_t st) {
   const int stages = env_int("DEFER_PERSIST_STAGES", MAX_STAGES);
   if (aff)
-    return nplanes == 2 ? launch_persist_t<2, 64, false, true>(dev_op, n_tiles, stages, st)
-                        : launch_persist_t<1, 64, false, true>(dev_op, n_tiles, stages, st);
+    return nplanes == 2 ? launch_persist_t<2, 64, true>(dev_op, n_tiles, stages, st)
+                        : launch_persist_t<1, 64, true>(dev_op, n_tiles, stages, st);
   return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
 }
 
@@ -1314,10 +1484,10 @@ int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int
   (void)k_blocks;
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
   if (aff) {
-    if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128, false, true>(dev_op, n_tiles, stages, st)
-                                       : launch_persist_t<1, 128, false, true>(dev_op, n_tiles, stages, st);
-    if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64, false, true>(dev_op, n_tiles, stages, st)
-                                      : launch_persist_t<1, 64, false, true>(dev_op, n_tiles, stages, st);
+    if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128, true>(dev_op, n_tiles, stages, st)
+                                       : launch_persist_t<1, 128, true>(dev_op, n_tiles, stages, st);
+    if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64, true>(dev_op, n_tiles, stages, st)
+                                      : launch_persist_t<1, 64, true>(dev_op, n_tiles, stages, st);
   }
   if (bn == 128) return nplanes == 2 ? launch_persist_t<2, 128>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 128>(dev_op, n_tiles, stages, st);
   if (bn == 64) return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
@@ -1326,19 +1496,41 @@ int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int
 }
 
 // ---- fused stem: host side
-bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags) {
-  (void)n; (void)h; (void)w; (void)cin; (void)ho; (void)wo; (void)kh; (void)sh;
-  if (fmt != FMT_BF16X2 && fmt != FMT_BF16) return false;
-  return cout == 64 && !(flags & DEFER_FLAG_RESIDUAL);
+// M tile of the fused stem: 8 rows x 16 columns of output pixels of one image (fewer columns and more rows on a map
+// narrower than 16), and the image window it reads
+static void stem_tile(int ho, int wo, int kh, int kw, int sh, int sw, int cin, int* tile_h, int* tile_w, int* win_rows,
+                      int* win_cols) {
+  *tile_w = wo < STEM_TILE_W ? wo : STEM_TILE_W;
+  *tile_h = BM / *tile_w < ho ? BM / *tile_w : ho;
+  *win_rows = (*tile_h - 1) * sh + kh;
+  *win_cols = ((*tile_w - 1) * sw + kw) * cin;
 }
 
-void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l) {
+bool umma_stem_fusable(int fmt, int cin, int ho, int wo, int cout, int kh, int kw, int sh, int sw, uint32_t flags) {
+  if (fmt != FMT_BF16X2 && fmt != FMT_BF16) return false;
+  if (cout != 64 || (flags & DEFER_FLAG_RESIDUAL) || kh * kw * cin > 256) return false;
+  int tile_h, tile_w, win_rows, win_cols;
+  stem_tile(ho, wo, kh, kw, sh, sw, cin, &tile_h, &tile_w, &win_rows, &win_cols);
+  return (long long)win_rows * win_cols <= STEM_WIN_VALS;
+}
+
+int umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t,
+                       int pad_l) {
   MegaOp* op = reinterpret_cast<MegaOp*>(host_op);
+  KParams& p = op->p;
   op->stem_x = x;
   op->stem_h = h; op->stem_w = w; op->stem_cin = cin;
   op->stem_kh = kh; op->stem_kw = kw; op->stem_sh = sh; op->stem_sw = sw;
   op->stem_pad_t = pad_t; op->stem_pad_l = pad_l;
   op->stem_K = kh * kw * cin;
+  // the real output map replaces the plan's flat view of the patch matrix: tile_n = 1, tile_h x tile_w pixels
+  stem_tile(p.ho, p.wo, kh, kw, sh, sw, cin, &p.tile_h, &p.tile_w, &op->stem_win_rows, &op->stem_win_cols);
+  p.flat = 0;
+  p.tile_n = 1;
+  p.tiles_h = (p.ho + p.tile_h - 1) / p.tile_h;
+  p.tiles_w = (p.wo + p.tile_w - 1) / p.tile_w;
+  op->m_tiles = p.n * p.tiles_h * p.tiles_w;
+  return op->m_tiles * op->n_tiles;
 }
 
 void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]) {
@@ -1351,12 +1543,12 @@ void umma_mega_set_stem_u8(void* host_op, const uint8_t* x, const float shift[3]
 int launch_conv_stem(int nplanes, const void* dev_op, int n_tiles, bool u8, bool tf, cudaStream_t st) {
   const int stages = env_int("DEFER_STREAM_STAGES", MAX_STAGES);
   if (u8 && tf)
-    return nplanes == 2 ? launch_persist_t<2, 64, true, false, true>(dev_op, n_tiles, stages, st)
-                        : launch_persist_t<1, 64, true, false, true>(dev_op, n_tiles, stages, st);
+    return nplanes == 2 ? launch_stem_t<2, STEM_U8_TF>(dev_op, n_tiles, stages, st)
+                        : launch_stem_t<1, STEM_U8_TF>(dev_op, n_tiles, stages, st);
   if (u8)
-    return nplanes == 2 ? launch_persist_t<2, 64, true>(dev_op, n_tiles, stages, st)
-                        : launch_persist_t<1, 64, true>(dev_op, n_tiles, stages, st);
-  return nplanes == 2 ? launch_persist_t<2, 64>(dev_op, n_tiles, stages, st) : launch_persist_t<1, 64>(dev_op, n_tiles, stages, st);
+    return nplanes == 2 ? launch_stem_t<2, STEM_U8_CAFFE>(dev_op, n_tiles, stages, st)
+                        : launch_stem_t<1, STEM_U8_CAFFE>(dev_op, n_tiles, stages, st);
+  return nplanes == 2 ? launch_stem_t<2, STEM_F32>(dev_op, n_tiles, stages, st) : launch_stem_t<1, STEM_F32>(dev_op, n_tiles, stages, st);
 }
 
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st) {

@@ -63,9 +63,12 @@ int umma_mega_cluster_size();
 int launch_conv_mega(int nplanes, const void* dev_ops, int n_ops, cudaStream_t st);
 // one op on the streaming persistent kernel (deep operand ring, epilogue staged outside it)
 int launch_conv_stream(int nplanes, int bn, const void* dev_op, int n_tiles, int k_blocks, bool aff, cudaStream_t st);
-// fused stem: conv over a few-channel fp32 image with the im2col done inside the persistent kernel
-bool umma_stem_fusable(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int sh, uint32_t flags);
-void umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l);
+// fused stem: conv over a few-channel fp32 image with the im2col done inside the persistent kernel, from an image window
+// per output tile staged in shared memory.  Fusable when that window fits the kernel's window buffer.
+bool umma_stem_fusable(int fmt, int cin, int ho, int wo, int cout, int kh, int kw, int sh, int sw, uint32_t flags);
+// turns a persistent-kernel op descriptor (umma_mega_fill of the 1x1 plan over the patch matrix) into the fused stem's:
+// sets the image and the 2-D output tiling; returns the number of tiles to launch
+int umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int kh, int kw, int sh, int sw, int pad_t, int pad_l);
 // ... reading a uint8 RGB image instead, preprocessed on the fly (after umma_mega_set_stem): channel c of the conv input
 // is float(image[.., 2 - c]) + shift[c] (Keras caffe mode), or with tf float(image[.., c]) / 127.5 - 1 (Keras tf mode,
 // shift unused)

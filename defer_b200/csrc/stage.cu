@@ -87,6 +87,7 @@ struct OpRt {
   bool stem_fused = false;  // backend 4 without a patch matrix: conv_stem_kernel builds the A operand from the fp32 image
   bool stream = false;      // ... with the plan's N tile (64 | 128); false = the 64-wide persistent grid (DEFER_STREAM=0, launch_conv_persistent)
   int n_tiles64 = 0;
+  int stem_tiles = 0;       // fused stem: 2-D output tiles it launches over (umma_mega_set_stem)
   UmmaConvPlan umma;        // valid when backend == 2
   std::string kname;
   double alg_bytes = 0, alg_flops = 0;
@@ -203,8 +204,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
   switch (d.kind) {
     case DEFER_OP_CONV: {
       if (op.backend == 4 && op.stem_fused)
-        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w,
-                                op.u8_pre >= 0, op.u8_pre >= 0 && s->ops[op.u8_pre].d.mode == DEFER_PRE_TF, st);
+        return launch_conv_stem(op.umma.nplanes, L.persist_op[oi], op.stem_tiles, op.u8_pre >= 0,
+                                op.u8_pre >= 0 && s->ops[op.u8_pre].d.mode == DEFER_PRE_TF, st);
       if (op.backend == 4)
         DEFER_TRY(launch_stem_im2col(fmt, (const float*)x, L.im2col[oi], nb, bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t,
                                      d.pad_l, bo.h, bo.w, op.k_pad, st));
@@ -1022,8 +1023,8 @@ int defer_stage_finalize(defer_stage_t s) {
     {
       const int fuse = getenv("DEFER_STEM_FUSED") ? atoi(getenv("DEFER_STEM_FUSED")) : 1;
       const bool out_local = s->hop == HOP_COPY || !((d.out == s->cfg.output_buf) && !s->cfg.is_last);
-      op.stem_fused = stem && fuse && op.stream && op.umma.bn == 64 && op.umma.flat && out_local &&
-                      umma_stem_fusable(s->cfg.fmt, s->cfg.batch, bi.h, bi.w, bi.c, bo.h, bo.w, bo.c, d.kh, d.sh, d.flags);
+      op.stem_fused = stem && fuse && op.stream && op.umma.bn == 64 && out_local &&
+                      umma_stem_fusable(s->cfg.fmt, bi.c, bo.h, bo.w, bo.c, d.kh, d.kw, d.sh, d.sw, d.flags);
       if (op.stem_fused) {
         op.kname = "conv_stem_kernel";
         op.n_kernels = 1;
@@ -1049,8 +1050,8 @@ int defer_stage_finalize(defer_stage_t s) {
     }
   }
   // Fold a PREPROCESS op into the fused stem conv when that conv is the only reader of its (non-output) F32 image:
-  // the stem then reads the uint8 image and preprocesses each tap itself.  Every other path runs preprocess_kernel
-  // (preprocess_tf_kernel in tf mode).
+  // the stem then reads the uint8 image and preprocesses each value of its image window itself.  Every other path runs
+  // preprocess_kernel (preprocess_tf_kernel in tf mode).
   for (int pi = 0; pi < (int)s->ops.size(); ++pi) {
     OpRt& pre = s->ops[pi];
     if (pre.d.kind != DEFER_OP_PREPROCESS || pre.d.out == s->cfg.output_buf) continue;
@@ -1083,7 +1084,8 @@ int defer_stage_finalize(defer_stage_t s) {
       if (op.stem_fused) {
         const defer_op_desc& d = op.d;
         const Buf& bi = s->bufs[d.in0];
-        umma_mega_set_stem(host.data(), (const float*)L.buf[d.in0], bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw, d.pad_t, d.pad_l);
+        op.stem_tiles = umma_mega_set_stem(host.data(), (const float*)L.buf[d.in0], bi.h, bi.w, bi.c, d.kh, d.kw, d.sh, d.sw,
+                                           d.pad_t, d.pad_l);
         if (op.u8_pre >= 0) {
           const OpRt& pre = s->ops[op.u8_pre];
           umma_mega_set_stem_u8(host.data(), (const uint8_t*)L.buf[pre.d.in0], pre.pre_shift);
