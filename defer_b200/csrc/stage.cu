@@ -117,6 +117,9 @@ struct Lane {
   std::vector<void*> im2col;           // per op (backend 4): patch matrix scratch
   bool timed = false;
   void* peer_out = nullptr;   // HOP_COPY: this lane's input slot on the consumer GPU (destination of the hop copy)
+  // the microbatch the lane ran last (last stage: the one out_host is filled with); result() refuses any other
+  bool stepped = false;
+  uint64_t last_seq = 0;
 };
 
 // How a non-last stage's output reaches the next GPU's input slot (DEFER_HOP, read when the stage is created):
@@ -1189,6 +1192,8 @@ int defer_stage_step(defer_stage_t s, uint64_t seq) {
   }
   if (L.timed) DEFER_CUDA(cudaEventRecord(L.t1, L.stream));
   if (s->cfg.is_last) DEFER_CUDA(cudaEventRecord(L.done, L.stream));
+  L.stepped = true;
+  L.last_seq = seq;
   return DEFER_OK;
 }
 
@@ -1209,8 +1214,20 @@ int defer_stage_result(defer_stage_t s, uint64_t seq, void* host_out, uint64_t n
   DEFER_CHECK(s->cfg.is_last, "result: only the last stage returns results");
   const Buf& b = s->bufs[s->cfg.output_buf];
   DEFER_CHECK(nbytes == b.elems * 4, "result: got %llu bytes, stage output is %zu", (unsigned long long)nbytes, b.elems * 4);
+  const int lane = (int)(seq % s->cfg.depth);
+  Lane& L = s->lanes[lane];
+  // the lane's one output buffer holds only its latest microbatch: a later step on it has overwritten seq's output
+  if (!L.stepped || L.last_seq < seq) {
+    set_error("result: microbatch %llu was never stepped (lane %d last ran %s%llu)", (unsigned long long)seq, lane,
+              L.stepped ? "microbatch " : "nothing, ", (unsigned long long)L.last_seq);
+    return DEFER_ERR_STATE;
+  }
+  if (L.last_seq != seq) {
+    set_error("result: microbatch %llu is gone: lane %d has since run microbatch %llu over it (at most depth = %d microbatches "
+              "may be between step and result)", (unsigned long long)seq, lane, (unsigned long long)L.last_seq, s->cfg.depth);
+    return DEFER_ERR_STATE;
+  }
   DEFER_TRY(set_device(s));
-  Lane& L = s->lanes[seq % s->cfg.depth];
   DEFER_CUDA(cudaEventSynchronize(L.done));
   if (*reinterpret_cast<volatile int*>(L.status_host) != 0) {
     set_error("device-side flag wait timed out on device %d (upstream stage stalled or dead)", s->cfg.device);

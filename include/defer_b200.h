@@ -171,7 +171,9 @@ DEFER_API int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_
                              const void* const* host_ptrs, uint64_t nbytes_per_item);
 /* Enqueue microbatch `seq` on lane seq % depth: wait-input -> kernel chain -> hop -> flags. Async. */
 DEFER_API int defer_stage_step(defer_stage_t s, uint64_t seq);
-/* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host. */
+/* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host.  A lane keeps only the output
+ * of the latest microbatch stepped on it, so at most `depth` microbatches may be stepped from `seq` on before its result is
+ * collected: DEFER_ERR_STATE if lane seq % depth has run a later microbatch since, or never ran `seq`. */
 DEFER_API int defer_stage_result(defer_stage_t s, uint64_t seq, void* host_out, uint64_t nbytes);
 /* Convenience for single-stage use: submit + step + result. */
 DEFER_API int defer_stage_predict(defer_stage_t s, const void* host_in, uint64_t in_bytes, void* host_out, uint64_t out_bytes);

@@ -1,7 +1,8 @@
 """Worker of tests/test_gpu_dist.py: one process per GPU under torchrun.  Every rank runs the product's `Node.run`
 (CUDA-IPC link tokens, device-flag hop over NVLink); rank 0 is also the dispatcher (`DEFER.run_defer`).  Rank 0
-checks every result against the CPU oracle (<= 1e-3) and against a single-stage run of the same model on its own
-GPU (bitwise: the reference hop is a lossless codec, src/node.py:76-79,89-90,107-108)."""
+feeds a distinct seeded input per item and checks every result against a single-stage run of the same model on its own
+GPU (bitwise: the reference hop is a lossless codec, src/node.py:76-79,89-90,107-108), three of them also against the CPU
+oracle (<= 1e-3)."""
 import os
 import queue
 import sys
@@ -43,33 +44,35 @@ def main():
         t = threading.Thread(target=defer.run_defer, args=(model, cuts, in_q, out_q), daemon=True)
         t.start()
         assert defer.wait_ready(600), "pipeline did not come up"
-        x0 = applications.synthetic_input(1)
-        xs = [x0 * np.float32(1.0 + 0.1 * i) for i in range(3)]
-        for i in range(n_items):
-            in_q.put(xs[i % 3])
+        # one input per item: with inputs that repeat, a lane can hand over a stale slot and still give the right answer
+        xs = [applications.synthetic_input(1, seed=100 + i) for i in range(n_items)]
+        for x in xs:
+            in_q.put(x)
         outs = [out_q.get(timeout=120) for _ in range(n_items)]
         from oracle import keras_ref
-        refs = [keras_ref.predict(model.to_json(), model.get_weights(), x) for x in xs]
         single = StageRunner.from_model(model, device=local_rank, dtype="float32", max_batch=G, depth=1)
         try:
             whole = []
-            for x in xs:
-                xb = np.concatenate([x] * G, axis=0)
-                whole.append(single.predict(xb)[:1].copy())
+            for g in range(0, n_items, G):               # an item's result does not depend on its position in a group
+                group = xs[g:g + G]
+                y = single.predict(np.concatenate(group + [group[0]] * (G - len(group)), axis=0))
+                whole += [y[i:i + 1].copy() for i in range(len(group))]
         finally:
             single.close()
         worst = 0.0
         for i, y in enumerate(outs):
-            e = keras_ref.rel_err(y, refs[i % 3])
-            worst = max(worst, e)
-            if y.shape != (1, 1000) or e > 1e-3:
+            if y.shape != (1, 1000) or not np.array_equal(y, whole[i]):
                 ok = False
-                print(f"item {i}: shape {y.shape} rel err {e:.3e}", flush=True)
-            if not np.array_equal(y, whole[i % 3]):
-                ok = False
+                same = [j for j in range(n_items) if y.shape == (1, 1000) and np.array_equal(y, whole[j])]
                 print(f"item {i}: pipeline over {world} GPUs differs from the single-stage result "
-                      f"(max abs diff {np.max(np.abs(y - whole[i % 3])):.3e})", flush=True)
-        print(f"hop parity: {n_items} items over {world} GPUs, coalesce {G}, worst rel err vs oracle {worst:.3e}", flush=True)
+                      f"(it equals the result of items {same})", flush=True)
+        for i in (0, n_items // 2, n_items - 1):
+            e = keras_ref.rel_err(outs[i], keras_ref.predict(model.to_json(), model.get_weights(), xs[i]))
+            worst = max(worst, e)
+            if e > 1e-3:
+                ok = False
+                print(f"item {i}: rel err {e:.3e} against the oracle", flush=True)
+        print(f"hop parity: {n_items} items over {world} GPUs, coalesce {G}, worst rel err of 3 vs oracle {worst:.3e}", flush=True)
         defer.close()
         t.join(timeout=30)
     ctx.shutdown(nt)

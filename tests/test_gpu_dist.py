@@ -7,7 +7,6 @@ import subprocess
 import sys
 from pathlib import Path
 
-import numpy as np
 import pytest
 
 from defer_b200 import _cabi as A
@@ -46,22 +45,18 @@ def test_cross_process_hop_parity(coalesce):
     print(r.stdout[-500:])
 
 
-def test_pipeline_on_distinct_devices_bitwise(resnet50, x224):
-    """One process, stage i on GPU i (peer access): same answer as one stage on one GPU, bit for bit."""
+def test_pipeline_on_distinct_devices_bitwise(resnet50):
+    """One process, stage i on GPU i (peer access): each of a distinct input per microbatch gets the answer of one stage on
+    one GPU, bit for bit."""
     n = _n_gpus()
     if n < 2:
         pytest.skip("needs 2 GPUs")
-    from test_gpu_model import _oracle, _pipeline_on_one_gpu, _rel
-    from defer_b200.node import StageRunner
+    import handover_check as H
+    from test_gpu_model import _items, _oracle, _rel, _single_stage
     k = min(n, 4)
     cuts = applications.default_cuts(resnet50, k)
-    outs = _pipeline_on_one_gpu(resnet50, cuts, x224, "float32", depth=3, n_items=7, devices=list(range(k)))
-    r = StageRunner.from_model(resnet50, device=0, dtype="float32", max_batch=1, depth=1)
-    try:
-        whole = r.predict(x224)
-    finally:
-        r.close()
-    ref = _oracle(resnet50, x224)
-    for y in outs:
-        assert _rel(y, ref) <= 1e-3
-        assert np.array_equal(y, whole)
+    xs = _items(11, 700)
+    run = H.run_chain(resnet50, cuts, xs, depth=3, devices=list(range(k)))
+    assert run["status"] == ["ok"] * k
+    assert _rel(run["results"][0], _oracle(resnet50, xs[0])) <= 1e-3
+    H.check_results(run["results"], _single_stage(resnet50, xs), depth=3)

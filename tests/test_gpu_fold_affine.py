@@ -13,8 +13,9 @@ import threading
 import numpy as np
 import pytest
 
+import handover_check as H
 from defer_b200 import _cabi as A
-from defer_b200 import applications, dag_util
+from defer_b200 import applications
 from defer_b200 import keras_like as K
 from defer_b200.node import StageRunner
 
@@ -197,54 +198,26 @@ def test_folded_equals_default_bitwise(v2_models, monkeypatch):
     assert outs[None][1] == outs[0][1] and outs[0][1] - outs[1][1] == 16
 
 
-def _pipeline(model, cuts, x, dtype):
-    names = [model.input._keras_history[0].name] + list(cuts) + [model.output._keras_history[0].name]
-    parts = [dag_util.construct_model(model, names[i], names[i + 1], part_name=f"part{i+1}") for i in range(len(names) - 1)]
-    n = len(parts)
-    runners = [StageRunner.from_wire(p.to_json(), p.get_weights(), device=0, dtype=dtype, max_batch=x.shape[0], depth=2,
-                                     is_first=(i == 0), is_last=(i == n - 1), finalize=False, wait_timeout_ms=2000)
-               for i, p in enumerate(parts)]
-    try:
-        for i in range(n - 1):
-            runners[i].link_to(runners[i + 1])
-        for r in runners:
-            r.finalize()
-        kernels = [r.op_info(i)["kernel"] for r in runners for i in range(len(r.plan.ops))]
-        outs = []
-        for seq in range(3):
-            runners[0].submit(seq, x)
-            for r in runners:
-                r.step(seq)
-            outs.append(runners[-1].result(seq))
-        for r in runners:
-            r.status()
-        return outs, kernels
-    finally:
-        for r in runners:
-            r.sync()
-        for r in runners:
-            r.close()
-
-
 @pytest.mark.parametrize("hop", ["copy", "tma", "direct"])
 def test_partitions_equal_one_stage_bitwise(v2_models, hop, monkeypatch):
     """Cuts at `_preact_relu` (the stage output IS a folded affine op's output) and at `_out` Adds."""
     _knobs(monkeypatch, DEFER_HOP=hop, DEFER_FOLD_AFFINE=1)
     m = v2_models["ResNet50V2"]
-    x = applications.synthetic_input(2, seed=9)
+    xs = [applications.synthetic_input(2, seed=9 + i) for i in range(4)]
     r = StageRunner.from_model(m, device=0, dtype="float32", max_batch=2, depth=1)
     try:
-        whole = r.predict(x)
+        whole = [r.predict(x) for x in xs]
     finally:
         r.close()
     cuts = ["conv3_block1_preact_relu", "conv3_block4_out", "conv5_block1_preact_relu", "conv5_block2_out"]
-    outs, kernels = _pipeline(m, cuts, x, "float32")
-    assert any(k.startswith("affine (fused into") for k in kernels), kernels
-    for y in outs:
-        assert np.array_equal(y, whole)
+    run = H.run_chain(m, cuts, xs, depth=2)
+    assert any(k.startswith("affine (fused into") for ks in run["kernels"] for k in ks), run["kernels"]
+    assert run["status"] == ["ok"] * 5
+    H.check_results(run["results"], whole, depth=2)
 
 
 def test_coalesced_items_position_independent(v2_models, monkeypatch):
+    """Three images repeat on purpose: an item's result must not depend on its position in a coalesced group."""
     from defer_b200 import DEFER
     _knobs(monkeypatch, DEFER_FOLD_AFFINE=1)
     m = v2_models["ResNet50V2"]

@@ -9,10 +9,11 @@ arithmetic by tests/test_simt_bars_host.py).  Each test prints the fraction of i
 import numpy as np
 import pytest
 
+import handover_check as H
 import simt_bars as S
 from conv_check import FMTS, TOL, _alloc_act, _decode, _encode, _ptr, _quantise, conv_errors, conv_oracle
 from defer_b200 import _cabi as A
-from defer_b200 import applications, dag_util, keras_like as K
+from defer_b200 import applications, keras_like as K
 from defer_b200.node import StageRunner
 from plan_interp import run_op
 
@@ -421,7 +422,8 @@ def vgg_head():
 def test_vgg_head_steps_and_lanes(vgg_head, dtype):
     """Three dense layers with 32, 32 and 8 column blocks share one lane workspace: six steps over two lanes give
     identical bits (the fused kernel's arrival counters re-arm across ops, steps and lanes), and every op of both lanes
-    passes its bar against run_op on the lane's own input buffer."""
+    passes its bar against run_op on the lane's own input buffer.  The input repeats on purpose: the test asserts that
+    steps and lanes do not change the bits."""
     fmt_name = DTYPE_FMT_NAME[dtype]
     for batch in (1, 8, 32):
         x = np.random.default_rng(batch).standard_normal((batch, 7, 7, 512), dtype=np.float32)
@@ -530,6 +532,8 @@ def models():
 @pytest.mark.parametrize("dtype", ["float32", "bfloat16"])
 @pytest.mark.parametrize("name", list(PIPELINES))
 def test_pipeline_every_op(models, name, dtype, batch):
+    """Every op of every stage against run_op on the operands it read.  Both lanes get the same input on purpose: their
+    results must be identical (lane independence); the hand-over with distinct inputs is in tests/test_gpu_handover.py."""
     if name not in models:
         models.clear()                                          # one model's weights at a time
         models[name] = getattr(applications, name)()
@@ -538,20 +542,8 @@ def test_pipeline_every_op(models, name, dtype, batch):
     x = applications.synthetic_input(batch, seed=20 + batch)
     if batch > 1:
         x *= np.linspace(0.7, 1.3, batch, dtype=np.float32).reshape(batch, 1, 1, 1)
-    names = [model.input._keras_history[0].name] + cuts + [model.output._keras_history[0].name]
-    parts = [dag_util.construct_model(model, names[i], names[i + 1], part_name=f"part{i + 1}") for i in range(len(names) - 1)]
-    n = len(parts)
     depth = 2
-    runners = []
-    try:
-        for i, p in enumerate(parts):
-            runners.append(StageRunner.from_wire(p.to_json(), p.get_weights(), device=0, dtype=dtype, max_batch=batch,
-                                                 depth=depth, is_first=(i == 0), is_last=(i == n - 1), finalize=False,
-                                                 wait_timeout_ms=5000))
-        for i in range(n - 1):
-            runners[i].link_to(runners[i + 1])
-        for r in runners:
-            r.finalize()
+    with H.open_chain(model, cuts, dtype=dtype, batch=batch, depth=depth, wait_timeout_ms=5000) as runners:
         for seq in range(depth):
             runners[0].submit(seq, x)
             for r in runners:
@@ -570,16 +562,3 @@ def test_pipeline_every_op(models, name, dtype, batch):
         if name == "VGG16":
             fc1 = runners[2].plan.ops[0]
             assert fc1.kind == A.OP_DENSE and fc1.flags == A.FLAG_RELU and runners[2].plan.bufs[fc1.out][3] == A.BUF_ACT
-    finally:
-        for r in runners:
-            try:
-                r.sync()
-            except Exception:
-                pass
-        for r in runners:
-            try:
-                r.unlink()
-            except Exception:
-                pass
-        for r in runners:
-            r.close()
