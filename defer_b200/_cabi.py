@@ -17,7 +17,7 @@ LINK_TOKEN_BYTES = 256
 
 # enums (include/defer_b200.h)
 FMT_F32, FMT_BF16X2, FMT_BF16 = 0, 1, 2
-OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS = range(1, 12)
+OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS, OP_RESIZE = range(1, 13)
 FLAG_RELU, FLAG_RESIDUAL = 1, 2
 BUF_ACT, BUF_F32, BUF_U8 = 0, 1, 2
 PRE_CAFFE, PRE_TF = 0, 1
@@ -28,6 +28,8 @@ FMT_NAMES = {FMT_F32: "f32", FMT_BF16X2: "bf16x2", FMT_BF16: "bf16"}
 OP_NAMES = {OP_CONV: "conv", OP_MAXPOOL: "maxpool", OP_GAP: "gap", OP_DENSE: "dense", OP_SOFTMAX: "softmax",
             OP_AFFINE: "affine", OP_RELU: "relu", OP_ADD: "add", OP_PAD: "pad", OP_COPY: "copy",
             OP_PREPROCESS: "preprocess"}
+#: OP_NAMES covers the ops of a model and of its preprocess_input; KIND_NAMES adds RESIZE, the load_img resize in front
+KIND_NAMES = {**OP_NAMES, OP_RESIZE: "resize"}
 
 
 class BufDesc(C.Structure):
@@ -99,6 +101,7 @@ PROTOTYPES = {
     "defer_k_decode": (_i, [_i, _vp, _vp, _u64, _vp]),
     "defer_k_preprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "defer_k_preprocess_tf": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
+    "defer_k_resize": (_i, [_vp, _vp, _vp, _vp] + [_i] * 7 + [_vp]),
 }
 
 _LIB = None

@@ -121,4 +121,15 @@ int defer_k_preprocess_tf(const uint8_t* x, float* y, int n, int h, int w, int c
   return launch_preprocess_tf(x, y, (size_t)n * h * w, (cudaStream_t)stream);
 }
 
+int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
+                   int w_in, int h_out, int w_out, int c, void* stream) {
+  DEFER_CHECK(x && y && bounds && taps, "k_resize: null pointer");
+  DEFER_CHECK(n >= 1 && h_in >= 1 && w_in >= 1 && h_out >= 1 && w_out >= 1 && ksize >= 1,
+              "k_resize: bad sizes (n %d, %dx%d -> %dx%d, ksize %d)", n, h_in, w_in, h_out, w_out, ksize);
+  DEFER_CHECK(c == 3, "k_resize: the resize takes RGB images (3 channels), got %d", c);
+  DEFER_CHECK((h_in != h_out) != (w_in != w_out), "k_resize: exactly one axis must change (%dx%d -> %dx%d)", h_in, w_in,
+              h_out, w_out);
+  return launch_resize(x, y, bounds, taps, ksize, n, h_in, w_in, h_out, w_out, (cudaStream_t)stream);
+}
+
 }  // extern "C"

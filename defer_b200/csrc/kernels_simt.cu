@@ -1210,6 +1210,67 @@ int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t 
   return DEFER_OK;
 }
 
+// Keras load_img resize (DEFER_OP_RESIZE): one axis of Pillow's 8-bit separable resampling over a uint8 RGB image.
+// Output i of the axis reads source [first, first + count) with int32 taps of 22 fractional bits:
+// y = clamp((2^21 + sum x * tap) >> 22, 0, 255), the same integer arithmetic as Pillow, so the result is exact.
+// HORIZ: one thread per output pixel, reading `count` consecutive source pixels of its row (3 bytes each).
+// Vertical: one thread per output byte, reading `count` rows at a stride of w * 3 bytes - consecutive threads read
+// consecutive bytes of a row.  Tables go through the read-only path; rows are independent of the batch index.
+__device__ __forceinline__ uint8_t resize_clip8(int acc) { return (uint8_t)min(max(acc >> 22, 0), 255); }
+
+template <bool HORIZ>
+__global__ void __launch_bounds__(256) resize_u8_kernel(const uint8_t* __restrict__ x, uint8_t* __restrict__ y,
+                                                        const int32_t* __restrict__ bounds, const int32_t* __restrict__ taps,
+                                                        int ksize, int h_in, int w_in, int h_out, int w_out, size_t n_out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_out) return;
+  if constexpr (HORIZ) {                         // i = output pixel; rows of input and output correspond 1:1
+    const int xo = (int)(i % w_out);
+    const size_t row = i / w_out;
+    const int first = __ldg(bounds + 2 * xo), count = __ldg(bounds + 2 * xo + 1);
+    const int32_t* t = taps + (size_t)xo * ksize;
+    const uint8_t* src = x + (row * w_in + first) * 3;
+    int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
+    for (int k = 0; k < count; ++k) {
+      const int c = __ldg(t + k);
+      a0 += (int)__ldg(src + 3 * k) * c;
+      a1 += (int)__ldg(src + 3 * k + 1) * c;
+      a2 += (int)__ldg(src + 3 * k + 2) * c;
+    }
+    uint8_t* dst = y + i * 3;
+    dst[0] = resize_clip8(a0);
+    dst[1] = resize_clip8(a1);
+    dst[2] = resize_clip8(a2);
+  } else {                                       // i = output byte; columns (x, c) of input and output correspond 1:1
+    const size_t row_bytes = (size_t)w_out * 3;
+    const size_t col = i % row_bytes, r = i / row_bytes;
+    const int yo = (int)(r % h_out);
+    const size_t img = r / h_out;
+    const int first = __ldg(bounds + 2 * yo), count = __ldg(bounds + 2 * yo + 1);
+    const int32_t* t = taps + (size_t)yo * ksize;
+    const uint8_t* src = x + (img * h_in + first) * row_bytes + col;
+    int a = 1 << 21;
+    for (int k = 0; k < count; ++k) a += (int)__ldg(src + k * row_bytes) * __ldg(t + k);
+    y[i] = resize_clip8(a);
+  }
+}
+int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
+                  int w_in, int h_out, int w_out, cudaStream_t st) {
+  const bool horiz = w_in != w_out;
+  const size_t n_out = (size_t)n * h_out * w_out * (horiz ? 1 : 3);
+  if (n_out == 0) return DEFER_OK;
+  const unsigned grid = (unsigned)((n_out + 255) / 256);
+  if (horiz) {
+    prefer_max_smem(resize_u8_kernel<true>);
+    resize_u8_kernel<true><<<grid, 256, 0, st>>>(x, y, bounds, taps, ksize, h_in, w_in, h_out, w_out, n_out);
+  } else {
+    prefer_max_smem(resize_u8_kernel<false>);
+    resize_u8_kernel<false><<<grid, 256, 0, st>>>(x, y, bounds, taps, ksize, h_in, w_in, h_out, w_out, n_out);
+  }
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
 __global__ void __launch_bounds__(256) f32_to_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, size_t n) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) y[i] = __float2bfloat16_rn(x[i]);

@@ -266,6 +266,9 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       if (op.folded_into >= 0) return DEFER_OK;   // applied by the stem conv as it reads the image
       if (d.mode == DEFER_PRE_TF) return launch_preprocess_tf((const uint8_t*)x, (float*)y, (size_t)nb * bi.h * bi.w, st);
       return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
+    case DEFER_OP_RESIZE:
+      return launch_resize((const uint8_t*)x, (uint8_t*)y, (const int32_t*)s->d_weights[d.w_scale],
+                           (const int32_t*)s->d_weights[d.w_kernel], d.kw, nb, bi.h, bi.w, bo.h, bo.w, st);
   }
   set_error("launch_op: unknown op kind %d", d.kind);
   return DEFER_ERR_INVALID;
@@ -342,6 +345,10 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
     case DEFER_OP_ADD:
       op.alg_bytes = 2 * in_b + out_b;
       op.alg_flops = nb * bi.h * bi.w * bi.c;
+      break;
+    case DEFER_OP_RESIZE:   // + the two int32 tables
+      op.alg_bytes = in_b + out_b + (double)s->weight_bytes[d.w_scale] + (double)s->weight_bytes[d.w_kernel];
+      op.alg_flops = 2.0 * nb * bo.h * bo.w * bo.c * d.kw;
       break;
     default:
       op.alg_bytes = in_b + out_b;
@@ -424,9 +431,13 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       set_error("buffer %d: bad descriptor (%d,%d,%d,elem %d)", i, b.h, b.w, b.c, b.elem);
       return fail(DEFER_ERR_INVALID);
     }
-    if (b.elem == DEFER_BUF_U8 && !(cfg->is_first && i == cfg->input_buf)) {
-      set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer", i);
-      return fail(DEFER_ERR_INVALID);
+    if (b.elem == DEFER_BUF_U8) {   // the first stage's image, or that image resized
+      bool resized = false;
+      for (int j = 0; j < n_ops; ++j) resized |= ops[j].out == i && ops[j].kind == DEFER_OP_RESIZE;
+      if (!cfg->is_first || (i != cfg->input_buf && !resized)) {
+        set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE op", i);
+        return fail(DEFER_ERR_INVALID);
+      }
     }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;
     b.bytes = buf_bytes(b, cfg->fmt);
@@ -491,8 +502,9 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     const Buf& bi = s->bufs[d.in0];
     const Buf& bo = s->bufs[d.out];
-    if ((bi.elem == DEFER_BUF_U8 && d.kind != DEFER_OP_PREPROCESS) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_U8)) {
-      set_error("op %d: only a PREPROCESS op may read the U8 input buffer (as in0)", i);
+    if ((bi.elem == DEFER_BUF_U8 && d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE) ||
+        (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_U8)) {
+      set_error("op %d: only a RESIZE or PREPROCESS op may read a U8 buffer (as in0)", i);
       return fail(DEFER_ERR_INVALID);
     }
     if (d.kind != DEFER_OP_PREPROCESS && d.mode != 0) {
@@ -614,6 +626,37 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         }
         memcpy(op.pre_shift, weight_ptrs[d.w_shift], sizeof op.pre_shift);
         break;
+      case DEFER_OP_RESIZE: {
+        op.kname = "resize_u8_kernel";
+        if (bi.elem != DEFER_BUF_U8 || bo.elem != DEFER_BUF_U8 || bi.c != 3 || bo.c != 3) {
+          set_error("op %d (resize): needs U8 buffers with 3 channels (in elem %d c %d, out elem %d c %d)", i, bi.elem, bi.c,
+                    bo.elem, bo.c);
+          return fail(DEFER_ERR_INVALID);
+        }
+        if ((bi.h != bo.h) == (bi.w != bo.w) || d.in1 >= 0 || d.flags || d.w_shift >= 0) {
+          set_error("op %d (resize): exactly one axis must change (%dx%d -> %dx%d), no in1 / flags / w_shift", i, bi.h, bi.w,
+                    bo.h, bo.w);
+          return fail(DEFER_ERR_INVALID);
+        }
+        const bool horiz = bi.w != bo.w;
+        const int in_len = horiz ? bi.w : bi.h, out_len = horiz ? bo.w : bo.h, ksize = d.kw;
+        if (ksize < 1 || d.w_scale < 0 || d.w_kernel < 0 || s->weight_bytes[d.w_scale] != (size_t)out_len * 2 * 4 ||
+            s->weight_bytes[d.w_kernel] != (size_t)out_len * ksize * 4) {
+          set_error("op %d (resize): w_scale must hold int32 [%d, 2] (first, count) and w_kernel int32 [%d, kw = %d] taps", i,
+                    out_len, out_len, ksize);
+          return fail(DEFER_ERR_INVALID);
+        }
+        const int32_t* b = static_cast<const int32_t*>(weight_ptrs[d.w_scale]);
+        for (int o = 0; o < out_len; ++o) {
+          const int first = b[2 * o], count = b[2 * o + 1];
+          if (first < 0 || count < 1 || count > ksize || first > in_len - count) {
+            set_error("op %d (resize): output %d reads source [%d, %d + %d); needs 0 <= first, 1 <= count <= kw = %d, "
+                      "first + count <= %d", i, o, first, first, count, ksize, in_len);
+            return fail(DEFER_ERR_INVALID);
+          }
+        }
+        break;
+      }
       default:
         set_error("op %d: unknown kind %d", i, d.kind);
         return fail(DEFER_ERR_INVALID);

@@ -14,7 +14,7 @@ What changed underneath:
 
 Non-reference additions: ``close()`` / context manager (the reference can only be killed), keyword-only
 ``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1),
-``coalesce`` and ``preprocess``.
+``coalesce``, ``preprocess``, ``image_size`` and ``interpolation``.
 
 Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the host before every ``input_q.put``
 (``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
@@ -23,6 +23,13 @@ GPU, bit for bit what ``applications.preprocess_input`` gives on the host; an im
 instead of 4.  ``preprocess="tf"`` does the same with the ResNet V2 family's transform
 (``applications.resnet_v2_preprocess_input``), and is refused for a model whose Keras preprocessing is caffe mode.
 Other item dtypes are refused.
+
+Resizing: the same driver loads every image with ``load_img(path, target_size=(224, 224))``, a Pillow resize on the host.
+With ``image_size=(h, w)`` (and ``preprocess``) queue items are uint8 images of that size, e.g. camera frames, and the
+first stage resizes them to the model input on its GPU before preprocessing, bit for bit what
+``applications.resize_image(item, (H, W), interpolation)`` gives; ``interpolation`` takes the names ``load_img`` accepts
+(default ``"nearest"``, as in Keras).  One pipeline takes one image size.  An ``image_size`` equal to the model input
+changes nothing, as Keras does not resize then.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -36,12 +43,13 @@ from __future__ import annotations
 import queue
 import threading
 import time
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 import numpy as np
 
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
+from .resize import check_interpolation, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
 
@@ -49,11 +57,20 @@ from .node import DTYPE_TO_FMT, StageRunner, parse_device
 class DEFER:
     def __init__(self, computeNodes, *, dtype: str = "float32", depth: int = 4, batch: Optional[int] = None,
                  coalesce: int = 1, linger_us: float = 200.0, conv_backend: int = 0, dist=None,
-                 wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None) -> None:
+                 wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None,
+                 image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest") -> None:
         if preprocess is not None:
             check_preprocess(preprocess)
+        check_interpolation(interpolation)
+        if image_size is not None:
+            image_size = check_size(image_size)
+            if preprocess is None:
+                raise ValueError(f"image_size={image_size}: resizing takes uint8 images and needs preprocess= (float items "
+                                 "are already preprocessed, and Keras resizes before preprocessing)")
         self.computeNodes = list(computeNodes)
         self.preprocess = preprocess        # None | "caffe" | "tf": uint8 queue items, preprocessed on stage 0's GPU
+        self.image_size = image_size        # None | (h, w) of the uint8 queue items, resized on stage 0's GPU
+        self.interpolation = interpolation
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -113,7 +130,9 @@ class DEFER:
                                          "next_node": str(next_node), "fmt": self.dtype, "batch": batch,
                                          "depth": self.depth, "conv_backend": self.conv_backend,
                                          "wait_timeout_ms": self.wait_timeout_ms,
-                                         "preprocess": self.preprocess if i == 0 else None})
+                                         "preprocess": self.preprocess if i == 0 else None,
+                                         "image_size": self.image_size if i == 0 else None,
+                                         "interpolation": self.interpolation})
             self.dist.wait_all_ready()      # the 1-byte ACK of dispatcher.py:64-65
             return
         runners = []
@@ -124,7 +143,9 @@ class DEFER:
                                       max_batch=batch, depth=self.depth, is_first=(i == 0), is_last=(i == n - 1),
                                       finalize=False, conv_backend=self.conv_backend,
                                       wait_timeout_ms=self.wait_timeout_ms,
-                                      preprocess=self.preprocess if i == 0 else None)
+                                      preprocess=self.preprocess if i == 0 else None,
+                                      image_size=self.image_size if i == 0 else None,
+                                      interpolation=self.interpolation)
             r.name = f"part{i+1}"
             runners.append(r)
         for i in range(n - 1):              # next hop = nodeIPs[i+1] (dispatcher.py:51-55)

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 import time
-from typing import Dict, List, Optional, Sequence, Union
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -79,6 +79,8 @@ class StageRunner:
         # the Keras mode of the stage's PREPROCESS op, for messages (None: no preprocessing; the library refuses a bad mode)
         pre_modes = [o.mode for o in plan.ops if o.kind == A.OP_PREPROCESS]
         self.preprocess = {v: k for k, v in A.PRE_MODES.items()}.get(pre_modes[0]) if pre_modes else None
+        # planned with image_size=: the stage resizes its images to the model input first (for messages)
+        self.resizes = any(o.kind == A.OP_RESIZE for o in plan.ops)
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
         self.out_elems = int(np.prod(self.out_shape))
@@ -107,10 +109,13 @@ class StageRunner:
     @classmethod
     def from_model(cls, model: K.Model, device=0, dtype: str = "float32", max_batch: int = 1, depth: int = 1,
                    is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
-                   **kw) -> "StageRunner":
+                   image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest", **kw) -> "StageRunner":
         """``preprocess="caffe"`` or ``"tf"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the
-        stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family)."""
-        plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess)
+        stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family).
+        ``image_size=(h, w)`` (with ``preprocess``): inputs are uint8 RGB images of that size, resized on the GPU to the
+        model's input as Keras' ``load_img(target_size=..., interpolation=...)`` does (``resize.resize_image``)."""
+        plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
+                          interpolation=interpolation)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
                 is_last=is_last, name=model.name, **kw)
@@ -158,7 +163,7 @@ class StageRunner:
                                 "img_to_array(img).astype(np.uint8), not preprocessed or float data")
             if x.ndim != 4 or tuple(x.shape[1:]) != self.in_shape[1:]:   # e.g. channels-first: same bytes, wrong image
                 raise ValueError(f"{self.name}: image shape {tuple(x.shape)} is not (k,) + {self.in_shape[1:]} "
-                                 "(channels-last RGB)")
+                                 "(channels-last RGB" + (f", image_size={self.in_shape[1:3]}" if self.resizes else "") + ")")
             if not x.flags["C_CONTIGUOUS"]:
                 x = np.ascontiguousarray(x)
                 self._keep = x
@@ -381,7 +386,9 @@ class Node:
                                        depth=msg["depth"], is_first=(rank == 0), is_last=(rank == world - 1),
                                        finalize=False, conv_backend=msg.get("conv_backend", 0),
                                        wait_timeout_ms=msg.get("wait_timeout_ms", 0),
-                                       preprocess=msg.get("preprocess") if rank == 0 else None)
+                                       preprocess=msg.get("preprocess") if rank == 0 else None,
+                                       image_size=msg.get("image_size") if rank == 0 else None,
+                                       interpolation=msg.get("interpolation", "nearest"))
         ns.model = runner                               # src/node.py:38
         self.runner = runner
         # wire the hop: my consumer gives me its input-side token, I give it my output-side token

@@ -17,7 +17,9 @@ not the stage output - otherwise that tensor must exist in memory.
 
 With ``preprocess="caffe"`` or ``"tf"`` (first stage only) the stage input is a uint8 RGB image and a
 ``PREPROCESS`` op (Keras' ``preprocess_input`` in that mode) writes the fp32 tensor the rest of the plan reads;
-the library folds it into the fused RGB stem when it can.
+the library folds it into the fused RGB stem when it can.  With ``image_size=(h, w)`` as well, the stage input is a uint8
+image of that size and up to two ``RESIZE`` ops (width, then height: Keras' ``load_img(target_size=...)`` through Pillow,
+tables from ``resize.resize_tables``) bring it to the model's input size before ``PREPROCESS``.
 """
 from __future__ import annotations
 
@@ -29,6 +31,7 @@ import numpy as np
 from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
+from .resize import check_interpolation, check_size, resize_tables
 
 
 def same_pad(size: int, k: int, s: int) -> Tuple[int, int]:
@@ -74,7 +77,7 @@ class Plan:
     def describe(self) -> str:
         lines = []
         for i, op in enumerate(self.ops):
-            lines.append(f"[{i:2d}] {A.OP_NAMES[op.kind]:8s} b{op.in0}" + (f"+b{op.in1}" if op.in1 >= 0 else "") +
+            lines.append(f"[{i:2d}] {A.KIND_NAMES[op.kind]:8s} b{op.in0}" + (f"+b{op.in1}" if op.in1 >= 0 else "") +
                          f" -> b{op.out} {self.bufs[op.out][:3]} flags={op.flags} <- {','.join(op.layers)}")
         return "\n".join(lines)
 
@@ -88,12 +91,19 @@ def _hwc(shape) -> Tuple[int, int, int]:
     raise ValueError(f"unsupported tensor rank {shape}")
 
 
-def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None) -> Plan:
+def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None,
+               image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest") -> Plan:
     if preprocess is not None:
         check_preprocess(preprocess)
         if not is_first:
             raise ValueError(f"preprocess={preprocess!r}: only the first stage takes images")
         check_model_preprocess(model, preprocess)
+    check_interpolation(interpolation)
+    if image_size is not None:
+        image_size = check_size(image_size)
+        if preprocess is None:
+            raise ValueError(f"image_size={image_size}: resizing takes uint8 images and needs preprocess= (float items "
+                             "are already preprocessed, and Keras resizes before preprocessing)")
     nodes = list(model.iter_nodes())
     # names as recorded at map time (tensor histories may be re-tagged later by Input(tensor=...))
     order = [l.name for l, _ in nodes]
@@ -128,6 +138,10 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
 
     def add_weight(a: np.ndarray) -> int:
         weights.append(np.ascontiguousarray(a, dtype=np.float32))
+        return len(weights) - 1
+
+    def add_table(a: np.ndarray) -> int:       # RESIZE tables stay int32
+        weights.append(np.ascontiguousarray(a, dtype=np.int32))
         return len(weights) - 1
 
     def emit(op: PlanOp) -> PlanOp:
@@ -176,14 +190,29 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         return materialise(t), (0, 0, 0, 0), []
 
     # stage input
+    input_shape = tuple(shapes[in_name][1:])
     if preprocess is None:
         tensor_buf[in_name] = new_buf(shapes[in_name], A.BUF_F32 if is_first else A.BUF_ACT)
         input_buf = tensor_buf[in_name]
     else:
         if _hwc(shapes[in_name])[2] != 3 or len(shapes[in_name]) != 4:
             raise ValueError(f"preprocess={preprocess!r}: the input must be an RGB image (h, w, 3), got {shapes[in_name][1:]}")
-        input_buf = new_buf(shapes[in_name], A.BUF_U8)
-        op = emit(PlanOp(A.OP_PREPROCESS, input_buf, new_buf(shapes[in_name], A.BUF_F32),
+        H, W, _ = _hwc(shapes[in_name])
+        h, w = image_size if image_size is not None else (H, W)
+        input_shape = (h, w, 3)
+        input_buf = img = new_buf((None,) + input_shape, A.BUF_U8)
+        # Pillow resizes the width first and skips an axis whose size does not change (so does Keras: no resize at all
+        # when the image is already at target_size)
+        for axis, n_in, n_out, shape in (("width", w, W, (h, W, 3)), ("height", h, H, (H, W, 3))):
+            if n_in == n_out:
+                continue
+            first, count, coef = resize_tables(n_in, n_out, interpolation)
+            op = emit(PlanOp(A.OP_RESIZE, img, new_buf((None,) + shape, A.BUF_U8), kw=coef.shape[1],
+                             layers=[f"load_img({axis} {n_in}->{n_out}, {interpolation})"]))
+            op.w_scale = add_table(np.stack([first, count], axis=1))
+            op.w_kernel = add_table(coef)
+            img = op.out
+        op = emit(PlanOp(A.OP_PREPROCESS, img, new_buf(shapes[in_name], A.BUF_F32),
                          mode=A.PRE_MODES[preprocess], layers=[f"preprocess_input({preprocess})"]))
         if preprocess == "caffe":                     # tf: Keras hard-codes 127.5 and 1, no weights
             op.w_shift = add_weight(caffe_shift())
@@ -356,5 +385,5 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         if op.shift is not None:
             op.w_shift = add_weight(op.shift.astype(np.float32))
     return Plan(bufs=bufs, ops=ops, weights=weights, input_buf=input_buf, output_buf=out_buf,
-                input_shape=tuple(shapes[in_name][1:]), output_shape=tuple(shapes[out_name][1:]),
+                input_shape=input_shape, output_shape=tuple(shapes[out_name][1:]),
                 tensor_buf=dict(tensor_buf))

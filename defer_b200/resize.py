@@ -1,0 +1,177 @@
+"""Keras ``load_img(target_size=..., interpolation=...)`` resize, restated from Pillow's ``Image.resize`` on uint8 images.
+
+This module owns the per-axis table format that both the host restatement (``resize_image``) and the planner's
+``DEFER_OP_RESIZE`` use, so the two cannot drift apart.  For one axis of ``in_len`` source pixels resized to ``out_len``,
+``resize_tables`` gives int32 arrays
+
+* ``first[out]``        - the first source index output ``i`` reads,
+* ``count[out]``        - how many consecutive source indices it reads (``1 <= count <= ksize``, ``first + count <= in_len``),
+* ``coef[out, ksize]``  - their weights in fixed point with ``PRECISION_BITS`` fractional bits (zero past ``count``),
+
+and one pass over that axis computes, per channel, ``clamp((2**21 + sum_k src[first + k] * coef[k]) >> 22, 0, 255)``.
+
+The filters are Pillow's 8-bit path (``libImaging/Resample.c``): support scaled by ``max(in/out, 1)``, weights normalised
+by their sequential sum in double precision and rounded half away from zero.  Pillow resizes the horizontal axis first,
+rounds to uint8, then the vertical axis, and skips an axis whose size does not change; ``resize_image`` does the same.
+``nearest`` is Pillow's affine nearest path: the source index is ``int(xo)``, where ``xo`` starts at ``0.5 * in/out`` and
+accumulates ``+= in/out`` in double precision (the closed form ``floor((i + 0.5) * in/out)`` differs from it at some
+sizes).  It fits the same tables with one tap of weight ``1 << 22``: an exact gather, so a 2-D nearest resize is the
+horizontal gather followed by the vertical one.
+"""
+from __future__ import annotations
+
+import math
+from typing import Tuple
+
+import numpy as np
+
+#: the ``interpolation=`` names Keras' ``load_img`` accepts (its default is "nearest")
+INTERPOLATIONS = ("nearest", "bilinear", "bicubic", "hamming", "box", "lanczos")
+#: fractional bits of the fixed-point weights (Pillow: 32 - 8 - 2)
+PRECISION_BITS = 22
+
+
+def _box(x: float) -> float:
+    return 1.0 if -0.5 < x <= 0.5 else 0.0
+
+
+def _bilinear(x: float) -> float:
+    x = abs(x)
+    return 1.0 - x if x < 1.0 else 0.0
+
+
+_F32_054 = float(np.float32(0.54))   # Pillow writes 0.54f and 0.46f: single-precision constants in a double expression
+_F32_046 = float(np.float32(0.46))
+
+
+def _hamming(x: float) -> float:
+    x = abs(x)
+    if x == 0.0:
+        return 1.0
+    if x >= 1.0:
+        return 0.0
+    x = x * math.pi
+    return math.sin(x) / x * (_F32_054 + _F32_046 * math.cos(x))
+
+
+def _bicubic(x: float) -> float:
+    a = -0.5
+    x = abs(x)
+    if x < 1.0:
+        return ((a + 2.0) * x - (a + 3.0)) * x * x + 1
+    if x < 2.0:
+        return (((x - 5) * x + 8) * x - 4) * a
+    return 0.0
+
+
+def _sinc(x: float) -> float:
+    if x == 0.0:
+        return 1.0
+    x = x * math.pi
+    return math.sin(x) / x
+
+
+def _lanczos(x: float) -> float:
+    return _sinc(x) * _sinc(x / 3) if -3.0 <= x < 3.0 else 0.0
+
+
+#: name -> (filter, support)
+_FILTERS = {"box": (_box, 0.5), "bilinear": (_bilinear, 1.0), "hamming": (_hamming, 1.0),
+            "bicubic": (_bicubic, 2.0), "lanczos": (_lanczos, 3.0)}
+
+
+def check_interpolation(name) -> None:
+    if name not in INTERPOLATIONS:
+        raise ValueError(f"interpolation={name!r}: Keras' load_img accepts {', '.join(map(repr, INTERPOLATIONS))}")
+
+
+def check_size(size, what: str = "image_size") -> Tuple[int, int]:
+    """``size`` as ``(h, w)`` of positive ints, or a ValueError naming ``what``."""
+    try:
+        h, w = (int(v) for v in size)
+        ok = (h, w) == tuple(size)
+    except (TypeError, ValueError):
+        ok = False
+    if not ok or h < 1 or w < 1:
+        raise ValueError(f"{what}={size!r}: expected (height, width), two positive integers")
+    return h, w
+
+
+def resize_tables(in_len: int, out_len: int, interpolation: str = "nearest") -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """``(first, count, coef)`` of one axis: int32 ``[out_len]``, ``[out_len]`` and ``[out_len, ksize]`` (module docstring).
+
+    Plain Python floats on purpose: every step is the double-precision operation Pillow's C code performs, in its order
+    (a vectorised sum or a SIMD ``sin`` could round differently)."""
+    check_interpolation(interpolation)
+    if in_len < 1 or out_len < 1:
+        raise ValueError(f"resize_tables: sizes must be positive, got {in_len} -> {out_len}")
+    scale = in_len / out_len
+    first = np.empty(out_len, np.int32)
+    count = np.empty(out_len, np.int32)
+    if interpolation == "nearest":
+        xo = scale * 0.5
+        for i in range(out_len):
+            # Pillow's affine nearest fills a pixel whose index leaves the image with 0; the accumulated position stays
+            # below in_len for any size this engine can hold, and the clamp keeps the table valid regardless
+            first[i] = min(int(xo), in_len - 1)
+            xo += scale
+        count[:] = 1
+        return first, count, np.full((out_len, 1), 1 << PRECISION_BITS, np.int32)
+    filt, filter_support = _FILTERS[interpolation]
+    filterscale = max(scale, 1.0)
+    support = filter_support * filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    ss = 1.0 / filterscale
+    coef = np.zeros((out_len, ksize), np.int32)
+    one = float(1 << PRECISION_BITS)
+    for i in range(out_len):
+        center = (i + 0.5) * scale
+        lo = max(int(center - support + 0.5), 0)
+        hi = min(int(center + support + 0.5), in_len)
+        w = [filt((k + lo - center + 0.5) * ss) for k in range(hi - lo)]
+        ww = 0.0
+        for v in w:
+            ww += v
+        for k, v in enumerate(w):
+            if ww != 0.0:
+                v /= ww
+            coef[i, k] = int(v * one - 0.5) if v < 0 else int(v * one + 0.5)   # int() truncates, as the C cast does
+        first[i], count[i] = lo, hi - lo
+    return first, count, coef
+
+
+def resize_axis(x: np.ndarray, axis: int, first: np.ndarray, count: np.ndarray, coef: np.ndarray) -> np.ndarray:
+    """One pass of the tables over ``axis`` of the uint8 array ``x`` (what ``DEFER_OP_RESIZE`` computes on the GPU)."""
+    x = np.asarray(x)
+    if x.dtype != np.uint8:
+        raise TypeError(f"resize_axis: expected uint8, got {x.dtype}")
+    in_len = x.shape[axis]
+    acc = np.full(x.shape[:axis] + (len(first),) + x.shape[axis + 1:], 1 << (PRECISION_BITS - 1), np.int64)
+    bshape = [1] * x.ndim
+    bshape[axis] = len(first)
+    for k in range(coef.shape[1]):
+        idx = np.minimum(first + k, in_len - 1)                  # taps past `count` have weight 0
+        w = np.where(k < count, coef[:, k], 0).astype(np.int64).reshape(bshape)
+        acc += np.take(x, idx, axis=axis).astype(np.int64) * w
+    return np.clip(acc >> PRECISION_BITS, 0, 255).astype(np.uint8)
+
+
+def resize_image(x: np.ndarray, target_size, interpolation: str = "nearest") -> np.ndarray:
+    """Resize uint8 RGB ``x`` of shape ``(h, w, 3)`` or ``(n, h, w, 3)`` to ``target_size = (height, width)``, bit for bit
+    as Keras' ``load_img(path, target_size=..., interpolation=...)`` does with Pillow's ``Image.resize``.
+
+    Horizontal pass first, then vertical; an axis whose size does not change is not touched, and an image already at
+    ``target_size`` comes back as a copy.  ``DEFER(..., image_size=(h, w), interpolation=...)`` runs the same passes on
+    the GPU."""
+    check_interpolation(interpolation)
+    th, tw = check_size(target_size, "target_size")
+    x = np.asarray(x)
+    if x.dtype != np.uint8 or x.ndim not in (3, 4) or x.shape[-1] != 3:
+        raise ValueError(f"resize_image: expected a uint8 RGB image (h, w, 3) or (n, h, w, 3), got {x.dtype} {x.shape}")
+    h_ax, w_ax = x.ndim - 3, x.ndim - 2
+    y = x.copy()
+    if x.shape[w_ax] != tw:
+        y = resize_axis(y, w_ax, *resize_tables(x.shape[w_ax], tw, interpolation))
+    if x.shape[h_ax] != th:
+        y = resize_axis(y, h_ax, *resize_tables(x.shape[h_ax], th, interpolation))
+    return y

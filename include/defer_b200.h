@@ -63,10 +63,17 @@ typedef enum defer_op_kind {
   DEFER_OP_ADD = 8,      /* standalone Add of two tensors [+ relu]                                            */
   DEFER_OP_PAD = 9,      /* standalone ZeroPadding2D                                                          */
   DEFER_OP_COPY = 10,    /* identity / Flatten / format cast                                                  */
-  DEFER_OP_PREPROCESS = 11 /* Keras preprocess_input: in0 = U8 image (c == 3), out = F32 of the same shape;     */
+  DEFER_OP_PREPROCESS = 11, /* Keras preprocess_input: in0 = U8 image (c == 3), out = F32 of the same shape;    */
                          /* `mode` DEFER_PRE_CAFFE: w_shift = 3 fp32 values in output-channel order,            */
                          /*   y[..., c] = float(x[..., 2 - c]) + shift[c]  (RGB -> BGR, minus the ImageNet mean)  */
                          /* `mode` DEFER_PRE_TF: no weights, y = float(x) / 127.5 - 1 in fp32 (ResNet V2)       */
+  DEFER_OP_RESIZE = 12   /* Keras load_img(target_size=...) resize, one axis of Pillow's 8-bit resampling:       */
+                         /*   in0 = U8 (h_in, w_in, 3), out = U8 (h_out, w_out, 3), exactly one of h / w differs  */
+                         /*   (that is the axis; `mode` 0).  Weights are int32 tables of that axis:               */
+                         /*   w_scale  = [out_len, 2] (first, count): output i reads source [first, first + count) */
+                         /*   w_kernel = [out_len, kw] fixed-point taps, 22 fractional bits;  kw = ksize          */
+                         /*   y[i] = clamp((2^21 + sum_{k < count} x[first + k] * tap[k]) >> 22, 0, 255) per     */
+                         /*   channel; 0 <= first, 1 <= count <= kw, first + count <= in_len (checked at create)  */
 } defer_op_kind;
 
 /* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
@@ -79,7 +86,8 @@ typedef enum defer_op_kind {
 /* Buffer element type. */
 #define DEFER_BUF_ACT 0   /* stage activation format (defer_fmt of the stage) */
 #define DEFER_BUF_F32 1   /* plain fp32 regardless of the stage format (image in, probabilities out) */
-#define DEFER_BUF_U8  2   /* uint8 NHWC, 1 B/elem: only the first stage's input buffer, read only by DEFER_OP_PREPROCESS */
+#define DEFER_BUF_U8  2   /* uint8 NHWC, 1 B/elem, first stage only: its input buffer or the output of a DEFER_OP_RESIZE; */
+                          /* read only by DEFER_OP_RESIZE and DEFER_OP_PREPROCESS                                          */
 
 /* One logical tensor of the plan.  Shapes are per sample, NHWC; vectors use h = w = 1. */
 typedef struct defer_buf_desc {
@@ -95,8 +103,8 @@ typedef struct defer_op_desc {
   int32_t kh, kw, sh, sw;  /* CONV / MAXPOOL window and stride */
   int32_t pad_t, pad_l, pad_b, pad_r; /* explicit zero padding applied to in0 (fused ZeroPadding2D / 'same') */
   uint32_t flags;          /* DEFER_FLAG_* */
-  int32_t w_kernel;        /* CONV: fp32 HWIO kernel;  DENSE: fp32 (in,out) kernel */
-  int32_t w_scale;         /* CONV / AFFINE: fp32 per-channel scale (NULL id -1 = ones) */
+  int32_t w_kernel;        /* CONV: fp32 HWIO kernel;  DENSE: fp32 (in,out) kernel;  RESIZE: int32 taps */
+  int32_t w_scale;         /* CONV / AFFINE: fp32 per-channel scale (NULL id -1 = ones);  RESIZE: int32 (first, count) */
   int32_t w_shift;         /* CONV / AFFINE / PREPROCESS: fp32 per-channel shift;  DENSE: bias */
   int32_t mode;            /* PREPROCESS: DEFER_PRE_*;  every other kind: 0 */
 } defer_op_desc;
@@ -129,7 +137,8 @@ DEFER_API int defer_device_count(int* count);
 DEFER_API int defer_device_info(int device, char* name, int name_len, int* sm_count, int* cc, uint64_t* hbm_bytes);
 
 /* ---- stage life cycle  (replaces model_from_json + set_weights, src/node.py:31-38) ---------- */
-/* weights: host pointers to fp32 arrays, copied; the caller keeps ownership of host memory. */
+/* weights: host pointers to fp32 arrays (int32 for the tables of DEFER_OP_RESIZE), copied; the caller keeps ownership
+ * of host memory. */
 DEFER_API int defer_stage_create(const defer_stage_config* cfg,
                        const defer_buf_desc* bufs, int n_bufs,
                        const defer_op_desc* ops, int n_ops,
@@ -245,6 +254,10 @@ DEFER_API int defer_k_preprocess(const uint8_t* x, const float* shift, float* y,
 /* Keras tf-mode preprocess_input (DEFER_OP_PREPROCESS, DEFER_PRE_TF): uint8 NHWC image (c == 3) -> fp32,
  * y = fl32(fl32(float(x) / 127.5) - 1), channels in place */
 DEFER_API int defer_k_preprocess_tf(const uint8_t* x, float* y, int n, int h, int w, int c, void* stream);
+/* One pass of DEFER_OP_RESIZE: uint8 NHWC (n, h_in, w_in, c == 3) -> (n, h_out, w_out, 3), exactly one axis changing.
+ * bounds = int32 [out_len, 2] (first, count) and taps = int32 [out_len, ksize] on the device (not validated here). */
+DEFER_API int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n,
+                             int h_in, int w_in, int h_out, int w_out, int c, void* stream);
 
 #ifdef __cplusplus
 }

@@ -9,12 +9,22 @@ round):
      applications.preprocess_input (caffe) or applications.resnet_v2_preprocess_input (tf)
   c  uint8 items on a full input queue, DEFER(preprocess=mode): the first stage preprocesses on the GPU
 
+With --image-size HxW (and --interpolation NAME, default nearest) the items are uint8 frames of that size, as a camera
+gives them, and two more arms run in the same alternation:
+
+  d  uint8 frames, Pillow's Image.resize to 224 x 224 in the feeding thread (Keras load_img's resize, what a
+     reference-style driver does), DEFER(preprocess=mode)
+  e  uint8 frames on a full input queue, DEFER(preprocess=mode, image_size=..., interpolation=...): the first stage
+     resizes and preprocesses on the GPU
+
 It prints one JSON line: end-to-end inferences/s per arm (median, min, max over the rounds), H2D bytes per item, the
 device time of the fp32 fused stem, the uint8 fused stem of the mode and its standalone preprocessing kernel (time_op,
-L2 flushed), the host time of one preprocessing call, and the card's name and power limit (read-only nvidia-smi query).
+L2 flushed), the host time of one preprocessing call, and the card's name and power limit (read-only nvidia-smi query);
+with --image-size also the host time of one Pillow resize and the time_op of each RESIZE op at 32 frames.
 
     python tools/ingress_bench.py [--model resnet50 --preprocess caffe] [--items 640] [--reps 3]
     python tools/ingress_bench.py --model resnet50v2 --preprocess tf
+    python tools/ingress_bench.py --image-size 480x640 --interpolation bilinear
 """
 from __future__ import annotations
 
@@ -55,9 +65,9 @@ def card():
 
 
 class Arm:
-    def __init__(self, model, preprocess, host_preprocess):
+    def __init__(self, model, preprocess, host_preprocess, **defer_kw):
         self.host_preprocess = host_preprocess
-        self.defer = DEFER([0], depth=DEPTH, coalesce=G, linger_us=2000, preprocess=preprocess)
+        self.defer = DEFER([0], depth=DEPTH, coalesce=G, linger_us=2000, preprocess=preprocess, **defer_kw)
         self.in_q, self.out_q = queue.Queue(), queue.Queue()
         self.err = []
         self.thread = threading.Thread(target=self._run, args=(model,), daemon=True)
@@ -126,6 +136,34 @@ def stem_times(model, mode, iters):
     return out
 
 
+def pillow_resize(size, interpolation):
+    """Keras load_img's resize of one (1, h, w, 3) uint8 item to ``size`` through Pillow, as a feeding thread does it."""
+    from PIL import Image
+    method = getattr(Image, interpolation.upper())
+
+    def fn(x):
+        return np.asarray(Image.fromarray(x[0]).resize((size[1], size[0]), method))[None]
+    return fn
+
+
+def resize_times(model, mode, image_size, interpolation, iters):
+    """time_op (us) of each RESIZE op at the benchmarked microbatch (32 frames), L2 flushed."""
+    r = StageRunner.from_model(model, device=0, dtype="float32", max_batch=G, depth=1, preprocess=mode,
+                               image_size=image_size, interpolation=interpolation)
+    out = {}
+    try:
+        r.predict(applications.synthetic_image(G, image_size + (3,), seed=1))
+        for i, op in enumerate(r.plan.ops):
+            if r.op_info(i)["kernel"] != "resize_u8_kernel":
+                continue
+            ts = [r.time_op(i, iters=iters, flush_l2=True) for _ in range(3)]
+            out[op.layers[0]] = {"us": round(statistics.median(ts), 2), "spread_us": round(max(ts) - min(ts), 2),
+                                 "alg_bytes": r.op_info(i)["alg_bytes"]}
+    finally:
+        r.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--items", type=int, default=640, help="queue items per timed round (batch-1 images)")
@@ -134,9 +172,18 @@ def main():
     ap.add_argument("--model", choices=sorted(MODELS), default="resnet50")
     ap.add_argument("--preprocess", choices=sorted(HOST_PREPROCESS), default="caffe",
                     help="Keras preprocessing mode (the model's own: caffe for resnet50, tf for resnet50v2)")
+    ap.add_argument("--image-size", default=None, help="HxW of uint8 frames for arms d and e, e.g. 480x640")
+    ap.add_argument("--interpolation", choices=applications.INTERPOLATIONS, default="nearest")
     args = ap.parse_args()
     if args.reps < 3:
         ap.error("--reps must be >= 3")
+    image_size = None
+    if args.image_size:
+        try:
+            image_size = tuple(int(v) for v in args.image_size.lower().split("x"))
+            assert len(image_size) == 2 and min(image_size) >= 1
+        except (ValueError, AssertionError):
+            ap.error(f"--image-size {args.image_size!r}: expected HxW, e.g. 480x640")
 
     model = MODELS[args.model]()
     host_fn = HOST_PREPROCESS[args.preprocess]
@@ -152,6 +199,17 @@ def main():
     arms = {"a_f32_items": Arm(model, None, host_fn), "b_u8_host_preprocess": Arm(model, None, host_fn),
             "c_u8_gpu_preprocess": Arm(model, args.preprocess, host_fn)}
     feeds = {"a_f32_items": (pre, False), "b_u8_host_preprocess": (imgs, True), "c_u8_gpu_preprocess": (imgs, False)}
+    if image_size is not None:
+        frames = [applications.synthetic_image(1, image_size + (3,), seed=i) for i in range(args.items)]
+        resize_fn = pillow_resize((224, 224), args.interpolation)
+        t0 = time.perf_counter()
+        for i in range(n_host):
+            resize_fn(frames[i % len(frames)])
+        resize_us = (time.perf_counter() - t0) / n_host * 1e6
+        arms["d_u8_host_resize"] = Arm(model, args.preprocess, resize_fn)
+        arms["e_u8_gpu_resize"] = Arm(model, args.preprocess, None, image_size=image_size, interpolation=args.interpolation)
+        feeds["d_u8_host_resize"] = (frames, True)
+        feeds["e_u8_gpu_resize"] = (frames, False)
     rates = {k: [] for k in arms}
     try:
         for rnd in range(args.reps + 1):
@@ -173,6 +231,10 @@ def main():
         "host_preprocess_input_us": round(host_us, 1),
         "stem_time_op": stem_times(model, args.preprocess, args.op_iters),
     }
+    if image_size is not None:
+        res.update({"image_size": list(image_size), "interpolation": args.interpolation,
+                    "host_pillow_resize_us": round(resize_us, 1),
+                    "resize_time_op": resize_times(model, args.preprocess, image_size, args.interpolation, args.op_iters)})
     res.update(card())
     print(json.dumps(res), flush=True)
 
