@@ -22,6 +22,7 @@ FLAG_RELU, FLAG_RESIDUAL = 1, 2
 BUF_ACT, BUF_F32, BUF_U8 = 0, 1, 2
 PRE_CAFFE, PRE_TF = 0, 1
 PRE_MODES = {"caffe": PRE_CAFFE, "tf": PRE_TF}
+RESIZE_SAMPLE_W, RESIZE_SAMPLE_H = 1, 2
 OK, ERR_INVALID, ERR_CUDA, ERR_TIMEOUT, ERR_STATE = 0, -1, -2, -3, -4
 
 FMT_NAMES = {FMT_F32: "f32", FMT_BF16X2: "bf16x2", FMT_BF16: "bf16"}
@@ -72,6 +73,7 @@ PROTOTYPES = {
     "defer_stage_submit": (_i, [_vp, _u64, _vp, _u64]),
     "defer_stage_submit_part": (_i, [_vp, _u64, _i, _i, _vp, _u64]),
     "defer_stage_submit_parts": (_i, [_vp, _u64, _i, _i, _i, C.POINTER(_vp), _u64]),
+    "defer_stage_submit_frames": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_step": (_i, [_vp, _u64]),
     "defer_stage_result": (_i, [_vp, _u64, _vp, _u64]),
     "defer_stage_predict": (_i, [_vp, _vp, _u64, _vp, _u64]),
@@ -102,6 +104,7 @@ PROTOTYPES = {
     "defer_k_preprocess": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "defer_k_preprocess_tf": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "defer_k_resize": (_i, [_vp, _vp, _vp, _vp] + [_i] * 7 + [_vp]),
+    "defer_k_resize_frames": (_i, [_i, _vp, _vp, _vp] + [_i] * 8 + [_vp]),
 }
 
 _LIB = None

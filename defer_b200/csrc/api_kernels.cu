@@ -132,4 +132,16 @@ int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const in
   return launch_resize(x, y, bounds, taps, ksize, n, h_in, w_in, h_out, w_out, (cudaStream_t)stream);
 }
 
+int defer_k_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,
+                          int W_out, int kw_w, int kw_h, int c, void* stream) {
+  DEFER_CHECK(x && y && tables, "k_resize_frames: null pointer");
+  DEFER_CHECK(pass == DEFER_RESIZE_SAMPLE_W || pass == DEFER_RESIZE_SAMPLE_H, "k_resize_frames: pass %d is not %d (width) or %d "
+              "(height)", pass, DEFER_RESIZE_SAMPLE_W, DEFER_RESIZE_SAMPLE_H);
+  DEFER_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && H_out >= 1 && W_out >= 1 && kw_w >= 1 && kw_h >= 1,
+              "k_resize_frames: bad sizes (n %d, %dx%d -> %dx%d, kw %d/%d)", n, H, W, H_out, W_out, kw_w, kw_h);
+  DEFER_CHECK(c == 3, "k_resize_frames: the resize takes RGB images (3 channels), got %d", c);
+  DEFER_CHECK(((uintptr_t)tables & 3) == 0, "k_resize_frames: tables must be 4-byte aligned");
+  return launch_resize_frames(pass, x, y, tables, n, H, W, H_out, W_out, kw_w, kw_h, (cudaStream_t)stream);
+}
+
 }  // extern "C"

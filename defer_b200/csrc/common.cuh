@@ -195,6 +195,10 @@ int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t 
 // changes is the one resized (w_in != w_out: horizontal, else vertical).  bounds [out, 2] (first, count), taps [out, ksize].
 int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
                   int w_in, int h_out, int w_out, cudaStream_t st);
+// Keras load_img resize of mixed sizes, one pass (DEFER_OP_RESIZE, pass = DEFER_RESIZE_SAMPLE_W | _H): each of the n
+// samples reads its size and tables from its int32 block in `tables` (layout: include/defer_b200.h).
+int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,
+                         int W_out, int kw_w, int kw_h, cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

@@ -1218,6 +1218,24 @@ int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t 
 // consecutive bytes of a row.  Tables go through the read-only path; rows are independent of the batch index.
 __device__ __forceinline__ uint8_t resize_clip8(int acc) { return (uint8_t)min(max(acc >> 22, 0), 255); }
 
+// The integer arithmetic of every resize kernel, in one place so the fixed-size and the per-sample paths cannot drift:
+// dst[c] = clamp((2^21 + sum_{k < count} src[k * step + c] * taps[k]) >> 22, 0, 255) for c < C.
+template <int C>
+__device__ __forceinline__ void resize_accumulate(const uint8_t* __restrict__ src, size_t step,
+                                                  const int32_t* __restrict__ taps, int count, uint8_t* __restrict__ dst) {
+  int a[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) a[c] = 1 << 21;
+  for (int k = 0; k < count; ++k) {
+    const int t = __ldg(taps + k);
+    const uint8_t* p = src + k * step;
+#pragma unroll
+    for (int c = 0; c < C; ++c) a[c] += (int)__ldg(p + c) * t;
+  }
+#pragma unroll
+  for (int c = 0; c < C; ++c) dst[c] = resize_clip8(a[c]);
+}
+
 template <bool HORIZ>
 __global__ void __launch_bounds__(256) resize_u8_kernel(const uint8_t* __restrict__ x, uint8_t* __restrict__ y,
                                                         const int32_t* __restrict__ bounds, const int32_t* __restrict__ taps,
@@ -1228,30 +1246,14 @@ __global__ void __launch_bounds__(256) resize_u8_kernel(const uint8_t* __restric
     const int xo = (int)(i % w_out);
     const size_t row = i / w_out;
     const int first = __ldg(bounds + 2 * xo), count = __ldg(bounds + 2 * xo + 1);
-    const int32_t* t = taps + (size_t)xo * ksize;
-    const uint8_t* src = x + (row * w_in + first) * 3;
-    int a0 = 1 << 21, a1 = 1 << 21, a2 = 1 << 21;
-    for (int k = 0; k < count; ++k) {
-      const int c = __ldg(t + k);
-      a0 += (int)__ldg(src + 3 * k) * c;
-      a1 += (int)__ldg(src + 3 * k + 1) * c;
-      a2 += (int)__ldg(src + 3 * k + 2) * c;
-    }
-    uint8_t* dst = y + i * 3;
-    dst[0] = resize_clip8(a0);
-    dst[1] = resize_clip8(a1);
-    dst[2] = resize_clip8(a2);
+    resize_accumulate<3>(x + (row * w_in + first) * 3, 3, taps + (size_t)xo * ksize, count, y + i * 3);
   } else {                                       // i = output byte; columns (x, c) of input and output correspond 1:1
     const size_t row_bytes = (size_t)w_out * 3;
     const size_t col = i % row_bytes, r = i / row_bytes;
     const int yo = (int)(r % h_out);
     const size_t img = r / h_out;
     const int first = __ldg(bounds + 2 * yo), count = __ldg(bounds + 2 * yo + 1);
-    const int32_t* t = taps + (size_t)yo * ksize;
-    const uint8_t* src = x + (img * h_in + first) * row_bytes + col;
-    int a = 1 << 21;
-    for (int k = 0; k < count; ++k) a += (int)__ldg(src + k * row_bytes) * __ldg(t + k);
-    y[i] = resize_clip8(a);
+    resize_accumulate<1>(x + (img * h_in + first) * row_bytes + col, row_bytes, taps + (size_t)yo * ksize, count, y + i);
   }
 }
 int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
@@ -1266,6 +1268,60 @@ int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int
   } else {
     prefer_max_smem(resize_u8_kernel<false>);
     resize_u8_kernel<false><<<grid, 256, 0, st>>>(x, y, bounds, taps, ksize, h_in, w_in, h_out, w_out, n_out);
+  }
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
+// Keras load_img resize of images of mixed sizes (DEFER_OP_RESIZE, modes DEFER_RESIZE_SAMPLE_W / _H).  Sample s of the
+// microbatch reads its geometry and tables from its own int32 block (layout in include/defer_b200.h), so one launch - and
+// one lane graph - serves any mix of sizes up to the slot's (H, W).  blockIdx.y = sample.
+// SAMPLE_W: x = the input slots (n, H, W, 3), image s packed at the start of its slot as (h_in, w_in, 3);
+//           y = (n, H, W_out, 3), rows [0, h_in) written, one thread per output pixel.
+// SAMPLE_H: x = that (n, H, W_out, 3) buffer, rows [0, h_in) read; y = (n, H_out, W_out, 3), one thread per output byte.
+// Memory safety does not depend on the block: h_in / w_in are clamped into [1, H] / [1, W], first into [0, in_len) and
+// count into [0, min(kcap, in_len - first)], so a stale, zero or corrupt block gives wrong bytes, never a read outside
+// the sample's slot.  A zero block (a never-written sample of a partial group) gives zero bytes.
+template <bool HORIZ>
+__global__ void __launch_bounds__(256) resize_frames_u8_kernel(const uint8_t* __restrict__ x, uint8_t* __restrict__ y,
+                                                               const int32_t* __restrict__ tables, int block_ints, int H,
+                                                               int W, int H_out, int W_out, int kw_w, int kw_h) {
+  const int s = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int32_t* blk = tables + (size_t)s * block_ints;
+  const int h_in = min(max(__ldg(blk), 1), H);
+  if constexpr (HORIZ) {
+    if (i >= h_in * W_out) return;               // rows past this sample's height
+    const int w_in = min(max(__ldg(blk + 1), 1), W);
+    const int xo = i % W_out, row = i / W_out;
+    const int32_t* bounds = blk + 2;
+    const int first = min(max(__ldg(bounds + 2 * xo), 0), w_in - 1);
+    const int count = min(max(__ldg(bounds + 2 * xo + 1), 0), min(kw_w, w_in - first));
+    resize_accumulate<3>(x + (size_t)s * H * W * 3 + ((size_t)row * w_in + first) * 3, 3,
+                         bounds + 2 * W_out + (size_t)xo * kw_w, count, y + ((size_t)s * H * W_out + i) * 3);
+  } else {
+    const int row_bytes = W_out * 3;
+    if (i >= H_out * row_bytes) return;
+    const int col = i % row_bytes, yo = i / row_bytes;
+    const int32_t* bounds = blk + 2 + W_out * (2 + kw_w);
+    const int first = min(max(__ldg(bounds + 2 * yo), 0), h_in - 1);
+    const int count = min(max(__ldg(bounds + 2 * yo + 1), 0), min(kw_h, h_in - first));
+    resize_accumulate<1>(x + ((size_t)s * H + first) * row_bytes + col, (size_t)row_bytes,
+                         bounds + 2 * H_out + (size_t)yo * kw_h, count, y + (size_t)s * H_out * row_bytes + i);
+  }
+}
+int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,
+                         int W_out, int kw_w, int kw_h, cudaStream_t st) {
+  const int block_ints = 2 + W_out * (2 + kw_w) + H_out * (2 + kw_h);
+  const bool horiz = pass == DEFER_RESIZE_SAMPLE_W;
+  const size_t per_sample = horiz ? (size_t)H * W_out : (size_t)H_out * W_out * 3;
+  const dim3 grid((unsigned)((per_sample + 255) / 256), (unsigned)n);
+  if (horiz) {
+    prefer_max_smem(resize_frames_u8_kernel<true>);
+    resize_frames_u8_kernel<true><<<grid, 256, 0, st>>>(x, y, tables, block_ints, H, W, H_out, W_out, kw_w, kw_h);
+  } else {
+    prefer_max_smem(resize_frames_u8_kernel<false>);
+    resize_frames_u8_kernel<false><<<grid, 256, 0, st>>>(x, y, tables, block_ints, H, W, H_out, W_out, kw_w, kw_h);
   }
   DEFER_CUDA(cudaGetLastError());
   return DEFER_OK;

@@ -117,6 +117,7 @@ struct Lane {
   std::vector<void*> im2col;           // per op (backend 4): patch matrix scratch
   bool timed = false;
   void* peer_out = nullptr;   // HOP_COPY: this lane's input slot on the consumer GPU (destination of the hop copy)
+  int32_t* tables = nullptr;  // DEFER_RESIZE_SAMPLE_*: `batch` table blocks, next to the lane's input slot in the arena
   // the microbatch the lane ran last (last stage: the one out_host is filled with); result() refuses any other
   bool stepped = false;
   uint64_t last_seq = 0;
@@ -172,6 +173,13 @@ struct defer_stage_s {
   };
   std::vector<MegaGroup> groups;
   std::vector<int> op_group;      // group index per op, -1 = launched on its own
+  // images of mixed sizes: the DEFER_RESIZE_SAMPLE_W / _H pair (op indices, -1 = none), its geometry and table blocks
+  struct Frames {
+    int op_w = -1, op_h = -1;
+    int H = 0, W = 0, H_out = 0, W_out = 0, kw_w = 0, kw_h = 0;
+    size_t block_ints = 0;        // int32 values per sample block
+    size_t tables_off = 0;        // offset of a lane's blocks from its input slot
+  } frames;
 
   uint32_t* ctrl_u32(size_t off) { return reinterpret_cast<uint32_t*>(arena + off); }
   uint32_t* ready_flag(int d) { return ctrl_u32(OFF_READY + d * FLAG_STRIDE); }
@@ -267,6 +275,11 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       if (d.mode == DEFER_PRE_TF) return launch_preprocess_tf((const uint8_t*)x, (float*)y, (size_t)nb * bi.h * bi.w, st);
       return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
     case DEFER_OP_RESIZE:
+      if (d.mode != 0) {
+        const auto& f = s->frames;
+        return launch_resize_frames(d.mode, (const uint8_t*)x, (uint8_t*)y, L.tables, nb, f.H, f.W, f.H_out, f.W_out, f.kw_w,
+                                    f.kw_h, st);
+      }
       return launch_resize((const uint8_t*)x, (uint8_t*)y, (const int32_t*)s->d_weights[d.w_scale],
                            (const int32_t*)s->d_weights[d.w_kernel], d.kw, nb, bi.h, bi.w, bo.h, bo.w, st);
   }
@@ -347,6 +360,12 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
       op.alg_flops = nb * bi.h * bi.w * bi.c;
       break;
     case DEFER_OP_RESIZE:   // + the two int32 tables
+      if (d.mode != 0) {    // an upper bound: every sample at the slot's size, plus its header and its axis' tables
+        const int out_len = d.mode == DEFER_RESIZE_SAMPLE_W ? bo.w : bo.h;
+        op.alg_bytes = in_b + out_b + nb * (2.0 + out_len * (2.0 + d.kw)) * 4.0;
+        op.alg_flops = 2.0 * nb * bo.h * bo.w * bo.c * d.kw;
+        break;
+      }
       op.alg_bytes = in_b + out_b + (double)s->weight_bytes[d.w_scale] + (double)s->weight_bytes[d.w_kernel];
       op.alg_flops = 2.0 * nb * bo.h * bo.w * bo.c * d.kw;
       break;
@@ -507,8 +526,8 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       set_error("op %d: only a RESIZE or PREPROCESS op may read a U8 buffer (as in0)", i);
       return fail(DEFER_ERR_INVALID);
     }
-    if (d.kind != DEFER_OP_PREPROCESS && d.mode != 0) {
-      set_error("op %d: mode %d is meaningful only on a PREPROCESS op and must be 0 here", i, d.mode);
+    if (d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE && d.mode != 0) {
+      set_error("op %d: mode %d is meaningful only on a PREPROCESS or RESIZE op and must be 0 here", i, d.mode);
       return fail(DEFER_ERR_INVALID);
     }
     switch (d.kind) {
@@ -633,6 +652,40 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
                     bo.elem, bo.c);
           return fail(DEFER_ERR_INVALID);
         }
+        if (d.mode == DEFER_RESIZE_SAMPLE_W || d.mode == DEFER_RESIZE_SAMPLE_H) {   // images of mixed sizes
+          const bool horiz = d.mode == DEFER_RESIZE_SAMPLE_W;
+          op.kname = "resize_frames_u8_kernel";
+          auto& f = s->frames;
+          if (d.in1 >= 0 || d.flags || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0) {
+            set_error("op %d (resize, per sample): takes no weights, in1 or flags (its tables come with each microbatch)", i);
+            return fail(DEFER_ERR_INVALID);
+          }
+          if (horiz ? (d.in0 != cfg->input_buf || bo.h != bi.h || f.op_w >= 0) : (bo.w != bi.w || f.op_h >= 0)) {
+            set_error("op %d (resize, per sample): SAMPLE_W maps the stage input (H, W) to (H, W_out), SAMPLE_H maps (H, W_out) "
+                      "to (H_out, W_out), one of each per stage (got %dx%d -> %dx%d, mode %d)", i, bi.h, bi.w, bo.h, bo.w, d.mode);
+            return fail(DEFER_ERR_INVALID);
+          }
+          // kw holds the axis' taps for every source length up to the bound: at most the widest filter's (lanczos, support 3)
+          const int in_len = horiz ? bi.w : bi.h, out_len = horiz ? bo.w : bo.h;
+          const int kmax = 2 * (int)ceil(3.0 * fmax((double)in_len / out_len, 1.0)) + 1;
+          if (d.kw < 1 || d.kw > kmax) {
+            set_error("op %d (resize, per sample): kw = %d taps, needs 1 <= kw <= %d for %d -> %d", i, d.kw, kmax, in_len, out_len);
+            return fail(DEFER_ERR_INVALID);
+          }
+          if (horiz) {
+            f.op_w = i;
+            f.H = bi.h; f.W = bi.w; f.W_out = bo.w; f.kw_w = d.kw;
+          } else {
+            f.op_h = i;
+            f.H_out = bo.h; f.kw_h = d.kw;
+          }
+          break;
+        }
+        if (d.mode != 0) {
+          set_error("op %d (resize): unknown mode %d (0, SAMPLE_W %d, SAMPLE_H %d)", i, d.mode, DEFER_RESIZE_SAMPLE_W,
+                    DEFER_RESIZE_SAMPLE_H);
+          return fail(DEFER_ERR_INVALID);
+        }
         if ((bi.h != bo.h) == (bi.w != bo.w) || d.in1 >= 0 || d.flags || d.w_shift >= 0) {
           set_error("op %d (resize): exactly one axis must change (%dx%d -> %dx%d), no in1 / flags / w_shift", i, bi.h, bi.w,
                     bo.h, bo.w);
@@ -668,6 +721,15 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     return fail(DEFER_ERR_INVALID);
   }
   s->output_writer = writer[cfg->output_buf];
+  if (s->frames.op_w >= 0 || s->frames.op_h >= 0) {
+    auto& f = s->frames;
+    if (f.op_w < 0 || f.op_h < 0 || ops[f.op_h].in0 != ops[f.op_w].out) {
+      set_error("the per-sample resize ops come as a pair: SAMPLE_W on the stage input, SAMPLE_H on its output (ops %d, %d)",
+                f.op_w, f.op_h);
+      return fail(DEFER_ERR_INVALID);
+    }
+    f.block_ints = 2 + (size_t)f.W_out * (2 + f.kw_w) + (size_t)f.H_out * (2 + f.kw_h);
+  }
   for (int i = 0; i < n_ops; ++i)
     if (ops[i].in0 == cfg->input_buf || ops[i].in1 == cfg->input_buf) s->last_input_reader = i;
   if (s->last_input_reader < 0) {
@@ -708,6 +770,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
   // ---- arena: ctrl + input slots (exported to the upstream stage)
   size_t in_bytes = s->bufs[cfg->input_buf].bytes;
   s->slot_stride = (in_bytes + 1023) / 1024 * 1024;
+  if (s->frames.op_w >= 0) {   // the lane's table blocks follow its input slot (zeroed with the arena below)
+    s->frames.tables_off = s->slot_stride;
+    s->slot_stride += ((size_t)cfg->batch * s->frames.block_ints * 4 + 1023) / 1024 * 1024;
+  }
   s->arena_bytes = CTRL_BYTES + s->slot_stride * cfg->depth;
   if (cudaMalloc((void**)&s->arena, s->arena_bytes) != cudaSuccess) {
     set_error("cudaMalloc arena (%zu bytes) failed", s->arena_bytes);
@@ -731,6 +797,7 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     L.buf.assign(n_bufs, nullptr);
     L.buf[cfg->input_buf] = s->arena + CTRL_BYTES + s->slot_stride * l;
+    if (s->frames.op_w >= 0) L.tables = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->frames.tables_off);
     for (int b = 0; b < n_bufs; ++b) {
       if (b == cfg->input_buf) continue;
       if (b == cfg->output_buf && !cfg->is_last && s->hop != HOP_COPY) continue;  // bound to the consumer's slot at link time
@@ -1175,6 +1242,7 @@ int defer_stage_finalize(defer_stage_t s) {
 int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit: null");
   DEFER_CHECK(s->cfg.is_first, "submit: only the first stage takes host input");
+  DEFER_CHECK(s->frames.op_w < 0, "submit: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   DEFER_CHECK(nbytes == b.bytes, "submit: got %llu bytes, stage input is %zu", (unsigned long long)nbytes, b.bytes);
   DEFER_TRY(set_device(s));
@@ -1186,6 +1254,7 @@ int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint6
 int defer_stage_submit_part(defer_stage_t s, uint64_t seq, int index, int count, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit_part: null");
   DEFER_CHECK(s->cfg.is_first, "submit_part: only the first stage takes host input");
+  DEFER_CHECK(s->frames.op_w < 0, "submit_part: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;       // first-stage input is plain fp32 NHWC: samples are contiguous
   DEFER_CHECK(index >= 0 && count >= 1 && index + count <= s->cfg.batch, "submit_part: samples [%d, %d) outside the microbatch of %d",
@@ -1203,6 +1272,7 @@ int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_index, int
                              const void* const* host_ptrs, uint64_t nbytes_per_item) {
   DEFER_CHECK(s && host_ptrs && n_items >= 1 && samples_per_item >= 1, "submit_parts: bad arguments");
   DEFER_CHECK(s->cfg.is_first, "submit_parts: only the first stage takes host input");
+  DEFER_CHECK(s->frames.op_w < 0, "submit_parts: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;
   DEFER_CHECK(first_index >= 0 && first_index + n_items * samples_per_item <= s->cfg.batch,
@@ -1217,6 +1287,36 @@ int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_index, int
     DEFER_CHECK(host_ptrs[i], "submit_parts: item %d is null", i);
     DEFER_CUDA(cudaMemcpyAsync(dst + (size_t)i * nbytes_per_item, host_ptrs[i], nbytes_per_item, cudaMemcpyHostToDevice, L.stream));
   }
+  return DEFER_OK;
+}
+
+int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* images,
+                              const int32_t* hw, const int32_t* tables, uint64_t table_bytes) {
+  DEFER_CHECK(s && images && hw && tables && n >= 1, "submit_frames: bad arguments");
+  DEFER_CHECK(s->cfg.is_first, "submit_frames: only the first stage takes host input");
+  const auto& f = s->frames;
+  DEFER_CHECK(f.op_w >= 0, "submit_frames: the stage takes one image size (no DEFER_RESIZE_SAMPLE_* ops); use defer_stage_submit*");
+  DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_frames: samples [%d, %d) outside the microbatch of %d",
+              first_index, first_index + n, s->cfg.batch);
+  DEFER_CHECK(table_bytes == (uint64_t)n * f.block_ints * 4, "submit_frames: got %llu table bytes, %d blocks are %zu",
+              (unsigned long long)table_bytes, n, (size_t)n * f.block_ints * 4);
+  for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
+    const int h = hw[2 * i], w = hw[2 * i + 1];
+    const int32_t* blk = tables + (size_t)i * f.block_ints;
+    DEFER_CHECK(images[i], "submit_frames: image %d is null", i);
+    DEFER_CHECK(h >= 1 && h <= f.H && w >= 1 && w <= f.W, "submit_frames: image %d is %dx%d, the slot takes 1..%d x 1..%d", i, h,
+                w, f.H, f.W);
+    DEFER_CHECK(blk[0] == h && blk[1] == w, "submit_frames: table block %d is for %dx%d, image %d is %dx%d", i, blk[0], blk[1], i,
+                h, w);
+  }
+  DEFER_TRY(set_device(s));
+  Lane& L = s->lanes[seq % s->cfg.depth];
+  const size_t sample = (size_t)f.H * f.W * 3;
+  uint8_t* slot = (uint8_t*)L.buf[s->cfg.input_buf];
+  for (int i = 0; i < n; ++i)   // the image's own bytes only, packed at the start of its sample slot
+    DEFER_CUDA(cudaMemcpyAsync(slot + (size_t)(first_index + i) * sample, images[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3,
+                               cudaMemcpyHostToDevice, L.stream));
+  DEFER_CUDA(cudaMemcpyAsync(L.tables + (size_t)first_index * f.block_ints, tables, table_bytes, cudaMemcpyHostToDevice, L.stream));
   return DEFER_OK;
 }
 

@@ -14,7 +14,7 @@ What changed underneath:
 
 Non-reference additions: ``close()`` / context manager (the reference can only be killed), keyword-only
 ``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1),
-``coalesce``, ``preprocess``, ``image_size`` and ``interpolation``.
+``coalesce``, ``preprocess``, ``image_size``, ``max_image_size`` and ``interpolation``.
 
 Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the host before every ``input_q.put``
 (``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
@@ -28,8 +28,10 @@ Resizing: the same driver loads every image with ``load_img(path, target_size=(2
 With ``image_size=(h, w)`` (and ``preprocess``) queue items are uint8 images of that size, e.g. camera frames, and the
 first stage resizes them to the model input on its GPU before preprocessing, bit for bit what
 ``applications.resize_image(item, (H, W), interpolation)`` gives; ``interpolation`` takes the names ``load_img`` accepts
-(default ``"nearest"``, as in Keras).  One pipeline takes one image size.  An ``image_size`` equal to the model input
-changes nothing, as Keras does not resize then.
+(default ``"nearest"``, as in Keras).  An ``image_size`` equal to the model input changes nothing, as Keras does not
+resize then.  Photos and frames from several cameras come in many sizes: with ``max_image_size=(H, W)`` instead, each
+queue item is a uint8 image ``(batch, h, w, 3)`` of its own size with ``h <= H`` and ``w <= W``, items of different sizes
+share a microbatch, and each gives exactly what ``image_size=(h, w)`` would.  Only the image's own bytes cross PCIe.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -49,7 +51,7 @@ import numpy as np
 
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
-from .resize import check_interpolation, check_size
+from .resize import check_frame, check_interpolation, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
 
@@ -58,7 +60,8 @@ class DEFER:
     def __init__(self, computeNodes, *, dtype: str = "float32", depth: int = 4, batch: Optional[int] = None,
                  coalesce: int = 1, linger_us: float = 200.0, conv_backend: int = 0, dist=None,
                  wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None,
-                 image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest") -> None:
+                 image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
+                 max_image_size: Optional[Tuple[int, int]] = None) -> None:
         if preprocess is not None:
             check_preprocess(preprocess)
         check_interpolation(interpolation)
@@ -67,10 +70,19 @@ class DEFER:
             if preprocess is None:
                 raise ValueError(f"image_size={image_size}: resizing takes uint8 images and needs preprocess= (float items "
                                  "are already preprocessed, and Keras resizes before preprocessing)")
+        if max_image_size is not None:
+            max_image_size = check_size(max_image_size, "max_image_size")
+            if preprocess is None:
+                raise ValueError(f"max_image_size={max_image_size}: resizing takes uint8 images and needs preprocess= "
+                                 "(float items are already preprocessed, and Keras resizes before preprocessing)")
+            if image_size is not None:
+                raise ValueError(f"max_image_size={max_image_size} and image_size={image_size}: give one (image_size: "
+                                 "every image has that size; max_image_size: each image has its own size up to that bound)")
         self.computeNodes = list(computeNodes)
         self.preprocess = preprocess        # None | "caffe" | "tf": uint8 queue items, preprocessed on stage 0's GPU
         self.image_size = image_size        # None | (h, w) of the uint8 queue items, resized on stage 0's GPU
         self.interpolation = interpolation
+        self.max_image_size = max_image_size  # None | (H, W): uint8 queue items of any size up to it, resized on stage 0
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -132,7 +144,8 @@ class DEFER:
                                          "wait_timeout_ms": self.wait_timeout_ms,
                                          "preprocess": self.preprocess if i == 0 else None,
                                          "image_size": self.image_size if i == 0 else None,
-                                         "interpolation": self.interpolation})
+                                         "interpolation": self.interpolation,
+                                         "max_image_size": self.max_image_size if i == 0 else None})
             self.dist.wait_all_ready()      # the 1-byte ACK of dispatcher.py:64-65
             return
         runners = []
@@ -145,7 +158,8 @@ class DEFER:
                                       wait_timeout_ms=self.wait_timeout_ms,
                                       preprocess=self.preprocess if i == 0 else None,
                                       image_size=self.image_size if i == 0 else None,
-                                      interpolation=self.interpolation)
+                                      interpolation=self.interpolation,
+                                      max_image_size=self.max_image_size if i == 0 else None)
             r.name = f"part{i+1}"
             runners.append(r)
         for i in range(n - 1):              # next hop = nodeIPs[i+1] (dispatcher.py:51-55)
@@ -159,6 +173,7 @@ class DEFER:
         first = self.stages[0] if self.stages else self.dist.local_runner()
         G, B = self.coalesce, self.batch or 1
         u8 = self.preprocess is not None
+        bound = self.max_image_size
         hold, nh = self._hold, len(self._hold)
         get_nowait = input.get_nowait
         submit_items = first.submit_items if hasattr(first, "submit_items") else None
@@ -166,6 +181,9 @@ class DEFER:
             def submit_items(seq, group):
                 for i, x in enumerate(group):
                     first.submit_part(seq, i * B, x)
+        if bound is not None:                # each image with its own size and tables, one C call per group
+            def submit_items(seq, group):
+                first.submit_frames(seq, 0, group)
         try:
             while not self._stop.is_set():
                 try:
@@ -182,7 +200,9 @@ class DEFER:
                 in_shape = None
                 while True:
                     x = model_input
-                    if u8:
+                    if bound is not None:            # any size up to the bound: no same-shape rule within a group
+                        x = check_frame(x, bound)
+                    elif u8:
                         if not (isinstance(x, np.ndarray) and x.dtype == np.uint8):
                             raise TypeError(f"DEFER(preprocess={self.preprocess!r}) takes uint8 RGB images "
                                             "(img_to_array(img).astype(np.uint8)), got "
@@ -192,9 +212,9 @@ class DEFER:
                         x = np.ascontiguousarray(x, dtype=np.float32)
                     if x.shape[0] != B:
                         raise ValueError(f"queue item has batch {x.shape[0]}, DEFER was built for batch {B}")
-                    if in_shape is None:
+                    if bound is None and in_shape is None:
                         in_shape = x.shape
-                    elif x.shape != in_shape:
+                    elif bound is None and x.shape != in_shape:
                         raise ValueError(f"queue items of one group differ in shape: {x.shape} vs {in_shape}")
                     hold[self.items_submitted % nh] = x      # keep alive until the DMA has certainly happened
                     self.items_submitted += 1

@@ -24,6 +24,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .node_state import NodeState
 from .planner import Plan, plan_stage
+from .resize import check_frame, pack_frame_tables
 
 DTYPE_TO_FMT = {
     "float32": A.FMT_BF16X2,        # fp32 parity path on the tensor cores (bf16x3 split, fp32 accumulate)
@@ -81,6 +82,9 @@ class StageRunner:
         self.preprocess = {v: k for k, v in A.PRE_MODES.items()}.get(pre_modes[0]) if pre_modes else None
         # planned with image_size=: the stage resizes its images to the model input first (for messages)
         self.resizes = any(o.kind == A.OP_RESIZE for o in plan.ops)
+        # planned with max_image_size=: images of mixed sizes, fed by submit_frames with their table blocks
+        self.frames = plan.frames
+        self._tables: Dict[int, tuple] = {}          # per lane: blocks, sizes and images of its latest microbatch (kept alive)
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
         self.out_elems = int(np.prod(self.out_shape))
@@ -109,13 +113,16 @@ class StageRunner:
     @classmethod
     def from_model(cls, model: K.Model, device=0, dtype: str = "float32", max_batch: int = 1, depth: int = 1,
                    is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
-                   image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest", **kw) -> "StageRunner":
+                   image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
+                   max_image_size: Optional[Tuple[int, int]] = None, **kw) -> "StageRunner":
         """``preprocess="caffe"`` or ``"tf"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the
         stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family).
         ``image_size=(h, w)`` (with ``preprocess``): inputs are uint8 RGB images of that size, resized on the GPU to the
-        model's input as Keras' ``load_img(target_size=..., interpolation=...)`` does (``resize.resize_image``)."""
+        model's input as Keras' ``load_img(target_size=..., interpolation=...)`` does (``resize.resize_image``).
+        ``max_image_size=(H, W)`` (with ``preprocess``, instead of ``image_size``): the same for images of any size up to
+        ``(H, W)``, each resized from its own size; feed them with ``submit_frames`` / ``predict_frames``."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
-                          interpolation=interpolation)
+                          interpolation=interpolation, max_image_size=max_image_size)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
                 is_last=is_last, name=model.name, **kw)
@@ -155,6 +162,9 @@ class StageRunner:
         """``x`` as the C-contiguous array the stage copies from.  A stage without preprocessing converts to float32.
         A preprocessing stage takes uint8 only: a float array may be ``img_to_array`` output or already preprocessed,
         and neither can be told apart from the other."""
+        if self.frames is not None:
+            raise ValueError(f"{self.name}: this stage takes images of mixed sizes up to max_image_size="
+                             f"{self.frames['max_image_size']}; feed them with submit_frames / predict_frames")
         if self.in_dtype == np.uint8:
             if getattr(x, "dtype", None) != np.uint8:
                 raise TypeError(f"{self.name}: this stage preprocesses uint8 RGB images on the GPU "
@@ -205,6 +215,36 @@ class StageRunner:
             ptrs[i] = x.__array_interface__["data"][0]
         x0 = items[0]
         A.check(self.lib.defer_stage_submit_parts(self.handle, seq, 0, n, x0.shape[0], ptrs, x0.nbytes))
+
+    def submit_frames(self, seq: int, index: int, frames) -> None:
+        """Ingress of a ``max_image_size=(H, W)`` stage: ``frames`` is a list of uint8 RGB items ``(k, h, w, 3)`` (or
+        ``(h, w, 3)``), each of its own size with ``1 <= h <= H`` and ``1 <= w <= W``; their samples go to samples
+        ``[index, index + total k)`` of microbatch ``seq``, each with its table block.  One C call copies each image's own
+        bytes and then the blocks.  Same lifetime rule as ``submit``."""
+        if self.frames is None:
+            raise ValueError(f"{self.name}: submit_frames needs a stage planned with max_image_size=")
+        bound = self.frames["max_image_size"]
+        images = []
+        for x in frames:
+            x = check_frame(x, bound)
+            images.extend(x[j] for j in range(x.shape[0]))
+        n = len(images)
+        if not 0 <= index <= self.batch - n:
+            raise ValueError(f"{self.name}: {n} images from sample {index} do not fit the microbatch of {self.batch}")
+        hw = np.array([im.shape[:2] for im in images], np.int32).reshape(n, 2)
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"])
+        self._tables[seq % self.depth] = (tables, hw, images)
+        ptrs = (C.c_void_p * n)(*[im.__array_interface__["data"][0] for im in images])
+        A.check(self.lib.defer_stage_submit_frames(self.handle, seq, index, n, ptrs, hw.ctypes.data, tables.ctypes.data,
+                                                   tables.nbytes))
+
+    def predict_frames(self, frames) -> np.ndarray:
+        """Single-stage ``model.predict`` of a ``max_image_size`` stage: the outputs of the samples of ``frames`` (see
+        ``submit_frames``), in order."""
+        self.submit_frames(0, 0, frames)
+        self.step(0)
+        n = sum(1 if np.ndim(x) == 3 else len(x) for x in frames)
+        return self.result(0)[:n]
 
     def step(self, seq: int) -> None:
         A.check(self.lib.defer_stage_step(self.handle, seq))
@@ -388,7 +428,8 @@ class Node:
                                        wait_timeout_ms=msg.get("wait_timeout_ms", 0),
                                        preprocess=msg.get("preprocess") if rank == 0 else None,
                                        image_size=msg.get("image_size") if rank == 0 else None,
-                                       interpolation=msg.get("interpolation", "nearest"))
+                                       interpolation=msg.get("interpolation", "nearest"),
+                                       max_image_size=msg.get("max_image_size") if rank == 0 else None)
         ns.model = runner                               # src/node.py:38
         self.runner = runner
         # wire the hop: my consumer gives me its input-side token, I give it my output-side token

@@ -20,6 +20,9 @@ With ``preprocess="caffe"`` or ``"tf"`` (first stage only) the stage input is a 
 the library folds it into the fused RGB stem when it can.  With ``image_size=(h, w)`` as well, the stage input is a uint8
 image of that size and up to two ``RESIZE`` ops (width, then height: Keras' ``load_img(target_size=...)`` through Pillow,
 tables from ``resize.resize_tables``) bring it to the model's input size before ``PREPROCESS``.
+With ``max_image_size=(H, W)`` instead, the stage input is a uint8 slot of that size per sample and two per-sample
+``RESIZE`` ops (``RESIZE_SAMPLE_W``, then ``_H``) read each image's size and tables from a block that comes with it
+(``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.
 """
 from __future__ import annotations
 
@@ -31,7 +34,7 @@ import numpy as np
 from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
-from .resize import check_interpolation, check_size, resize_tables
+from .resize import check_interpolation, check_size, kcap, resize_tables
 
 
 def same_pad(size: int, k: int, s: int) -> Tuple[int, int]:
@@ -73,6 +76,9 @@ class Plan:
     input_shape: Tuple[int, ...]
     output_shape: Tuple[int, ...]
     tensor_buf: Dict[str, int]                        # layer name -> buffer id holding its output (if materialised)
+    # max_image_size=: {"max_image_size": (H, W), "target": (H_out, W_out), "kw": (kw_w, kw_h), "interpolation": name},
+    # what the stage's feeder needs to pack each image's table block (resize.pack_frame_tables); None otherwise
+    frames: Optional[dict] = None
 
     def describe(self) -> str:
         lines = []
@@ -92,7 +98,8 @@ def _hwc(shape) -> Tuple[int, int, int]:
 
 
 def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None,
-               image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest") -> Plan:
+               image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
+               max_image_size: Optional[Tuple[int, int]] = None) -> Plan:
     if preprocess is not None:
         check_preprocess(preprocess)
         if not is_first:
@@ -104,6 +111,14 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         if preprocess is None:
             raise ValueError(f"image_size={image_size}: resizing takes uint8 images and needs preprocess= (float items "
                              "are already preprocessed, and Keras resizes before preprocessing)")
+    if max_image_size is not None:
+        max_image_size = check_size(max_image_size, "max_image_size")
+        if preprocess is None:
+            raise ValueError(f"max_image_size={max_image_size}: resizing takes uint8 images and needs preprocess= (float "
+                             "items are already preprocessed, and Keras resizes before preprocessing)")
+        if image_size is not None:
+            raise ValueError(f"max_image_size={max_image_size} and image_size={image_size}: give one (image_size: every "
+                             "image has that size; max_image_size: each image has its own size up to that bound)")
     nodes = list(model.iter_nodes())
     # names as recorded at map time (tensor histories may be re-tagged later by Input(tensor=...))
     order = [l.name for l, _ in nodes]
@@ -191,6 +206,7 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
 
     # stage input
     input_shape = tuple(shapes[in_name][1:])
+    frames = None
     if preprocess is None:
         tensor_buf[in_name] = new_buf(shapes[in_name], A.BUF_F32 if is_first else A.BUF_ACT)
         input_buf = tensor_buf[in_name]
@@ -198,13 +214,21 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         if _hwc(shapes[in_name])[2] != 3 or len(shapes[in_name]) != 4:
             raise ValueError(f"preprocess={preprocess!r}: the input must be an RGB image (h, w, 3), got {shapes[in_name][1:]}")
         H, W, _ = _hwc(shapes[in_name])
-        h, w = image_size if image_size is not None else (H, W)
+        h, w = image_size or max_image_size or (H, W)
         input_shape = (h, w, 3)
         input_buf = img = new_buf((None,) + input_shape, A.BUF_U8)
+        if max_image_size is not None:
+            # images of mixed sizes up to (h, w): both passes always, the tables come with each image
+            kw = (kcap(w, W, interpolation), kcap(h, H, interpolation))
+            op_w = emit(PlanOp(A.OP_RESIZE, img, new_buf((None, h, W, 3), A.BUF_U8), kw=kw[0], mode=A.RESIZE_SAMPLE_W,
+                               layers=[f"load_img(width <={w}->{W}, {interpolation})"]))
+            img = emit(PlanOp(A.OP_RESIZE, op_w.out, new_buf((None, H, W, 3), A.BUF_U8), kw=kw[1], mode=A.RESIZE_SAMPLE_H,
+                              layers=[f"load_img(height <={h}->{H}, {interpolation})"])).out
+            frames = {"max_image_size": (h, w), "target": (H, W), "kw": kw, "interpolation": interpolation}
         # Pillow resizes the width first and skips an axis whose size does not change (so does Keras: no resize at all
         # when the image is already at target_size)
         for axis, n_in, n_out, shape in (("width", w, W, (h, W, 3)), ("height", h, H, (H, W, 3))):
-            if n_in == n_out:
+            if n_in == n_out or frames is not None:
                 continue
             first, count, coef = resize_tables(n_in, n_out, interpolation)
             op = emit(PlanOp(A.OP_RESIZE, img, new_buf((None,) + shape, A.BUF_U8), kw=coef.shape[1],
@@ -386,4 +410,4 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
             op.w_shift = add_weight(op.shift.astype(np.float32))
     return Plan(bufs=bufs, ops=ops, weights=weights, input_buf=input_buf, output_buf=out_buf,
                 input_shape=input_shape, output_shape=tuple(shapes[out_name][1:]),
-                tensor_buf=dict(tensor_buf))
+                tensor_buf=dict(tensor_buf), frames=frames)

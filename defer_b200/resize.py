@@ -20,6 +20,7 @@ horizontal gather followed by the vertical one.
 """
 from __future__ import annotations
 
+import functools
 import math
 from typing import Tuple
 
@@ -175,3 +176,87 @@ def resize_image(x: np.ndarray, target_size, interpolation: str = "nearest") -> 
     if x.shape[h_ax] != th:
         y = resize_axis(y, h_ax, *resize_tables(x.shape[h_ax], th, interpolation))
     return y
+
+
+# ------------------------------------------------------------------------------------------------ frames of mixed sizes
+# ``DEFER(..., max_image_size=(H, W))`` takes images of any size up to (H, W).  Each sample of a microbatch then carries
+# its own tables in a fixed-size int32 block (``DEFER_RESIZE_SAMPLE_W`` / ``_H`` in include/defer_b200.h):
+#
+#     [h_in, w_in,
+#      width axis:  (first, count) [W_out, 2],  taps [W_out, kw_w],
+#      height axis: (first, count) [H_out, 2],  taps [H_out, kw_h]]
+#
+# with taps zero past ``count``, ``kw_w = kcap(W, W_out)`` and ``kw_h = kcap(H, H_out)``.  An axis whose length already
+# equals the target gets the identity table (first = i, count 1, one tap of 2^22): an exact copy, which is what Pillow's
+# skipping that axis gives.
+
+def kcap(max_len: int, out_len: int, interpolation: str = "nearest") -> int:
+    """Taps per output that ``resize_tables(n, out_len, interpolation)`` needs for every source length ``1 <= n <=
+    max_len``.  Its ksize, ``2 * ceil(support * max(n / out_len, 1)) + 1``, does not decrease with ``n``, so this is the
+    ksize at ``max_len``, computed with the same double-precision steps."""
+    check_interpolation(interpolation)
+    if max_len < 1 or out_len < 1:
+        raise ValueError(f"kcap: sizes must be positive, got {max_len} -> {out_len}")
+    if interpolation == "nearest":
+        return 1
+    support = _FILTERS[interpolation][1] * max(max_len / out_len, 1.0)
+    return int(math.ceil(support)) * 2 + 1
+
+
+@functools.lru_cache(maxsize=1024)
+def axis_tables(in_len: int, out_len: int, interpolation: str = "nearest") -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """``(first, count, coef)`` of one axis of a per-sample block, memoised per (axis length, target, interpolation) -
+    ``resize_tables`` is plain Python and costs milliseconds per new length, and a stream of a few resolutions repeats
+    its axis lengths.  ``in_len == out_len`` gives the identity table.  The arrays are read-only."""
+    if in_len == out_len:
+        t = (np.arange(out_len, dtype=np.int32), np.ones(out_len, np.int32),
+             np.full((out_len, 1), 1 << PRECISION_BITS, np.int32))
+    else:
+        t = resize_tables(in_len, out_len, interpolation)
+    for a in t:
+        a.setflags(write=False)
+    return t
+
+
+def frame_block_ints(target, kw) -> int:
+    """int32 values in one sample's block for a model input ``target = (H_out, W_out)`` and ``kw = (kw_w, kw_h)``."""
+    (h_out, w_out), (kw_w, kw_h) = target, kw
+    return 2 + w_out * (2 + kw_w) + h_out * (2 + kw_h)
+
+
+def pack_frame_tables(hws, target, kw, interpolation: str = "nearest") -> np.ndarray:
+    """The blocks of images of sizes ``hws = [(h, w), ...]``: int32 ``[len(hws), frame_block_ints(target, kw)]``."""
+    (h_out, w_out), (kw_w, kw_h) = target, kw
+    blocks = np.zeros((len(hws), frame_block_ints(target, kw)), np.int32)
+    for blk, (h, w) in zip(blocks, hws):
+        blk[0], blk[1] = h, w
+        off = 2
+        for in_len, out_len, k in ((w, w_out, kw_w), (h, h_out, kw_h)):
+            first, count, coef = axis_tables(int(in_len), out_len, interpolation)
+            if coef.shape[1] > k:
+                raise ValueError(f"pack_frame_tables: {in_len} -> {out_len} ({interpolation}) needs {coef.shape[1]} taps, "
+                                 f"the block holds {k}")
+            b = blk[off:off + 2 * out_len].reshape(out_len, 2)
+            b[:, 0], b[:, 1] = first, count
+            off += 2 * out_len
+            blk[off:off + out_len * k].reshape(out_len, k)[:, :coef.shape[1]] = coef
+            off += out_len * k
+    return blocks
+
+
+def check_frame(x, max_image_size) -> np.ndarray:
+    """Queue item ``x`` of a ``max_image_size=(H, W)`` pipeline as a C-contiguous uint8 ``(k, h, w, 3)`` array (an
+    ``(h, w, 3)`` image counts as ``k = 1``) with ``1 <= h <= H`` and ``1 <= w <= W``, or a ValueError naming the bound."""
+    H, W = max_image_size
+    bound = f"max_image_size=({H}, {W})"
+    if not (isinstance(x, np.ndarray) and x.dtype == np.uint8):
+        raise ValueError(f"{bound} takes uint8 RGB images (img_to_array(img).astype(np.uint8)), got "
+                         f"{getattr(x, 'dtype', type(x).__name__)}; do not preprocess or resize them on the host")
+    if x.ndim == 3:
+        x = x[None]
+    if x.ndim != 4 or x.shape[0] < 1 or x.shape[-1] != 3:
+        raise ValueError(f"image shape {tuple(x.shape)} is not (k, h, w, 3), channels-last RGB ({bound})")
+    h, w = x.shape[1:3]
+    if not (1 <= h <= H and 1 <= w <= W):
+        raise ValueError(f"a {h}x{w} image is outside {bound}: needs 1 <= h <= {H} and 1 <= w <= {W}")
+    return np.ascontiguousarray(x)

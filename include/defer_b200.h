@@ -74,7 +74,24 @@ typedef enum defer_op_kind {
                          /*   w_kernel = [out_len, kw] fixed-point taps, 22 fractional bits;  kw = ksize          */
                          /*   y[i] = clamp((2^21 + sum_{k < count} x[first + k] * tap[k]) >> 22, 0, 255) per     */
                          /*   channel; 0 <= first, 1 <= count <= kw, first + count <= in_len (checked at create)  */
+                         /* `mode` DEFER_RESIZE_SAMPLE_W / _H: images of mixed sizes, tables per sample (below)   */
 } defer_op_kind;
+
+/* defer_op_desc.mode of a DEFER_OP_RESIZE op.  0: the fixed-size resize above (one image size per stage).
+ * The two per-sample modes come as a pair and take images of any size up to the stage input (H, W):
+ *   DEFER_RESIZE_SAMPLE_W  in0 = the stage input, U8 (H, W, 3)  ->  out U8 (H, W_out, 3)      kw = kw_w
+ *   DEFER_RESIZE_SAMPLE_H  in0 = that output, U8 (H, W_out, 3)  ->  out U8 (H_out, W_out, 3)  kw = kw_h
+ * They have no weights.  Each sample of a microbatch carries its own int32 table block, written next to its input slot
+ * by defer_stage_submit_frames:
+ *   [h_in, w_in,  width axis: (first, count) [W_out, 2], taps [W_out, kw_w],
+ *                 height axis: (first, count) [H_out, 2], taps [H_out, kw_h]]          (taps zero past count)
+ * with 1 <= h_in <= H, 1 <= w_in <= W; the image is packed as (h_in, w_in, 3) at the start of its slot.  An axis whose
+ * length equals the target has the identity table (first = i, count 1, tap 2^22).  The arithmetic is mode 0's.  The
+ * kernel clamps h_in / w_in, first and count into the slot, so no block content can make it read outside the slot, and
+ * the blocks are zeroed at create (a never-written sample reads as a 1x1 image of weight 0).  Both ops are always
+ * planned, even when an axis of the bound already equals the target, as the axis cannot be told from the shapes then. */
+#define DEFER_RESIZE_SAMPLE_W 1
+#define DEFER_RESIZE_SAMPLE_H 2
 
 /* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
 #define DEFER_PRE_CAFFE 0   /* keras_applications imagenet_utils mode='caffe' (ResNet50/101/152, VGG16) */
@@ -106,7 +123,7 @@ typedef struct defer_op_desc {
   int32_t w_kernel;        /* CONV: fp32 HWIO kernel;  DENSE: fp32 (in,out) kernel;  RESIZE: int32 taps */
   int32_t w_scale;         /* CONV / AFFINE: fp32 per-channel scale (NULL id -1 = ones);  RESIZE: int32 (first, count) */
   int32_t w_shift;         /* CONV / AFFINE / PREPROCESS: fp32 per-channel shift;  DENSE: bias */
-  int32_t mode;            /* PREPROCESS: DEFER_PRE_*;  every other kind: 0 */
+  int32_t mode;            /* PREPROCESS: DEFER_PRE_*;  RESIZE: 0 | DEFER_RESIZE_SAMPLE_*;  every other kind: 0 */
 } defer_op_desc;
 
 typedef struct defer_stage_config {
@@ -178,6 +195,14 @@ DEFER_API int defer_stage_submit_part(defer_stage_t s, uint64_t seq, int index, 
  * [first_index + i * samples_per_item, ...). */
 DEFER_API int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_index, int n_items, int samples_per_item,
                              const void* const* host_ptrs, uint64_t nbytes_per_item);
+/* First stage with a DEFER_RESIZE_SAMPLE_W / _H pair, images of mixed sizes: image i (hw[i] = (h, w), 1 <= h <= H,
+ * 1 <= w <= W of the stage input; h * w * 3 contiguous bytes at images[i]) goes to the start of sample slot
+ * first_index + i, and its table block (tables: n blocks, table_bytes = n x block bytes; header (h, w) equal to hw[i])
+ * next to the slots.  Only the images' own bytes are copied.  Everything is checked before anything is copied
+ * (DEFER_ERR_INVALID, nothing copied).  The copies go on the lane's stream; memory as for defer_stage_submit.
+ * defer_stage_submit / _part / _parts refuse such a stage. */
+DEFER_API int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* images,
+                              const int32_t* hw /* [n][2] */, const int32_t* tables, uint64_t table_bytes);
 /* Enqueue microbatch `seq` on lane seq % depth: wait-input -> kernel chain -> hop -> flags. Async. */
 DEFER_API int defer_stage_step(defer_stage_t s, uint64_t seq);
 /* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host.  A lane keeps only the output
@@ -258,6 +283,12 @@ DEFER_API int defer_k_preprocess_tf(const uint8_t* x, float* y, int n, int h, in
  * bounds = int32 [out_len, 2] (first, count) and taps = int32 [out_len, ksize] on the device (not validated here). */
 DEFER_API int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n,
                              int h_in, int w_in, int h_out, int w_out, int c, void* stream);
+
+/* One pass of a DEFER_RESIZE_SAMPLE_W / _H pair (pass = that mode) over n samples: SAMPLE_W reads x = (n, H, W, 3) slots
+ * and writes y = (n, H, W_out, 3); SAMPLE_H reads x = (n, H, W_out, 3) and writes y = (n, H_out, W_out, 3).  tables = n
+ * int32 blocks of the layout above (kw_w, kw_h taps), on the device, 4-byte aligned; c must be 3. */
+DEFER_API int defer_k_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W,
+                                    int H_out, int W_out, int kw_w, int kw_h, int c, void* stream);
 
 #ifdef __cplusplus
 }

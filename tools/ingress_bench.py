@@ -17,14 +17,22 @@ gives them, and two more arms run in the same alternation:
   e  uint8 frames on a full input queue, DEFER(preprocess=mode, image_size=..., interpolation=...): the first stage
      resizes and preprocesses on the GPU
 
+With --mixed-sizes HxW,HxW,... one more arm runs in the alternation:
+
+  f  uint8 frames cycling through those sizes on a full input queue, DEFER(preprocess=mode, max_image_size=the largest,
+     interpolation=...): each frame is resized on the GPU from its own size, frames of different sizes share a microbatch
+
 It prints one JSON line: end-to-end inferences/s per arm (median, min, max over the rounds), H2D bytes per item, the
 device time of the fp32 fused stem, the uint8 fused stem of the mode and its standalone preprocessing kernel (time_op,
 L2 flushed), the host time of one preprocessing call, and the card's name and power limit (read-only nvidia-smi query);
-with --image-size also the host time of one Pillow resize and the time_op of each RESIZE op at 32 frames.
+with --image-size also the host time of one Pillow resize and the time_op of each RESIZE op at 32 frames; with
+--mixed-sizes the time_op of the two per-sample RESIZE ops at 32 mixed frames and at 32 frames of the first size (under
+a bound of that size), and arm f's H2D bytes per item (the image's own bytes plus its table block).
 
     python tools/ingress_bench.py [--model resnet50 --preprocess caffe] [--items 640] [--reps 3]
     python tools/ingress_bench.py --model resnet50v2 --preprocess tf
     python tools/ingress_bench.py --image-size 480x640 --interpolation bilinear
+    python tools/ingress_bench.py --image-size 480x640 --mixed-sizes 480x640,720x1280,1080x1920
 """
 from __future__ import annotations
 
@@ -46,6 +54,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 from defer_b200 import applications  # noqa: E402
 from defer_b200.dispatcher import DEFER  # noqa: E402
 from defer_b200.node import StageRunner  # noqa: E402
+from defer_b200.resize import frame_block_ints  # noqa: E402
 
 G, DEPTH = 32, 4
 MODELS = {"resnet50": applications.ResNet50, "resnet50v2": applications.ResNet50V2}
@@ -164,6 +173,29 @@ def resize_times(model, mode, image_size, interpolation, iters):
     return out
 
 
+def frames_times(model, mode, bound, sizes, interpolation, iters):
+    """time_op (us) of the two per-sample RESIZE ops at 32 frames cycling through ``sizes`` under ``bound``, L2 flushed."""
+    r = StageRunner.from_model(model, device=0, dtype="float32", max_batch=G, depth=1, preprocess=mode,
+                               max_image_size=bound, interpolation=interpolation)
+    out = {"bound": list(bound), "sizes": [list(v) for v in sizes]}
+    try:
+        r.predict_frames([applications.synthetic_image(1, sizes[i % len(sizes)] + (3,), seed=i) for i in range(G)])
+        for i, op in enumerate(r.plan.ops[:2]):
+            ts = [r.time_op(i, iters=iters, flush_l2=True) for _ in range(3)]
+            out[op.layers[0]] = {"kernel": r.op_info(i)["kernel"], "us": round(statistics.median(ts), 2),
+                                 "spread_us": round(max(ts) - min(ts), 2), "alg_bytes_bound": r.op_info(i)["alg_bytes"]}
+    finally:
+        r.close()
+    return out
+
+
+def parse_size(text):
+    h, w = (int(v) for v in text.lower().split("x"))
+    if min(h, w) < 1:
+        raise ValueError(text)
+    return h, w
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--items", type=int, default=640, help="queue items per timed round (batch-1 images)")
@@ -174,6 +206,7 @@ def main():
                     help="Keras preprocessing mode (the model's own: caffe for resnet50, tf for resnet50v2)")
     ap.add_argument("--image-size", default=None, help="HxW of uint8 frames for arms d and e, e.g. 480x640")
     ap.add_argument("--interpolation", choices=applications.INTERPOLATIONS, default="nearest")
+    ap.add_argument("--mixed-sizes", default=None, help="HxW,HxW,... of uint8 frames for arm f, e.g. 480x640,720x1280")
     args = ap.parse_args()
     if args.reps < 3:
         ap.error("--reps must be >= 3")
@@ -184,6 +217,13 @@ def main():
             assert len(image_size) == 2 and min(image_size) >= 1
         except (ValueError, AssertionError):
             ap.error(f"--image-size {args.image_size!r}: expected HxW, e.g. 480x640")
+    mixed = None
+    if args.mixed_sizes:
+        try:
+            mixed = [parse_size(v) for v in args.mixed_sizes.split(",")]
+        except ValueError:
+            ap.error(f"--mixed-sizes {args.mixed_sizes!r}: expected HxW,HxW,..., e.g. 480x640,720x1280")
+        bound = (max(h for h, _ in mixed), max(w for _, w in mixed))
 
     model = MODELS[args.model]()
     host_fn = HOST_PREPROCESS[args.preprocess]
@@ -210,6 +250,11 @@ def main():
         arms["e_u8_gpu_resize"] = Arm(model, args.preprocess, None, image_size=image_size, interpolation=args.interpolation)
         feeds["d_u8_host_resize"] = (frames, True)
         feeds["e_u8_gpu_resize"] = (frames, False)
+    if mixed is not None:
+        mixed_frames = [applications.synthetic_image(1, mixed[i % len(mixed)] + (3,), seed=i) for i in range(args.items)]
+        arms["f_u8_gpu_resize_mixed"] = Arm(model, args.preprocess, None, max_image_size=bound,
+                                            interpolation=args.interpolation)
+        feeds["f_u8_gpu_resize_mixed"] = (mixed_frames, False)
     rates = {k: [] for k in arms}
     try:
         for rnd in range(args.reps + 1):
@@ -219,6 +264,10 @@ def main():
                 if rnd > 0:                                   # round 0 warms every shape up
                     rates[k].append(r)
         h2d = {k: arm.h2d_per_item for k, arm in arms.items()}
+        if mixed is not None:                                 # only the image's own bytes cross, plus its block
+            plan = arms["f_u8_gpu_resize_mixed"].defer.stages[0].plan.frames
+            block = frame_block_ints(plan["target"], plan["kw"]) * 4
+            h2d["f_u8_gpu_resize_mixed"] = round(statistics.mean(x.nbytes for x in mixed_frames) + block, 1)
     finally:
         for arm in arms.values():
             arm.close()
@@ -235,6 +284,14 @@ def main():
         res.update({"image_size": list(image_size), "interpolation": args.interpolation,
                     "host_pillow_resize_us": round(resize_us, 1),
                     "resize_time_op": resize_times(model, args.preprocess, image_size, args.interpolation, args.op_iters)})
+    if mixed is not None:
+        res.update({"mixed_sizes": [list(v) for v in mixed], "max_image_size": list(bound),
+                    "frames_time_op": {"mixed": frames_times(model, args.preprocess, bound, mixed, args.interpolation,
+                                                             args.op_iters),
+                                       "uniform": frames_times(model, args.preprocess, mixed[0], mixed[:1],
+                                                               args.interpolation, args.op_iters)}})
+        if image_size is None:
+            res["interpolation"] = args.interpolation
     res.update(card())
     print(json.dumps(res), flush=True)
 
