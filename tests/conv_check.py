@@ -8,6 +8,9 @@ every convolution check asserts on:
 * per-output-channel: max over c of max|y_c - ref_c| / max|ref_c|.  An epilogue error confined to channels with small
   outputs (a wrong shift, scale or residual plane for a few channels) hides under the global max norm; it does not
   hide here.
+
+These bars are the precision check for random operands.  Every executor is also checked bit for bit against exact
+expected bits on exactly summable operands (tests/exact_conv.py, tests/test_gpu_conv_exact.py), which one wrong term fails.
 """
 import ctypes as C
 
