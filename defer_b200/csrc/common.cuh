@@ -199,6 +199,11 @@ int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int
 // samples reads its size and tables from its int32 block in `tables` (layout: include/defer_b200.h).
 int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,
                          int W_out, int kw_w, int kw_h, cudaStream_t st);
+// DEFER_OP_JPEG_DECODE (jpeg.cu): n JPEG files in H * W * 3-byte slots, with their blocks -> n U8 (H, W, 3) images, through a
+// workspace of jpeg_workspace_bytes(H, W, n) (256-byte aligned)
+size_t jpeg_workspace_bytes(int H, int W, int n);
+int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
+                       cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

@@ -1,0 +1,616 @@
+// jpeg.cu - DEFER_OP_JPEG_DECODE: baseline JPEG files decoded on the GPU, bit for bit as libjpeg-turbo 3.1 (through Pillow)
+// decodes them, and as defer_b200/jpeg.py restates it.  Three kernels per microbatch, each with a fixed grid sized from the
+// slot bound (H, W) and an early exit per sample:
+//   jpeg_entropy_kernel  one CTA per sample: unstuff the entropy data, Huffman-decode it by self-synchronisation,
+//                        write de-zigzagged int16 coefficients, then the DC prediction as a segmented prefix sum
+//   jpeg_idct_kernel     dequantise + libjpeg's integer ISLOW IDCT, 8 threads per 8x8 block, into MCU-padded planes
+//   jpeg_color_kernel    libjpeg-turbo's fancy upsampling (h2v1 / h2v2) + jdcolor.c's fixed-point YCbCr -> RGB, one
+//                        thread per pixel, packed (h, w, 3) at the start of the sample's U8 slot
+// Nothing here trusts the per-sample block: sizes, sampling, offsets and table entries are clamped, so a stale, zero or
+// corrupt block gives wrong pixels, never an access outside the sample's slot or workspace.
+#include <climits>
+
+#include <cub/block/block_scan.cuh>
+
+#include "common.cuh"
+
+namespace defer {
+
+namespace {
+
+constexpr int JT = 512;          // threads of the entropy kernel (one CTA per sample)
+constexpr int UNSTUFF_ITEMS = 8; // entropy bytes per thread per unstuff step
+constexpr int S_BITS = DEFER_JPEG_SUBSEQ_BITS;
+constexpr int LUT = 1 << DEFER_JPEG_LOOKAHEAD;
+constexpr int HUFF = DEFER_JPEG_HUFF_INTS;
+constexpr int Q_OFF = DEFER_JPEG_HDR_INTS;
+constexpr int T_OFF = DEFER_JPEG_HDR_INTS + 3 * 64;
+
+__constant__ int c_zigzag[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
+                                 41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
+                                 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
+
+// Geometry of one sample, derived from its block header and clamped into the slot (H, W).
+struct Geom {
+  int h, w, ncomp, hs, vs, ri;
+  int mcux, mcuy, mcus, bpm, nb0, blocks, nseg;
+  int bw[3], bh[3];
+  size_t poff[3];
+  int off, len;   // entropy data within the file slot
+};
+
+__device__ __forceinline__ Geom geom(const int32_t* blk, int H, int W, size_t slot) {
+  Geom g;
+  g.h = min(max(blk[0], 1), H);
+  g.w = min(max(blk[1], 1), W);
+  g.ncomp = blk[2] == 3 ? 3 : 1;
+  g.hs = g.ncomp == 3 ? min(max(blk[3], 1), 2) : 1;
+  g.vs = g.ncomp == 3 ? min(max(blk[4], 1), 2) : 1;
+  if (g.vs == 2) g.hs = 2;               // 4:4:0 is refused by the parser; keep a corrupt block inside 4:2:0's bounds
+  g.ri = min(max(blk[5], 0), 65535);
+  const long long off = min(max((long long)blk[6], 0ll), (long long)slot);
+  g.off = (int)off;
+  g.len = (int)min(max((long long)blk[7], 0ll), (long long)slot - off);
+  g.mcux = (g.w + 8 * g.hs - 1) / (8 * g.hs);
+  g.mcuy = (g.h + 8 * g.vs - 1) / (8 * g.vs);
+  g.mcus = g.mcux * g.mcuy;
+  g.nb0 = g.hs * g.vs;
+  g.bpm = g.ncomp == 3 ? g.nb0 + 2 : 1;
+  g.blocks = g.mcus * g.bpm;
+  g.nseg = g.ri ? (g.mcus + g.ri - 1) / g.ri : 1;
+  size_t p = 0;
+  for (int c = 0; c < 3; ++c) {
+    const bool y = c == 0;
+    g.bw[c] = c < g.ncomp ? g.mcux * (y ? g.hs : 1) : 0;
+    g.bh[c] = c < g.ncomp ? g.mcuy * (y ? g.vs : 1) : 0;
+    g.poff[c] = p;
+    p += (size_t)g.bw[c] * g.bh[c] * 64;
+  }
+  return g;
+}
+
+__device__ __forceinline__ int comp_of(const Geom& g, int j) { return j < g.nb0 ? 0 : j - g.nb0 + 1; }
+
+// 16 bits at bit `pos` of buf, MSB first; bytes at or past end_bits / 8 read as zero (end_bits is a byte multiple)
+__device__ __forceinline__ uint32_t peek16(const uint8_t* __restrict__ buf, int pos, int end_bits) {
+  if (pos >= end_bits) return 0;
+  const int i = pos >> 3, nb = end_bits >> 3;
+  uint32_t v = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) v = (v << 8) | (i + q < nb ? (uint32_t)buf[i + q] : 0u);
+  return (v >> (16 - (pos & 7))) & 0xFFFFu;
+}
+
+// symbol of the code at the top of `p` and its length, or -1 for an invalid code (table layout: include/defer_b200.h)
+__device__ __forceinline__ int decode_sym(const int* __restrict__ t, uint32_t p, int& len) {
+  const int e = t[p >> (16 - DEFER_JPEG_LOOKAHEAD)];
+  if (e) {
+    len = min(max(e >> 8, 1), 16);
+    return e & 255;
+  }
+  for (int l = DEFER_JPEG_LOOKAHEAD + 1; l <= 16; ++l) {
+    const int code = (int)(p >> (16 - l));
+    if (code <= t[LUT + l]) {
+      len = l;
+      return t[LUT + 34 + min(max(code + t[LUT + 17 + l], 0), 255)] & 255;
+    }
+  }
+  return -1;
+}
+
+__device__ __forceinline__ int extend(int v, int s) { return (s && v < (1 << (s - 1))) ? v - (1 << s) + 1 : v; }
+
+// One symbol (code + extra bits) at coefficient k of a block (0 = DC).  Advances pos and k (k == 64 ends the block) and
+// sets z (zigzag index written, -1 for none) and v.  false: invalid code, or an AC run past coefficient 63.
+__device__ __forceinline__ bool jstep(const uint8_t* __restrict__ buf, int end_bits, const int* dct, const int* act,
+                                      int& pos, int& k, int& z, int& v) {
+  const uint32_t p = peek16(buf, pos, end_bits);
+  int l;
+  if (k == 0) {
+    int s = decode_sym(dct, p, l);
+    if (s < 0) return false;
+    s &= 15;
+    pos += l;
+    v = s ? extend((int)(peek16(buf, pos, end_bits) >> (16 - s)), s) : 0;
+    pos += s;
+    k = 1;
+    z = 0;
+    return true;
+  }
+  const int sym = decode_sym(act, p, l);
+  if (sym < 0) return false;
+  pos += l;
+  const int r = sym >> 4, s = sym & 15;
+  z = -1;
+  if (s == 0) {
+    if (r != 15) {
+      k = 64;
+      return true;
+    }
+    if (k + 16 > 64) return false;
+    k += 16;
+    return true;
+  }
+  if (k + r > 63) return false;
+  v = extend((int)(peek16(buf, pos, end_bits) >> (16 - s)), s);
+  pos += s;
+  z = k + r;
+  k = z + 1;
+  return true;
+}
+
+// Decode from state (pos, j << 8 | k) to the first symbol boundary at or past `end`; returns the blocks that start before
+// `end`.  An invalid code restarts the decode one bit later at block 0, coefficient 0.  A decoder that started at a guessed
+// state meets invalid codes often; if it stopped there, the true state could only reach the subsequences behind it one
+// per round.  On the true path an invalid code is a real error: the write pass finds it and cuts the decode there, so
+// what this path does after it is never used.
+__device__ int sync_run(const uint8_t* __restrict__ buf, int seg_end, int end, const int* tabs, const Geom& g, int& pos,
+                        int& jk) {
+  int j = jk >> 8, k = jk & 255, count = 0;
+  while (pos < end) {
+    if (k == 0) ++count;
+    const int c = comp_of(g, j);
+    const int p0 = pos;
+    int z, v;
+    if (!jstep(buf, seg_end, tabs + c * HUFF, tabs + (3 + c) * HUFF, pos, k, z, v)) {
+      pos = p0 + 1;
+      j = k = 0;
+      continue;
+    }
+    if (k >= 64) {
+      k = 0;
+      j = j + 1 == g.bpm ? 0 : j + 1;
+    }
+  }
+  jk = (j << 8) | k;
+  return count;
+}
+
+struct SegPair {
+  int f;
+  unsigned v;
+};
+struct SegSum {
+  __device__ __forceinline__ SegPair operator()(const SegPair& a, const SegPair& b) const {
+    return SegPair{a.f | b.f, b.f ? b.v : a.v + b.v};
+  }
+};
+
+}  // namespace
+
+// Per-sample workspace layout (byte offsets from the sample's base); host and device compute it the same way.
+struct JpegWs {
+  size_t stats, coef, planes, comp, seg_start, seg_total, sub_base, sub, stride;
+  int mcu_cap, blocks_cap, subs_cap;
+  size_t slot;
+};
+enum { SUB_SEG, SUB_EPOS, SUB_EJK, SUB_XPOS, SUB_XJK, SUB_CNT, SUB_PRE, SUB_PPOS, SUB_PJK, SUB_FIELDS };
+
+__host__ __device__ inline JpegWs jpeg_ws(int H, int W) {
+  JpegWs L;
+  const int hp = (H + 15) / 16 * 16, wp = (W + 15) / 16 * 16;
+  L.slot = (size_t)H * W * 3;
+  L.mcu_cap = (hp / 8) * (wp / 8);
+  L.blocks_cap = 3 * L.mcu_cap;
+  L.subs_cap = (int)((L.slot * 8 + S_BITS - 1) / S_BITS) + L.mcu_cap;
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  size_t o = 0;
+  L.stats = o;      o += al(64);
+  L.coef = o;       o += al((size_t)L.blocks_cap * 128);
+  L.planes = o;     o += al((size_t)L.blocks_cap * 64);
+  L.comp = o;       o += al(L.slot + 16);
+  L.seg_start = o;  o += al(((size_t)L.mcu_cap + 2) * 4);
+  L.seg_total = o;  o += al(((size_t)L.mcu_cap + 1) * 4);
+  L.sub_base = o;   o += al(((size_t)L.mcu_cap + 1) * 4);
+  L.sub = o;        o += al((size_t)L.subs_cap * SUB_FIELDS * 4);
+  L.stride = o;
+  return L;
+}
+
+namespace {
+
+__global__ void __launch_bounds__(JT) jpeg_entropy_kernel(const uint8_t* __restrict__ files, const int32_t* __restrict__ blocks,
+                                                          uint8_t* __restrict__ ws, int H, int W, JpegWs L) {
+  using ScanI = cub::BlockScan<int, JT>;
+  using ScanP = cub::BlockScan<SegPair, JT>;
+  __shared__ union {
+    typename ScanI::TempStorage i;
+    typename ScanP::TempStorage p;
+  } tmp;
+  __shared__ int tabs[6 * HUFF];
+  __shared__ int sh_int[8];
+  const int s = blockIdx.x, tid = threadIdx.x;
+  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const Geom g = geom(blk, H, W, L.slot);
+  uint8_t* base = ws + (size_t)s * L.stride;
+  int32_t* stats = reinterpret_cast<int32_t*>(base + L.stats);
+  int16_t* coef = reinterpret_cast<int16_t*>(base + L.coef);
+  uint8_t* comp = base + L.comp;
+  int32_t* seg_start = reinterpret_cast<int32_t*>(base + L.seg_start);
+  int32_t* seg_total = reinterpret_cast<int32_t*>(base + L.seg_total);
+  int32_t* sub_base = reinterpret_cast<int32_t*>(base + L.sub_base);
+  int32_t* sub = reinterpret_cast<int32_t*>(base + L.sub);
+  auto F = [&](int field, int t) -> int32_t& { return sub[(size_t)field * L.subs_cap + t]; };
+  for (int i = tid; i < 6 * HUFF; i += JT) tabs[i] = blk[T_OFF + i];
+
+  // ---- 1. unstuff: drop 0x00 / RSTn after 0xFF and the 0xFF of RSTn; record where each restart interval starts
+  const uint8_t* src = files + (size_t)s * L.slot + g.off;
+  int out_n = 0, rst_n = 0;
+  for (int c0 = 0; c0 < g.len; c0 += JT * UNSTUFF_ITEMS) {
+    const int i0 = c0 + tid * UNSTUFF_ITEMS;
+    uint8_t b[UNSTUFF_ITEMS];
+    unsigned keep = 0, mark = 0;
+    int nk = 0, nr = 0;
+#pragma unroll
+    for (int q = 0; q < UNSTUFF_ITEMS; ++q) {
+      const int i = i0 + q;
+      b[q] = 0;
+      if (i >= g.len) continue;
+      const int x = src[i], prev = i > 0 ? src[i - 1] : 0, next = i + 1 < g.len ? src[i + 1] : 0;
+      b[q] = (uint8_t)x;
+      const bool rst = x >= 0xD0 && x <= 0xD7, m = x == 0xFF && next >= 0xD0 && next <= 0xD7;
+      if (!((prev == 0xFF && (x == 0 || rst)) || m)) keep |= 1u << q, ++nk;
+      if (m) mark |= 1u << q, ++nr;
+    }
+    int pre, tot;
+    ScanI(tmp.i).ExclusiveSum(nk | (nr << 16), pre, tot);
+    int pos = out_n + (pre & 0xFFFF), r = rst_n + (pre >> 16);
+#pragma unroll
+    for (int q = 0; q < UNSTUFF_ITEMS; ++q) {
+      if (mark >> q & 1) {
+        if (r + 1 <= g.nseg) seg_start[r + 1] = pos;
+        ++r;
+      }
+      if (keep >> q & 1) comp[pos++] = b[q];
+    }
+    out_n += tot & 0xFFFF;
+    rst_n += tot >> 16;
+    __syncthreads();
+  }
+  const int T = out_n, R = rst_n;
+  // ---- 2. restart intervals and their subsequences of S_BITS bits
+  for (int k = tid; k <= g.nseg; k += JT) {
+    if (k == 0) seg_start[0] = 0;
+    else if (k > R) seg_start[k] = T;
+    if (k < g.nseg) seg_total[k] = 0;
+  }
+  __syncthreads();
+  int nsubs = 0;
+  for (int k0 = 0; k0 < g.nseg; k0 += JT) {
+    const int k = k0 + tid;
+    const int n_k = k < g.nseg ? (int)(((long long)(seg_start[k + 1] - seg_start[k]) * 8 + S_BITS - 1) / S_BITS) : 0;
+    int pre, tot;
+    ScanI(tmp.i).ExclusiveSum(n_k, pre, tot);
+    if (k < g.nseg) sub_base[k] = nsubs + pre;
+    nsubs += tot;
+    __syncthreads();
+  }
+  nsubs = min(nsubs, L.subs_cap);
+  // ---- 3. every subsequence decodes from the default state at its first bit
+  for (int t = tid; t < nsubs; t += JT) {
+    int lo = 0, hi = g.nseg - 1;          // the last interval whose first subsequence is <= t
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (sub_base[mid] <= t) lo = mid; else hi = mid - 1;
+    }
+    const int a = seg_start[lo] * 8, e = seg_start[lo + 1] * 8;
+    int pos = a + (t - sub_base[lo]) * S_BITS, jk = 0;
+    const int end = min(pos + S_BITS, e);
+    F(SUB_SEG, t) = lo;
+    F(SUB_EPOS, t) = pos;
+    F(SUB_EJK, t) = 0;
+    F(SUB_CNT, t) = sync_run(comp, e, end, tabs, g, pos, jk);
+    F(SUB_XPOS, t) = pos;
+    F(SUB_XJK, t) = jk;
+  }
+  // ---- 4. synchronise: a subsequence whose predecessor (same interval) left in another state than it entered re-decodes
+  //         from there; until no entry changes.  The first subsequence of an interval starts at a known state.
+  int rounds = 1;
+  auto sub_end = [&](int t, int& seg_end) {
+    const int k = F(SUB_SEG, t);
+    seg_end = seg_start[k + 1] * 8;
+    return min(seg_start[k] * 8 + (t - sub_base[k] + 1) * S_BITS, seg_end);
+  };
+  for (;;) {
+    __syncthreads();
+    if (tid == 0) sh_int[0] = 0;
+    for (int t = tid; t < nsubs; t += JT) {
+      F(SUB_PPOS, t) = INT_MIN;
+      if (t == 0 || F(SUB_SEG, t - 1) != F(SUB_SEG, t)) continue;
+      const int np = F(SUB_XPOS, t - 1), njk = F(SUB_XJK, t - 1);
+      if (np != F(SUB_EPOS, t) || njk != F(SUB_EJK, t)) {
+        F(SUB_PPOS, t) = np;
+        F(SUB_PJK, t) = njk;
+      }
+    }
+    __syncthreads();
+    for (int t = tid; t < nsubs; t += JT) {
+      int pos = F(SUB_PPOS, t);
+      if (pos == INT_MIN) continue;
+      int jk = F(SUB_PJK, t);
+      F(SUB_EPOS, t) = pos;
+      F(SUB_EJK, t) = jk;
+      int seg_end;
+      const int end = sub_end(t, seg_end);
+      F(SUB_CNT, t) = sync_run(comp, seg_end, end, tabs, g, pos, jk);
+      F(SUB_XPOS, t) = pos;
+      F(SUB_XJK, t) = jk;
+      sh_int[0] = 1;
+    }
+    __syncthreads();
+    if (!sh_int[0]) break;
+    ++rounds;
+  }
+  // ---- 5. block positions: prefix sum of the blocks each subsequence starts
+  {
+    int carry = 0;
+    for (int t0 = 0; t0 < nsubs; t0 += JT) {
+      const int t = t0 + tid;
+      int pre, tot;
+      ScanI(tmp.i).ExclusiveSum(t < nsubs ? F(SUB_CNT, t) : 0, pre, tot);
+      if (t < nsubs) F(SUB_PRE, t) = carry + pre;
+      carry += tot;
+      __syncthreads();
+    }
+  }
+  if (tid == 0) sh_int[1] = g.blocks;    // first block that did not decode (cutoff)
+  __syncthreads();
+  for (int t = tid; t < nsubs; t += JT) {
+    const int k = F(SUB_SEG, t);
+    const int exp_k = (g.ri ? min(g.ri, g.mcus - k * g.ri) : g.mcus) * g.bpm;
+    const int done = F(SUB_PRE, t) - F(SUB_PRE, sub_base[k]);
+    if (t + 1 == nsubs || F(SUB_SEG, t + 1) != k) seg_total[k] = min(done + F(SUB_CNT, t), exp_k);
+  }
+  // ---- 6. write the coefficients: each block by the subsequence it starts in, all 64 values, zero runs included
+  for (int t = tid; t < nsubs; t += JT) {
+    int pos = F(SUB_EPOS, t);
+    const int k_seg = F(SUB_SEG, t);
+    int seg_end;
+    const int end = sub_end(t, seg_end);
+    int j = F(SUB_EJK, t) >> 8, k = F(SUB_EJK, t) & 255, z, v;
+    bool ok = true;
+    while (k != 0) {                     // the tail of a block that started in the predecessor
+      const int c = comp_of(g, j);
+      if (!jstep(comp, seg_end, tabs + c * HUFF, tabs + (3 + c) * HUFF, pos, k, z, v)) { ok = false; break; }
+      if (k >= 64) k = 0, j = j + 1 == g.bpm ? 0 : j + 1;
+    }
+    if (!ok) continue;
+    const int exp_k = (g.ri ? min(g.ri, g.mcus - k_seg * g.ri) : g.mcus) * g.bpm;
+    const int first = g.ri ? k_seg * g.ri * g.bpm : 0;
+    int idx = F(SUB_PRE, t) - F(SUB_PRE, sub_base[k_seg]);
+    while (pos < end && idx < exp_k) {
+      const int b = first + idx;
+      int16_t* out = coef + (size_t)b * 64;
+      const int c = comp_of(g, j);
+      do {
+        const int k0 = k;
+        if (!jstep(comp, seg_end, tabs + c * HUFF, tabs + (3 + c) * HUFF, pos, k, z, v)) { ok = false; break; }
+        for (int q = k0; q < k; ++q) out[c_zigzag[q]] = (int16_t)(q == z ? v : 0);
+      } while (k < 64);
+      if (!ok) {
+        atomicMin(&sh_int[1], b);
+        break;
+      }
+      k = 0;
+      j = j + 1 == g.bpm ? 0 : j + 1;
+      ++idx;
+    }
+  }
+  __syncthreads();
+  const int cutoff = sh_int[1];
+  // ---- 7. DC prediction: per component, a prefix sum in int32 segmented by restart interval; blocks that did not decode
+  //         are zero
+  for (int c = 0; c < g.ncomp; ++c) {
+    const int nbc = c == 0 ? g.nb0 : 1, offc = c == 0 ? 0 : g.nb0 + c - 1;
+    const int nq = g.mcus * nbc;
+    unsigned carry = 0;
+    for (int q0 = 0; q0 < nq; q0 += JT) {
+      const int q = q0 + tid;
+      int b = 0;
+      bool valid = false;
+      SegPair in{0, 0u};
+      if (q < nq) {
+        const int m = q / nbc, kseg = g.ri ? m / g.ri : 0;
+        b = m * g.bpm + offc + q % nbc;
+        in.f = q % nbc == 0 && (g.ri ? m % g.ri == 0 : m == 0);
+        valid = b < cutoff && b - (g.ri ? kseg * g.ri * g.bpm : 0) < seg_total[kseg];
+        in.v = valid ? (unsigned)(int)coef[(size_t)b * 64] : 0u;
+      }
+      SegPair out;
+      __syncthreads();
+      ScanP(tmp.p).InclusiveScan(in, out, SegSum());
+      const unsigned sum = out.f ? out.v : carry + out.v;
+      __syncthreads();
+      if (q < nq) {
+        int16_t* blkc = coef + (size_t)b * 64;
+        if (valid) {
+          blkc[0] = (int16_t)(int)sum;
+        } else {
+          for (int i = 0; i < 64; ++i) blkc[i] = 0;
+        }
+      }
+      if (tid == JT - 1) sh_int[2] = (int)sum;
+      __syncthreads();
+      carry = (unsigned)sh_int[2];
+    }
+  }
+  if (tid == 0) {
+    stats[0] = T;
+    stats[1] = R;
+    stats[2] = nsubs;
+    stats[3] = rounds;
+    stats[4] = cutoff;
+  }
+}
+
+// jidctint.c's ISLOW butterflies on one column (pass 1, descale by CONST_BITS - PASS1_BITS, stored as int) or one row
+// (pass 2, descale by CONST_BITS + PASS1_BITS + 3)
+__device__ __forceinline__ void idct_1d(const long long* s, long long* o, int sh) {
+  long long z2 = s[2], z3 = s[6];
+  long long z1 = (z2 + z3) * 4433;
+  const long long tmp2e = z1 + z3 * -15137, tmp3e = z1 + z2 * 6270;
+  const long long t0 = (s[0] + s[4]) * 8192, t1 = (s[0] - s[4]) * 8192;
+  const long long t10 = t0 + tmp3e, t13 = t0 - tmp3e, t11 = t1 + tmp2e, t12 = t1 - tmp2e;
+  long long tmp0 = s[7], tmp1 = s[5], tmp2 = s[3], tmp3 = s[1];
+  z1 = tmp0 + tmp3;
+  z2 = tmp1 + tmp2;
+  z3 = tmp0 + tmp2;
+  long long z4 = tmp1 + tmp3;
+  const long long z5 = (z3 + z4) * 9633;
+  tmp0 *= 2446;
+  tmp1 *= 16819;
+  tmp2 *= 25172;
+  tmp3 *= 12299;
+  z1 *= -7373;
+  z2 *= -20995;
+  z3 = z3 * -16069 + z5;
+  z4 = z4 * -3196 + z5;
+  tmp0 += z1 + z3;
+  tmp1 += z2 + z4;
+  tmp2 += z2 + z3;
+  tmp3 += z1 + z4;
+  const long long r = 1ll << (sh - 1);
+  o[0] = (t10 + tmp3 + r) >> sh;
+  o[7] = (t10 - tmp3 + r) >> sh;
+  o[1] = (t11 + tmp2 + r) >> sh;
+  o[6] = (t11 - tmp2 + r) >> sh;
+  o[2] = (t12 + tmp1 + r) >> sh;
+  o[5] = (t12 - tmp1 + r) >> sh;
+  o[3] = (t13 + tmp0 + r) >> sh;
+  o[4] = (t13 - tmp0 + r) >> sh;
+}
+
+constexpr int IDCT_BLOCKS = 16;   // 8x8 blocks per CTA, 8 threads each
+
+__global__ void __launch_bounds__(IDCT_BLOCKS * 8) jpeg_idct_kernel(const int32_t* __restrict__ blocks, uint8_t* __restrict__ ws,
+                                                                    int H, int W, JpegWs L) {
+  __shared__ int wsp[IDCT_BLOCKS][64];
+  const int s = blockIdx.y, lb = threadIdx.x >> 3, r = threadIdx.x & 7;
+  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const Geom g = geom(blk, H, W, L.slot);
+  const int b = blockIdx.x * IDCT_BLOCKS + lb;
+  if (b >= g.blocks) return;               // the 8 threads of a block leave together
+  const unsigned grp = 0xFFu << (threadIdx.x & 24);
+  uint8_t* base = ws + (size_t)s * L.stride;
+  const int16_t* cf = reinterpret_cast<const int16_t*>(base + L.coef) + (size_t)b * 64;
+  const int m = b / g.bpm, j = b % g.bpm, c = comp_of(g, j);
+  const int mx = m % g.mcux, my = m / g.mcux;
+  const int bx = c == 0 ? mx * g.hs + j % g.hs : mx, by = c == 0 ? my * g.vs + j / g.hs : my;
+  const int32_t* q = blk + Q_OFF + 64 * c;
+  long long in[8], o[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) in[k] = (long long)cf[k * 8 + r] * (long long)q[k * 8 + r];
+  idct_1d(in, o, 11);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) wsp[lb][k * 8 + r] = (int)o[k];
+  __syncwarp(grp);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) in[k] = wsp[lb][r * 8 + k];
+  idct_1d(in, o, 18);
+  uint32_t px[2] = {0, 0};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int v = (int)(((o[k] & 1023) ^ 512) - 512) + 128;   // idct_range_limit[x & RANGE_MASK]
+    px[k >> 2] |= (uint32_t)min(max(v, 0), 255) << (8 * (k & 3));
+  }
+  const int rs = g.bw[c] * 8;
+  uint8_t* dst = base + L.planes + g.poff[c] + (size_t)(by * 8 + r) * rs + bx * 8;
+  *reinterpret_cast<uint2*>(dst) = make_uint2(px[0], px[1]);
+}
+
+// chroma sample at output pixel (x, y) of a plane downsampled by (hs, vs): libjpeg-turbo's h2v1 / h2v2 fancy upsampling
+// when the downsampled width exceeds 2, else replication
+__device__ __forceinline__ int upsample(const uint8_t* __restrict__ p, int rs, int x, int y, int h, int w, int hs, int vs) {
+  if (hs == 1) return p[(size_t)y * rs + x];
+  const int dw = (w + 1) >> 1, i = x >> 1, odd = x & 1;
+  if (dw <= 2) return p[(size_t)(y / vs) * rs + i];
+  const int in_ = odd ? min(i + 1, dw - 1) : max(i - 1, 0);
+  if (vs == 1) {
+    const uint8_t* row = p + (size_t)y * rs;
+    const int a = row[i], n = row[in_];
+    if (odd) return i == dw - 1 ? a : (3 * a + n + 2) >> 2;
+    return i == 0 ? a : (3 * a + n + 1) >> 2;
+  }
+  const int dh = (h + 1) >> 1, r0 = y >> 1, r1 = (y & 1) ? min(r0 + 1, dh - 1) : max(r0 - 1, 0);
+  const uint8_t* p0 = p + (size_t)r0 * rs;
+  const uint8_t* p1 = p + (size_t)r1 * rs;
+  const int cs = 3 * p0[i] + p1[i], cn = 3 * p0[in_] + p1[in_];
+  if (odd) return i == dw - 1 ? (cs * 4 + 7) >> 4 : (3 * cs + cn + 7) >> 4;
+  return i == 0 ? (cs * 4 + 8) >> 4 : (3 * cs + cn + 8) >> 4;
+}
+
+__global__ void __launch_bounds__(256) jpeg_color_kernel(const int32_t* __restrict__ blocks, const uint8_t* __restrict__ ws,
+                                                         uint8_t* __restrict__ y_out, int H, int W, JpegWs L) {
+  const int s = blockIdx.y;
+  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const Geom g = geom(blk, H, W, L.slot);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= g.h * g.w) return;
+  const int x = i % g.w, y = i / g.w;
+  const uint8_t* pl = ws + (size_t)s * L.stride + L.planes;
+  const int Y = pl[g.poff[0] + (size_t)y * g.bw[0] * 8 + x];
+  uint8_t* o = y_out + (size_t)s * L.slot + (size_t)i * 3;
+  if (g.ncomp == 1) {
+    o[0] = o[1] = o[2] = (uint8_t)Y;
+    return;
+  }
+  const int rs = g.bw[1] * 8;
+  const int cb = upsample(pl + g.poff[1], rs, x, y, g.h, g.w, g.hs, g.vs) - 128;
+  const int cr = upsample(pl + g.poff[2], rs, x, y, g.h, g.w, g.hs, g.vs) - 128;
+  // jdcolor.c: FIX(1.40200) = 91881, FIX(1.77200) = 116130, FIX(0.71414) = 46802, FIX(0.34414) = 22554, SCALEBITS 16
+  const int R = Y + ((91881 * cr + 32768) >> 16);
+  const int G = Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
+  const int B = Y + ((116130 * cb + 32768) >> 16);
+  o[0] = (uint8_t)min(max(R, 0), 255);
+  o[1] = (uint8_t)min(max(G, 0), 255);
+  o[2] = (uint8_t)min(max(B, 0), 255);
+}
+
+}  // namespace
+
+size_t jpeg_workspace_bytes(int H, int W, int n) { return jpeg_ws(H, W).stride * (size_t)n; }
+
+int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
+                       cudaStream_t st) {
+  const JpegWs L = jpeg_ws(H, W);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  prefer_max_smem(jpeg_entropy_kernel);
+  jpeg_entropy_kernel<<<n, JT, 0, st>>>(files, blocks, ws, H, W, L);
+  prefer_max_smem(jpeg_idct_kernel);
+  jpeg_idct_kernel<<<dim3((unsigned)((L.blocks_cap + IDCT_BLOCKS - 1) / IDCT_BLOCKS), (unsigned)n), IDCT_BLOCKS * 8, 0, st>>>(
+      blocks, ws, H, W, L);
+  prefer_max_smem(jpeg_color_kernel);
+  jpeg_color_kernel<<<dim3((unsigned)(((size_t)H * W + 255) / 256), (unsigned)n), 256, 0, st>>>(blocks, ws, y, H, W, L);
+  DEFER_CUDA(cudaGetLastError());
+  return DEFER_OK;
+}
+
+}  // namespace defer
+
+using namespace defer;
+
+extern "C" {
+
+int defer_k_jpeg_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* coef_off,
+                           uint64_t* plane_off) {
+  DEFER_CHECK(H >= 1 && W >= 1 && n >= 1 && (uint64_t)H * W * 3 * 8 < (1ull << 31),
+              "k_jpeg_workspace: bad bound %dx%d (n %d)", H, W, n);
+  const JpegWs L = jpeg_ws(H, W);
+  if (bytes) *bytes = L.stride * (uint64_t)n;
+  if (sample_stride) *sample_stride = L.stride;
+  if (coef_off) *coef_off = L.coef;
+  if (plane_off) *plane_off = L.planes;
+  return DEFER_OK;
+}
+
+int defer_k_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
+                        void* stream) {
+  DEFER_CHECK(files && blocks && workspace && y, "k_jpeg_decode: null pointer");
+  DEFER_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && (uint64_t)H * W * 3 * 8 < (1ull << 31),
+              "k_jpeg_decode: bad sizes (n %d, bound %dx%d)", n, H, W);
+  DEFER_CHECK(((uintptr_t)blocks & 3) == 0 && ((uintptr_t)workspace & 255) == 0,
+              "k_jpeg_decode: blocks must be 4-byte and the workspace 256-byte aligned");
+  return launch_jpeg_decode(files, blocks, n, H, W, workspace, y, (cudaStream_t)stream);
+}
+
+}  // extern "C"

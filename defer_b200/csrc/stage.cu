@@ -118,6 +118,8 @@ struct Lane {
   bool timed = false;
   void* peer_out = nullptr;   // HOP_COPY: this lane's input slot on the consumer GPU (destination of the hop copy)
   int32_t* tables = nullptr;  // DEFER_RESIZE_SAMPLE_*: `batch` table blocks, next to the lane's input slot in the arena
+  int32_t* jpeg_blocks = nullptr;  // DEFER_OP_JPEG_DECODE: `batch` JPEG blocks, after the table blocks
+  void* jpeg_ws = nullptr;         // ... and its decode workspace (coefficients, planes, sync state)
   // the microbatch the lane ran last (last stage: the one out_host is filled with); result() refuses any other
   bool stepped = false;
   uint64_t last_seq = 0;
@@ -180,6 +182,12 @@ struct defer_stage_s {
     size_t block_ints = 0;        // int32 values per sample block
     size_t tables_off = 0;        // offset of a lane's blocks from its input slot
   } frames;
+  // JPEG files at ingress: the DEFER_OP_JPEG_DECODE op (-1 = none) in front of the per-sample resize pair
+  struct Jpeg {
+    int op = -1;
+    size_t blocks_off = 0;        // offset of a lane's JPEG blocks from its input slot
+    size_t ws_bytes = 0;          // decode workspace per lane
+  } jpeg;
 
   uint32_t* ctrl_u32(size_t off) { return reinterpret_cast<uint32_t*>(arena + off); }
   uint32_t* ready_flag(int d) { return ctrl_u32(OFF_READY + d * FLAG_STRIDE); }
@@ -191,7 +199,7 @@ struct defer_stage_s {
 namespace defer {
 
 static size_t elem_bytes(int elem, int fmt) {
-  return elem == DEFER_BUF_U8 ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
+  return elem == DEFER_BUF_U8 || elem == DEFER_BUF_JPEG ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
 }
 
 static size_t buf_bytes(const Buf& b, int fmt) { return b.elems * elem_bytes(b.elem, fmt); }
@@ -274,6 +282,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       if (op.folded_into >= 0) return DEFER_OK;   // applied by the stem conv as it reads the image
       if (d.mode == DEFER_PRE_TF) return launch_preprocess_tf((const uint8_t*)x, (float*)y, (size_t)nb * bi.h * bi.w, st);
       return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
+    case DEFER_OP_JPEG_DECODE:
+      return launch_jpeg_decode((const uint8_t*)x, L.jpeg_blocks, nb, bi.h, bi.w, L.jpeg_ws, (uint8_t*)y, st);
     case DEFER_OP_RESIZE:
       if (d.mode != 0) {
         const auto& f = s->frames;
@@ -369,6 +379,12 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
       op.alg_bytes = in_b + out_b + (double)s->weight_bytes[d.w_scale] + (double)s->weight_bytes[d.w_kernel];
       op.alg_flops = 2.0 * nb * bo.h * bo.w * bo.c * d.kw;
       break;
+    case DEFER_OP_JPEG_DECODE: {   // an upper bound: compressed slot + int16 coefficients + planes + image, at the slot's size
+      const double blocks_cap = 3.0 * ((bi.h + 15) / 16 * 2) * ((bi.w + 15) / 16 * 2);
+      op.alg_bytes = in_b + nb * blocks_cap * (128.0 + 64.0) + out_b;
+      op.alg_flops = 0;
+      break;
+    }
     default:
       op.alg_bytes = in_b + out_b;
       op.alg_flops = 0;
@@ -446,17 +462,25 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
   for (int i = 0; i < n_bufs; ++i) {
     Buf b;
     b.h = bufs[i].h; b.w = bufs[i].w; b.c = bufs[i].c; b.elem = bufs[i].elem;
-    if (b.h < 1 || b.w < 1 || b.c < 1 || (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8)) {
+    if (b.h < 1 || b.w < 1 || b.c < 1 ||
+        (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8 && b.elem != DEFER_BUF_JPEG)) {
       set_error("buffer %d: bad descriptor (%d,%d,%d,elem %d)", i, b.h, b.w, b.c, b.elem);
       return fail(DEFER_ERR_INVALID);
     }
     if (b.elem == DEFER_BUF_U8) {   // the first stage's image, or that image resized
       bool resized = false;
-      for (int j = 0; j < n_ops; ++j) resized |= ops[j].out == i && ops[j].kind == DEFER_OP_RESIZE;
+      for (int j = 0; j < n_ops; ++j)
+        resized |= ops[j].out == i && (ops[j].kind == DEFER_OP_RESIZE || ops[j].kind == DEFER_OP_JPEG_DECODE);
       if (!cfg->is_first || (i != cfg->input_buf && !resized)) {
-        set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE op", i);
+        set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE or "
+                  "JPEG_DECODE op", i);
         return fail(DEFER_ERR_INVALID);
       }
+    }
+    if (b.elem == DEFER_BUF_JPEG && (!cfg->is_first || i != cfg->input_buf || b.c != 3 ||
+                                     (uint64_t)b.h * b.w * 3 * 8 >= (1ull << 31))) {
+      set_error("buffer %d: a JPEG buffer is legal only as the first stage's input buffer, (H, W, 3) with H * W * 24 < 2^31", i);
+      return fail(DEFER_ERR_INVALID);
     }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;
     b.bytes = buf_bytes(b, cfg->fmt);
@@ -524,6 +548,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     if ((bi.elem == DEFER_BUF_U8 && d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE) ||
         (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_U8)) {
       set_error("op %d: only a RESIZE or PREPROCESS op may read a U8 buffer (as in0)", i);
+      return fail(DEFER_ERR_INVALID);
+    }
+    if ((bi.elem == DEFER_BUF_JPEG) != (d.kind == DEFER_OP_JPEG_DECODE) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_JPEG)) {
+      set_error("op %d: a JPEG buffer is read only by a JPEG_DECODE op (as in0), which reads nothing else", i);
       return fail(DEFER_ERR_INVALID);
     }
     if (d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE && d.mode != 0) {
@@ -660,7 +688,8 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
             set_error("op %d (resize, per sample): takes no weights, in1 or flags (its tables come with each microbatch)", i);
             return fail(DEFER_ERR_INVALID);
           }
-          if (horiz ? (d.in0 != cfg->input_buf || bo.h != bi.h || f.op_w >= 0) : (bo.w != bi.w || f.op_h >= 0)) {
+          const bool from_input = d.in0 == cfg->input_buf || (s->jpeg.op >= 0 && d.in0 == ops[s->jpeg.op].out);
+          if (horiz ? (!from_input || bo.h != bi.h || f.op_w >= 0) : (bo.w != bi.w || f.op_h >= 0)) {
             set_error("op %d (resize, per sample): SAMPLE_W maps the stage input (H, W) to (H, W_out), SAMPLE_H maps (H, W_out) "
                       "to (H_out, W_out), one of each per stage (got %dx%d -> %dx%d, mode %d)", i, bi.h, bi.w, bo.h, bo.w, d.mode);
             return fail(DEFER_ERR_INVALID);
@@ -710,6 +739,17 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         }
         break;
       }
+      case DEFER_OP_JPEG_DECODE:
+        op.kname = "jpeg_entropy_kernel+jpeg_idct_kernel+jpeg_color_kernel";
+        op.n_kernels = 3;
+        if (d.in0 != cfg->input_buf || bo.elem != DEFER_BUF_U8 || bo.h != bi.h || bo.w != bi.w || bo.c != 3 || d.in1 >= 0 ||
+            d.flags || d.mode || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0 || s->jpeg.op >= 0) {
+          set_error("op %d (jpeg decode): maps the stage's JPEG input (H, W, 3) to a U8 (H, W, 3) buffer, once, with no weights, "
+                    "in1, flags or mode", i);
+          return fail(DEFER_ERR_INVALID);
+        }
+        s->jpeg.op = i;
+        break;
       default:
         set_error("op %d: unknown kind %d", i, d.kind);
         return fail(DEFER_ERR_INVALID);
@@ -729,6 +769,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       return fail(DEFER_ERR_INVALID);
     }
     f.block_ints = 2 + (size_t)f.W_out * (2 + f.kw_w) + (size_t)f.H_out * (2 + f.kw_h);
+  }
+  if (s->jpeg.op >= 0 && (s->frames.op_w < 0 || ops[s->frames.op_w].in0 != ops[s->jpeg.op].out)) {
+    set_error("the JPEG_DECODE op (op %d) feeds the per-sample resize pair: its output is SAMPLE_W's input", s->jpeg.op);
+    return fail(DEFER_ERR_INVALID);
   }
   for (int i = 0; i < n_ops; ++i)
     if (ops[i].in0 == cfg->input_buf || ops[i].in1 == cfg->input_buf) s->last_input_reader = i;
@@ -774,6 +818,11 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     s->frames.tables_off = s->slot_stride;
     s->slot_stride += ((size_t)cfg->batch * s->frames.block_ints * 4 + 1023) / 1024 * 1024;
   }
+  if (s->jpeg.op >= 0) {       // then the JPEG blocks (zeroed with the arena too)
+    s->jpeg.blocks_off = s->slot_stride;
+    s->slot_stride += ((size_t)cfg->batch * DEFER_JPEG_BLOCK_INTS * 4 + 1023) / 1024 * 1024;
+    s->jpeg.ws_bytes = jpeg_workspace_bytes(s->bufs[cfg->input_buf].h, s->bufs[cfg->input_buf].w, cfg->batch);
+  }
   s->arena_bytes = CTRL_BYTES + s->slot_stride * cfg->depth;
   if (cudaMalloc((void**)&s->arena, s->arena_bytes) != cudaSuccess) {
     set_error("cudaMalloc arena (%zu bytes) failed", s->arena_bytes);
@@ -798,6 +847,14 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     L.buf.assign(n_bufs, nullptr);
     L.buf[cfg->input_buf] = s->arena + CTRL_BYTES + s->slot_stride * l;
     if (s->frames.op_w >= 0) L.tables = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->frames.tables_off);
+    if (s->jpeg.op >= 0) {
+      L.jpeg_blocks = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->jpeg.blocks_off);
+      if (cudaMalloc(&L.jpeg_ws, s->jpeg.ws_bytes) != cudaSuccess) {
+        set_error("cudaMalloc JPEG decode workspace (%zu bytes) failed", s->jpeg.ws_bytes);
+        return fail(DEFER_ERR_CUDA);
+      }
+      s->workspace.push_back(L.jpeg_ws);
+    }
     for (int b = 0; b < n_bufs; ++b) {
       if (b == cfg->input_buf) continue;
       if (b == cfg->output_buf && !cfg->is_last && s->hop != HOP_COPY) continue;  // bound to the consumer's slot at link time
@@ -1242,6 +1299,7 @@ int defer_stage_finalize(defer_stage_t s) {
 int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit: null");
   DEFER_CHECK(s->cfg.is_first, "submit: only the first stage takes host input");
+  DEFER_CHECK(s->jpeg.op < 0, "submit: this stage takes JPEG files (defer_stage_submit_jpegs)");
   DEFER_CHECK(s->frames.op_w < 0, "submit: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   DEFER_CHECK(nbytes == b.bytes, "submit: got %llu bytes, stage input is %zu", (unsigned long long)nbytes, b.bytes);
@@ -1254,6 +1312,7 @@ int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint6
 int defer_stage_submit_part(defer_stage_t s, uint64_t seq, int index, int count, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit_part: null");
   DEFER_CHECK(s->cfg.is_first, "submit_part: only the first stage takes host input");
+  DEFER_CHECK(s->jpeg.op < 0, "submit_part: this stage takes JPEG files (defer_stage_submit_jpegs)");
   DEFER_CHECK(s->frames.op_w < 0, "submit_part: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;       // first-stage input is plain fp32 NHWC: samples are contiguous
@@ -1272,6 +1331,7 @@ int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_index, int
                              const void* const* host_ptrs, uint64_t nbytes_per_item) {
   DEFER_CHECK(s && host_ptrs && n_items >= 1 && samples_per_item >= 1, "submit_parts: bad arguments");
   DEFER_CHECK(s->cfg.is_first, "submit_parts: only the first stage takes host input");
+  DEFER_CHECK(s->jpeg.op < 0, "submit_parts: this stage takes JPEG files (defer_stage_submit_jpegs)");
   DEFER_CHECK(s->frames.op_w < 0, "submit_parts: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;
@@ -1296,6 +1356,7 @@ int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, in
   DEFER_CHECK(s->cfg.is_first, "submit_frames: only the first stage takes host input");
   const auto& f = s->frames;
   DEFER_CHECK(f.op_w >= 0, "submit_frames: the stage takes one image size (no DEFER_RESIZE_SAMPLE_* ops); use defer_stage_submit*");
+  DEFER_CHECK(s->jpeg.op < 0, "submit_frames: this stage takes JPEG files (defer_stage_submit_jpegs)");
   DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_frames: samples [%d, %d) outside the microbatch of %d",
               first_index, first_index + n, s->cfg.batch);
   DEFER_CHECK(table_bytes == (uint64_t)n * f.block_ints * 4, "submit_frames: got %llu table bytes, %d blocks are %zu",
@@ -1317,6 +1378,44 @@ int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, in
     DEFER_CUDA(cudaMemcpyAsync(slot + (size_t)(first_index + i) * sample, images[i], (size_t)hw[2 * i] * hw[2 * i + 1] * 3,
                                cudaMemcpyHostToDevice, L.stream));
   DEFER_CUDA(cudaMemcpyAsync(L.tables + (size_t)first_index * f.block_ints, tables, table_bytes, cudaMemcpyHostToDevice, L.stream));
+  return DEFER_OK;
+}
+
+int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                             const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes) {
+  DEFER_CHECK(s && data && nbytes && blocks && n >= 1, "submit_jpegs: bad arguments");
+  DEFER_CHECK(s->cfg.is_first, "submit_jpegs: only the first stage takes host input");
+  DEFER_CHECK(s->jpeg.op >= 0, "submit_jpegs: the stage has no DEFER_OP_JPEG_DECODE op");
+  const auto& f = s->frames;
+  DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_jpegs: samples [%d, %d) outside the microbatch of %d",
+              first_index, first_index + n, s->cfg.batch);
+  const size_t per = f.block_ints + DEFER_JPEG_BLOCK_INTS;     // one file's resize block, then its JPEG block
+  DEFER_CHECK(block_bytes == (uint64_t)n * per * 4, "submit_jpegs: got %llu block bytes, %d files take %zu",
+              (unsigned long long)block_bytes, n, (size_t)n * per * 4);
+  const uint64_t slot = (uint64_t)f.H * f.W * 3;
+  for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
+    const int32_t* rb = blocks + (size_t)i * per;
+    const int32_t* jb = rb + f.block_ints;
+    DEFER_CHECK(data[i], "submit_jpegs: file %d is null", i);
+    DEFER_CHECK(nbytes[i] >= 4 && nbytes[i] <= slot, "submit_jpegs: file %d has %llu bytes, the slot takes 4..%llu", i,
+                (unsigned long long)nbytes[i], (unsigned long long)slot);
+    DEFER_CHECK(jb[0] >= 1 && jb[0] <= f.H && jb[1] >= 1 && jb[1] <= f.W, "submit_jpegs: file %d is %dx%d, the slot takes 1..%d x "
+                "1..%d", i, jb[0], jb[1], f.H, f.W);
+    DEFER_CHECK(rb[0] == jb[0] && rb[1] == jb[1], "submit_jpegs: resize block %d is for %dx%d, JPEG block %d for %dx%d", i, rb[0],
+                rb[1], i, jb[0], jb[1]);
+    DEFER_CHECK(jb[6] >= 0 && jb[7] >= 0 && (uint64_t)jb[6] + (uint64_t)jb[7] <= nbytes[i],
+                "submit_jpegs: file %d: entropy data [%d, %d + %d) outside its %llu bytes", i, jb[6], jb[6], jb[7],
+                (unsigned long long)nbytes[i]);
+  }
+  DEFER_TRY(set_device(s));
+  Lane& L = s->lanes[seq % s->cfg.depth];
+  uint8_t* dst = (uint8_t*)L.buf[s->cfg.input_buf];
+  for (int i = 0; i < n; ++i)   // the file's own bytes only, at the start of its sample slot
+    DEFER_CUDA(cudaMemcpyAsync(dst + (size_t)(first_index + i) * slot, data[i], nbytes[i], cudaMemcpyHostToDevice, L.stream));
+  DEFER_CUDA(cudaMemcpy2DAsync(L.tables + (size_t)first_index * f.block_ints, f.block_ints * 4, blocks, per * 4,
+                               f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
+  DEFER_CUDA(cudaMemcpy2DAsync(L.jpeg_blocks + (size_t)first_index * DEFER_JPEG_BLOCK_INTS, DEFER_JPEG_BLOCK_INTS * 4,
+                               blocks + f.block_ints, per * 4, DEFER_JPEG_BLOCK_INTS * 4, n, cudaMemcpyHostToDevice, L.stream));
   return DEFER_OK;
 }
 
@@ -1493,7 +1592,7 @@ int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_o
                 op.aff_op, buf_id);
   }
   DEFER_CUDA(cudaStreamSynchronize(s->lanes[lane].stream));
-  if (b.elem == DEFER_BUF_U8) {
+  if (b.elem == DEFER_BUF_U8 || b.elem == DEFER_BUF_JPEG) {
     std::vector<uint8_t> raw(b.elems);
     DEFER_CUDA(cudaMemcpy(raw.data(), src, b.elems, cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < b.elems; ++i) host_out[i] = (float)raw[i];

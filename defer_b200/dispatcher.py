@@ -14,7 +14,7 @@ What changed underneath:
 
 Non-reference additions: ``close()`` / context manager (the reference can only be killed), keyword-only
 ``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1),
-``coalesce``, ``preprocess``, ``image_size``, ``max_image_size`` and ``interpolation``.
+``coalesce``, ``preprocess``, ``image_size``, ``max_image_size``, ``interpolation`` and ``decode``.
 
 Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the host before every ``input_q.put``
 (``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
@@ -32,6 +32,9 @@ first stage resizes them to the model input on its GPU before preprocessing, bit
 resize then.  Photos and frames from several cameras come in many sizes: with ``max_image_size=(H, W)`` instead, each
 queue item is a uint8 image ``(batch, h, w, 3)`` of its own size with ``h <= H`` and ``w <= W``, items of different sizes
 share a microbatch, and each gives exactly what ``image_size=(h, w)`` would.  Only the image's own bytes cross PCIe.
+With ``decode="jpeg"`` as well, each queue item is a baseline JPEG file (``open(path, "rb").read()``); the first GPU
+decodes it exactly as ``load_img`` does with Pillow (``jpeg.decode_jpeg``), so only the compressed file crosses PCIe
+and the host only parses its markers.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -51,6 +54,7 @@ import numpy as np
 
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
+from .jpeg import check_decode, check_jpeg
 from .resize import check_frame, check_interpolation, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
@@ -61,7 +65,10 @@ class DEFER:
                  coalesce: int = 1, linger_us: float = 200.0, conv_backend: int = 0, dist=None,
                  wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None,
                  image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
-                 max_image_size: Optional[Tuple[int, int]] = None) -> None:
+                 max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None) -> None:
+        check_decode(decode, preprocess, image_size, max_image_size)
+        if decode is not None and batch not in (None, 1):
+            raise ValueError(f"decode={decode!r}: a queue item is one JPEG file, so batch must be 1, got {batch}")
         if preprocess is not None:
             check_preprocess(preprocess)
         check_interpolation(interpolation)
@@ -83,6 +90,7 @@ class DEFER:
         self.image_size = image_size        # None | (h, w) of the uint8 queue items, resized on stage 0's GPU
         self.interpolation = interpolation
         self.max_image_size = max_image_size  # None | (H, W): uint8 queue items of any size up to it, resized on stage 0
+        self.decode = decode                # None | "jpeg": queue items are JPEG files, decoded on stage 0
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -145,7 +153,8 @@ class DEFER:
                                          "preprocess": self.preprocess if i == 0 else None,
                                          "image_size": self.image_size if i == 0 else None,
                                          "interpolation": self.interpolation,
-                                         "max_image_size": self.max_image_size if i == 0 else None})
+                                         "max_image_size": self.max_image_size if i == 0 else None,
+                                         "decode": self.decode if i == 0 else None})
             self.dist.wait_all_ready()      # the 1-byte ACK of dispatcher.py:64-65
             return
         runners = []
@@ -159,7 +168,8 @@ class DEFER:
                                       preprocess=self.preprocess if i == 0 else None,
                                       image_size=self.image_size if i == 0 else None,
                                       interpolation=self.interpolation,
-                                      max_image_size=self.max_image_size if i == 0 else None)
+                                      max_image_size=self.max_image_size if i == 0 else None,
+                                      decode=self.decode if i == 0 else None)
             r.name = f"part{i+1}"
             runners.append(r)
         for i in range(n - 1):              # next hop = nodeIPs[i+1] (dispatcher.py:51-55)
@@ -184,6 +194,10 @@ class DEFER:
         if bound is not None:                # each image with its own size and tables, one C call per group
             def submit_items(seq, group):
                 first.submit_frames(seq, 0, group)
+        jpeg = self.decode == "jpeg"
+        if jpeg:                             # the files, parsed here, decoded on the GPU
+            def submit_items(seq, group):
+                first.submit_jpegs(seq, 0, [d for d, _ in group], [i for _, i in group])
         try:
             while not self._stop.is_set():
                 try:
@@ -200,7 +214,9 @@ class DEFER:
                 in_shape = None
                 while True:
                     x = model_input
-                    if bound is not None:            # any size up to the bound: no same-shape rule within a group
+                    if jpeg:                         # (file bytes, header): refused files raise here, as bad items do
+                        x = check_jpeg(x, bound)
+                    elif bound is not None:          # any size up to the bound: no same-shape rule within a group
                         x = check_frame(x, bound)
                     elif u8:
                         if not (isinstance(x, np.ndarray) and x.dtype == np.uint8):
@@ -210,11 +226,13 @@ class DEFER:
                         x = np.ascontiguousarray(x)
                     elif not (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]):
                         x = np.ascontiguousarray(x, dtype=np.float32)
-                    if x.shape[0] != B:
+                    if not jpeg and x.shape[0] != B:
                         raise ValueError(f"queue item has batch {x.shape[0]}, DEFER was built for batch {B}")
-                    if bound is None and in_shape is None:
+                    if jpeg or bound is not None:
+                        pass
+                    elif in_shape is None:
                         in_shape = x.shape
-                    elif bound is None and x.shape != in_shape:
+                    elif x.shape != in_shape:
                         raise ValueError(f"queue items of one group differ in shape: {x.shape} vs {in_shape}")
                     hold[self.items_submitted % nh] = x      # keep alive until the DMA has certainly happened
                     self.items_submitted += 1

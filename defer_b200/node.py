@@ -24,6 +24,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .node_state import NodeState
 from .planner import Plan, plan_stage
+from .jpeg import check_jpeg, pack_block
 from .resize import check_frame, pack_frame_tables
 
 DTYPE_TO_FMT = {
@@ -84,6 +85,7 @@ class StageRunner:
         self.resizes = any(o.kind == A.OP_RESIZE for o in plan.ops)
         # planned with max_image_size=: images of mixed sizes, fed by submit_frames with their table blocks
         self.frames = plan.frames
+        self.decode = plan.decode                    # "jpeg": fed by submit_jpegs, files with their JPEG blocks
         self._tables: Dict[int, tuple] = {}          # per lane: blocks, sizes and images of its latest microbatch (kept alive)
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
@@ -114,15 +116,19 @@ class StageRunner:
     def from_model(cls, model: K.Model, device=0, dtype: str = "float32", max_batch: int = 1, depth: int = 1,
                    is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
                    image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
-                   max_image_size: Optional[Tuple[int, int]] = None, **kw) -> "StageRunner":
+                   max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
+                   **kw) -> "StageRunner":
         """``preprocess="caffe"`` or ``"tf"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the
         stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family).
         ``image_size=(h, w)`` (with ``preprocess``): inputs are uint8 RGB images of that size, resized on the GPU to the
         model's input as Keras' ``load_img(target_size=..., interpolation=...)`` does (``resize.resize_image``).
         ``max_image_size=(H, W)`` (with ``preprocess``, instead of ``image_size``): the same for images of any size up to
-        ``(H, W)``, each resized from its own size; feed them with ``submit_frames`` / ``predict_frames``."""
+        ``(H, W)``, each resized from its own size; feed them with ``submit_frames`` / ``predict_frames``.
+        ``decode="jpeg"`` (with ``preprocess`` and ``max_image_size``): inputs are baseline JPEG files of images up to
+        ``(H, W)``, decoded on the GPU as Keras' ``load_img`` does (``jpeg.decode_jpeg``); feed them with
+        ``submit_jpegs`` / ``predict_jpegs``."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
-                          interpolation=interpolation, max_image_size=max_image_size)
+                          interpolation=interpolation, max_image_size=max_image_size, decode=decode)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
                 is_last=is_last, name=model.name, **kw)
@@ -223,6 +229,8 @@ class StageRunner:
         bytes and then the blocks.  Same lifetime rule as ``submit``."""
         if self.frames is None:
             raise ValueError(f"{self.name}: submit_frames needs a stage planned with max_image_size=")
+        if self.decode is not None:
+            raise ValueError(f"{self.name}: this stage takes JPEG files; feed them with submit_jpegs / predict_jpegs")
         bound = self.frames["max_image_size"]
         images = []
         for x in frames:
@@ -245,6 +253,37 @@ class StageRunner:
         self.step(0)
         n = sum(1 if np.ndim(x) == 3 else len(x) for x in frames)
         return self.result(0)[:n]
+
+    def submit_jpegs(self, seq: int, index: int, items, infos=None) -> None:
+        """Ingress of a ``decode="jpeg"`` stage: ``items`` is a list of JPEG files (``bytes``, ``bytearray``,
+        ``memoryview`` or 1-D uint8 arrays), one image each, of sizes up to ``max_image_size``; they go to samples
+        ``[index, index + len(items))`` of microbatch ``seq``, each with its resize and JPEG blocks.  The files' markers are
+        parsed here (``jpeg.check_jpeg``: a refused file raises a ValueError and nothing is copied); one C call copies each
+        file's own bytes and then the blocks.  ``infos``: the items' ``jpeg.check_jpeg`` headers when the caller has
+        already checked them (the items are then ``bytes``).  Same lifetime rule as ``submit``."""
+        if self.decode != "jpeg":
+            raise ValueError(f"{self.name}: submit_jpegs needs a stage planned with decode='jpeg'")
+        bound = self.frames["max_image_size"]
+        if infos is None:
+            items, infos = zip(*[check_jpeg(x, bound) for x in items]) if items else ((), ())
+        files = items
+        n = len(files)
+        if not 1 <= n <= self.batch - index or index < 0:
+            raise ValueError(f"{self.name}: {n} files from sample {index} do not fit the microbatch of {self.batch}")
+        hw = np.array([(i.h, i.w) for i in infos], np.int32).reshape(n, 2)
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"])
+        blocks = np.concatenate([tables, np.stack([pack_block(i) for i in infos])], axis=1)
+        sizes = np.array([len(f) for f in files], np.uint64)
+        self._tables[seq % self.depth] = (blocks, sizes, files)
+        ptrs = (C.c_void_p * n)(*[C.cast(C.c_char_p(f), C.c_void_p).value for f in files])
+        A.check(self.lib.defer_stage_submit_jpegs(self.handle, seq, index, n, ptrs, sizes.ctypes.data, blocks.ctypes.data,
+                                                  blocks.nbytes))
+
+    def predict_jpegs(self, items) -> np.ndarray:
+        """Single-stage ``model.predict`` of a ``decode="jpeg"`` stage: the outputs of the JPEG files ``items``, in order."""
+        self.submit_jpegs(0, 0, items)
+        self.step(0)
+        return self.result(0)[:len(items)]
 
     def step(self, seq: int) -> None:
         A.check(self.lib.defer_stage_step(self.handle, seq))
@@ -429,7 +468,8 @@ class Node:
                                        preprocess=msg.get("preprocess") if rank == 0 else None,
                                        image_size=msg.get("image_size") if rank == 0 else None,
                                        interpolation=msg.get("interpolation", "nearest"),
-                                       max_image_size=msg.get("max_image_size") if rank == 0 else None)
+                                       max_image_size=msg.get("max_image_size") if rank == 0 else None,
+                                       decode=msg.get("decode") if rank == 0 else None)
         ns.model = runner                               # src/node.py:38
         self.runner = runner
         # wire the hop: my consumer gives me its input-side token, I give it my output-side token

@@ -22,7 +22,9 @@ image of that size and up to two ``RESIZE`` ops (width, then height: Keras' ``lo
 tables from ``resize.resize_tables``) bring it to the model's input size before ``PREPROCESS``.
 With ``max_image_size=(H, W)`` instead, the stage input is a uint8 slot of that size per sample and two per-sample
 ``RESIZE`` ops (``RESIZE_SAMPLE_W``, then ``_H``) read each image's size and tables from a block that comes with it
-(``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.
+(``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.  With
+``decode="jpeg"`` as well, the stage input is a byte slot of ``H * W * 3`` per sample holding one JPEG file, and a
+``JPEG_DECODE`` op in front of the resize pair decodes it into the uint8 slot (``jpeg.pack_block``).
 """
 from __future__ import annotations
 
@@ -34,6 +36,7 @@ import numpy as np
 from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
+from .jpeg import check_decode
 from .resize import check_interpolation, check_size, kcap, resize_tables
 
 
@@ -79,6 +82,8 @@ class Plan:
     # max_image_size=: {"max_image_size": (H, W), "target": (H_out, W_out), "kw": (kw_w, kw_h), "interpolation": name},
     # what the stage's feeder needs to pack each image's table block (resize.pack_frame_tables); None otherwise
     frames: Optional[dict] = None
+    # decode="jpeg": the stage takes JPEG files (each with its jpeg.pack_block block after its table block); None otherwise
+    decode: Optional[str] = None
 
     def describe(self) -> str:
         lines = []
@@ -99,7 +104,8 @@ def _hwc(shape) -> Tuple[int, int, int]:
 
 def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None,
                image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
-               max_image_size: Optional[Tuple[int, int]] = None) -> Plan:
+               max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None) -> Plan:
+    check_decode(decode, preprocess, image_size, max_image_size)
     if preprocess is not None:
         check_preprocess(preprocess)
         if not is_first:
@@ -216,7 +222,11 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         H, W, _ = _hwc(shapes[in_name])
         h, w = image_size or max_image_size or (H, W)
         input_shape = (h, w, 3)
-        input_buf = img = new_buf((None,) + input_shape, A.BUF_U8)
+        input_buf = img = new_buf((None,) + input_shape, A.BUF_JPEG if decode else A.BUF_U8)
+        if decode is not None:
+            # the JPEG files decode into the image slot the per-sample resize reads (jpeg.pack_block per file)
+            img = emit(PlanOp(A.OP_JPEG_DECODE, img, new_buf((None,) + input_shape, A.BUF_U8),
+                              layers=[f"load_img(decode {decode} <={h}x{w})"])).out
         if max_image_size is not None:
             # images of mixed sizes up to (h, w): both passes always, the tables come with each image
             kw = (kcap(w, W, interpolation), kcap(h, H, interpolation))
@@ -410,4 +420,4 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
             op.w_shift = add_weight(op.shift.astype(np.float32))
     return Plan(bufs=bufs, ops=ops, weights=weights, input_buf=input_buf, output_buf=out_buf,
                 input_shape=input_shape, output_shape=tuple(shapes[out_name][1:]),
-                tensor_buf=dict(tensor_buf), frames=frames)
+                tensor_buf=dict(tensor_buf), frames=frames, decode=decode)

@@ -67,7 +67,7 @@ typedef enum defer_op_kind {
                          /* `mode` DEFER_PRE_CAFFE: w_shift = 3 fp32 values in output-channel order,            */
                          /*   y[..., c] = float(x[..., 2 - c]) + shift[c]  (RGB -> BGR, minus the ImageNet mean)  */
                          /* `mode` DEFER_PRE_TF: no weights, y = float(x) / 127.5 - 1 in fp32 (ResNet V2)       */
-  DEFER_OP_RESIZE = 12   /* Keras load_img(target_size=...) resize, one axis of Pillow's 8-bit resampling:       */
+  DEFER_OP_RESIZE = 12,  /* Keras load_img(target_size=...) resize, one axis of Pillow's 8-bit resampling:       */
                          /*   in0 = U8 (h_in, w_in, 3), out = U8 (h_out, w_out, 3), exactly one of h / w differs  */
                          /*   (that is the axis; `mode` 0).  Weights are int32 tables of that axis:               */
                          /*   w_scale  = [out_len, 2] (first, count): output i reads source [first, first + count) */
@@ -75,6 +75,9 @@ typedef enum defer_op_kind {
                          /*   y[i] = clamp((2^21 + sum_{k < count} x[first + k] * tap[k]) >> 22, 0, 255) per     */
                          /*   channel; 0 <= first, 1 <= count <= kw, first + count <= in_len (checked at create)  */
                          /* `mode` DEFER_RESIZE_SAMPLE_W / _H: images of mixed sizes, tables per sample (below)   */
+  DEFER_OP_JPEG_DECODE = 13 /* baseline JPEG files -> images (below): in0 = the stage input, a DEFER_BUF_JPEG (H, W, 3)    */
+                         /*   slot per sample; out = U8 (H, W, 3), each image packed (h, w, 3) at the start of its sample;  */
+                         /*   read by the DEFER_RESIZE_SAMPLE_W op.  No weights, mode 0.                                     */
 } defer_op_kind;
 
 /* defer_op_desc.mode of a DEFER_OP_RESIZE op.  0: the fixed-size resize above (one image size per stage).
@@ -93,6 +96,29 @@ typedef enum defer_op_kind {
 #define DEFER_RESIZE_SAMPLE_W 1
 #define DEFER_RESIZE_SAMPLE_H 2
 
+/* DEFER_OP_JPEG_DECODE decodes each sample's JPEG file on the GPU, bit for bit as libjpeg-turbo 3.1 does through Pillow
+ * (defer_b200/jpeg.py restates it).  It is planned before the DEFER_RESIZE_SAMPLE_W / _H pair, whose table blocks keep
+ * their layout.  The sample's file sits at the start of its H * W * 3-byte slot; its int32 block, written next to the
+ * slots by defer_stage_submit_jpegs after the resize blocks, is DEFER_JPEG_BLOCK_INTS values:
+ *   [0] h  [1] w  [2] components (1 | 3)  [3] luma h-sampling  [4] luma v-sampling (1x1, 2x1 or 2x2; chroma 1x1)
+ *   [5] restart interval in MCUs (0 = none)  [6] entropy-data offset in the file  [7] its length (up to EOI)
+ *   [8] MCUs across  [9] MCUs down  [10..15] 0
+ *   [16 + 64 c ...]  quantisation table of component c, natural order (c < 3)
+ *   [16 + 192 + t * DEFER_JPEG_HUFF_INTS ...]  Huffman table t = DC of component 0, 1, 2, then AC of component 0, 1, 2:
+ *        lookahead[2^DEFER_JPEG_LOOKAHEAD] (code length << 8 | symbol for codes of <= LOOKAHEAD bits, 0 otherwise),
+ *        maxcode[17] (largest code of each length, -1 if none), valoff[17] (symbol index - code), symbols[256]
+ * The decode never trusts the block: h / w are clamped into the slot, sampling into 4:4:4 / 4:2:2 / 4:2:0, the entropy
+ * extent into the slot and every table index into its table, so no block content makes it access memory outside the
+ * sample's slot, workspace or image.  The blocks are zeroed at create: a never-written sample decodes to a 1x1 image of
+ * value 128.  An invalid Huffman code ends the sample's decode (that block and all later ones are zero); the exact rule
+ * for corrupt data is defer_b200/jpeg.py's. */
+#define DEFER_JPEG_HDR_INTS 16
+#define DEFER_JPEG_LOOKAHEAD 9
+#define DEFER_JPEG_HUFF_INTS ((1 << DEFER_JPEG_LOOKAHEAD) + 17 + 17 + 256)
+#define DEFER_JPEG_BLOCK_INTS (DEFER_JPEG_HDR_INTS + 3 * 64 + 6 * DEFER_JPEG_HUFF_INTS)
+/* bits per subsequence of the self-synchronising Huffman decode */
+#define DEFER_JPEG_SUBSEQ_BITS 8192
+
 /* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
 #define DEFER_PRE_CAFFE 0   /* keras_applications imagenet_utils mode='caffe' (ResNet50/101/152, VGG16) */
 #define DEFER_PRE_TF    1   /* mode='tf' (ResNet50V2/101V2/152V2): fl32(fl32(x / 127.5) - 1), bit for bit */
@@ -105,11 +131,14 @@ typedef enum defer_op_kind {
 #define DEFER_BUF_F32 1   /* plain fp32 regardless of the stage format (image in, probabilities out) */
 #define DEFER_BUF_U8  2   /* uint8 NHWC, 1 B/elem, first stage only: its input buffer or the output of a DEFER_OP_RESIZE; */
                           /* read only by DEFER_OP_RESIZE and DEFER_OP_PREPROCESS                                          */
+                          /* (or of a DEFER_OP_JPEG_DECODE)                                                                */
+#define DEFER_BUF_JPEG 3  /* bytes of one JPEG file per sample, h * w * c of them: the first stage's input buffer only,   */
+                          /* read only by DEFER_OP_JPEG_DECODE                                                             */
 
 /* One logical tensor of the plan.  Shapes are per sample, NHWC; vectors use h = w = 1. */
 typedef struct defer_buf_desc {
   int32_t h, w, c;
-  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 */
+  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 | DEFER_BUF_JPEG */
 } defer_buf_desc;
 
 /* One fused op of the plan.  Buffer ids index the defer_buf_desc array; weight ids index the
@@ -203,6 +232,14 @@ DEFER_API int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_
  * defer_stage_submit / _part / _parts refuse such a stage. */
 DEFER_API int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* images,
                               const int32_t* hw /* [n][2] */, const int32_t* tables, uint64_t table_bytes);
+/* First stage with a DEFER_OP_JPEG_DECODE op: file i (nbytes[i] bytes at data[i], at most H * W * 3) goes to the start of
+ * sample slot first_index + i.  blocks holds, per file, its resize table block followed by its JPEG block
+ * (block_bytes = n x (resize block + DEFER_JPEG_BLOCK_INTS) x 4); the resize header (h, w) must equal the JPEG block's,
+ * with 1 <= h <= H, 1 <= w <= W, and the entropy extent must lie inside the file.  Everything is checked before anything
+ * is copied (DEFER_ERR_INVALID, nothing copied); then only each file's own bytes and the blocks are copied, on the lane's
+ * stream.  defer_stage_submit / _part / _parts / _frames refuse such a stage. */
+DEFER_API int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                             const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes);
 /* Enqueue microbatch `seq` on lane seq % depth: wait-input -> kernel chain -> hop -> flags. Async. */
 DEFER_API int defer_stage_step(defer_stage_t s, uint64_t seq);
 /* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host.  A lane keeps only the output
@@ -289,6 +326,17 @@ DEFER_API int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds
  * int32 blocks of the layout above (kw_w, kw_h taps), on the device, 4-byte aligned; c must be 3. */
 DEFER_API int defer_k_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W,
                                     int H_out, int W_out, int kw_w, int kw_h, int c, void* stream);
+
+/* The whole DEFER_OP_JPEG_DECODE of n samples: files = n slots of H * W * 3 bytes, blocks = n JPEG blocks (layout above,
+ * 4-byte aligned), y = n U8 (H, W, 3) images; workspace of defer_k_jpeg_workspace bytes, 256-byte aligned, caller-owned.
+ * Per sample (sample_stride apart) the workspace holds, from coef_off, the final quantised coefficients as int16 [blocks,
+ * 64] in stream order and natural coefficient order, and from plane_off the MCU-padded component planes (uint8, one after
+ * the other, each (8 * blocks down) x (8 * blocks across)).  Its first 5 int32 are the unstuffed entropy bytes, the RST
+ * markers found, the subsequences, the synchronisation rounds and the blocks before the first invalid code. */
+DEFER_API int defer_k_jpeg_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* coef_off,
+                                     uint64_t* plane_off);
+DEFER_API int defer_k_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace,
+                                  uint8_t* y, void* stream);
 
 #ifdef __cplusplus
 }
