@@ -202,6 +202,8 @@ int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* 
 // DEFER_OP_JPEG_DECODE (jpeg.cu): n JPEG files in H * W * 3-byte slots, with their blocks -> n U8 (H, W, 3) images, through a
 // workspace of jpeg_workspace_bytes(H, W, n) (256-byte aligned)
 size_t jpeg_workspace_bytes(int H, int W, int n);
+// the bounds (H, W) the decode takes: H * W * 24 + DEFER_JPEG_SUBSEQ_BITS < 2^31
+bool jpeg_bound_ok(int H, int W);
 int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
                        cudaStream_t st);
 

@@ -570,6 +570,9 @@ __global__ void __launch_bounds__(256) jpeg_color_kernel(const int32_t* __restri
 
 size_t jpeg_workspace_bytes(int H, int W, int n) { return jpeg_ws(H, W).stride * (size_t)n; }
 
+// Bit positions in the entropy kernel are ints: the last subsequence's end, up to slot * 8 + S_BITS, must fit in one
+bool jpeg_bound_ok(int H, int W) { return (uint64_t)H * W * 3 * 8 + S_BITS < (1ull << 31); }
+
 int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
                        cudaStream_t st) {
   const JpegWs L = jpeg_ws(H, W);
@@ -593,7 +596,7 @@ extern "C" {
 
 int defer_k_jpeg_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* coef_off,
                            uint64_t* plane_off) {
-  DEFER_CHECK(H >= 1 && W >= 1 && n >= 1 && (uint64_t)H * W * 3 * 8 < (1ull << 31),
+  DEFER_CHECK(H >= 1 && W >= 1 && n >= 1 && jpeg_bound_ok(H, W),
               "k_jpeg_workspace: bad bound %dx%d (n %d)", H, W, n);
   const JpegWs L = jpeg_ws(H, W);
   if (bytes) *bytes = L.stride * (uint64_t)n;
@@ -606,7 +609,7 @@ int defer_k_jpeg_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sampl
 int defer_k_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
                         void* stream) {
   DEFER_CHECK(files && blocks && workspace && y, "k_jpeg_decode: null pointer");
-  DEFER_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && (uint64_t)H * W * 3 * 8 < (1ull << 31),
+  DEFER_CHECK(n >= 1 && n <= 65535 && H >= 1 && W >= 1 && jpeg_bound_ok(H, W),
               "k_jpeg_decode: bad sizes (n %d, bound %dx%d)", n, H, W);
   DEFER_CHECK(((uintptr_t)blocks & 3) == 0 && ((uintptr_t)workspace & 255) == 0,
               "k_jpeg_decode: blocks must be 4-byte and the workspace 256-byte aligned");

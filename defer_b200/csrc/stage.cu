@@ -478,8 +478,9 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       }
     }
     if (b.elem == DEFER_BUF_JPEG && (!cfg->is_first || i != cfg->input_buf || b.c != 3 ||
-                                     (uint64_t)b.h * b.w * 3 * 8 >= (1ull << 31))) {
-      set_error("buffer %d: a JPEG buffer is legal only as the first stage's input buffer, (H, W, 3) with H * W * 24 < 2^31", i);
+                                     !jpeg_bound_ok(b.h, b.w))) {
+      set_error("buffer %d: a JPEG buffer is legal only as the first stage's input buffer, (H, W, 3) with "
+                "H * W * 24 + %d < 2^31", i, DEFER_JPEG_SUBSEQ_BITS);
       return fail(DEFER_ERR_INVALID);
     }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;

@@ -6,6 +6,12 @@ the host restatement that the GPU decode (``DEFER_OP_JPEG_DECODE``) is tested ag
 triangular upsampling, fixed-point YCbCr->RGB of ``jdcolor.c``).  Other libjpeg builds, IJG 9 among them, upsample
 differently and can give other pixels.
 
+That holds while every output of the IDCT stays within +-512 of 128, as it does for the blocks encoders write from 8-bit
+images.  Beyond that range the samples are defined by ``jidctint.c``: the output wraps to 10 bits before the clamp to
+0..255 (``idct_range_limit[x & 1023]``), so 128 + 1100 gives 204, not 255.  Only hand-made or corrupt files get there
+(large coefficients or quantisers), and there no single Pillow result exists: libjpeg-turbo's SIMD IDCT, which Pillow
+uses on x86, does not wrap, while a build without SIMD runs ``jidctint.c``.
+
 The feeder only walks the markers (``parse``) and decodes no Huffman code: past the scan header, byte searches find the
 EOI that ends the entropy-coded data.  Tables derived from DQT and DHT segments are memoised on the segment bytes,
 as a stream from one encoder repeats them.

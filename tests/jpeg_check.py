@@ -7,7 +7,10 @@ subsequence whose predecessor left in a state other than the one it entered re-d
 restarts a decoder one bit later at block 0, coefficient 0 (on the true path it is a real error, which the write pass
 finds).  Once no entry changes, each subsequence owns the blocks that start in it: a prefix sum gives their
 positions, and a last pass writes them (finishing a block past the subsequence's end, skipping the tail of one that
-started before it).  The result must equal ``jpeg.entropy_decode``; ``sync_decode`` also returns the rounds it took."""
+started before it).  The result must equal ``jpeg.entropy_decode``; ``sync_decode`` also returns the rounds it took, and
+``sync_stats`` the five counters the device writes to its ``stats``.  The rounds are deterministic (every pending
+subsequence of a round re-decodes from its predecessor's exit of the round before, as on the device), so all five
+counters must equal the device's exactly."""
 from __future__ import annotations
 
 import numpy as np
@@ -34,6 +37,14 @@ def _run(r, g, info, pos, j, k, end):
 
 def sync_decode(data, sbits: int):
     """(coef [blocks, 64] natural order with DC differences, decoded mask, rounds), as the device computes them."""
+    coef, decoded, stats = sync_stats(data, sbits)
+    return coef, decoded, int(stats[3])
+
+
+def sync_stats(data, sbits: int):
+    """(coef, decoded mask, stats): ``sync_decode``'s coefficients and mask, and int32 [5] of what the device writes to
+    ``stats[0..4]``: the unstuffed byte count T, the RST marker count R, the subsequence count, the rounds and the
+    cutoff (the first block whose decode met an invalid code, or the block count)."""
     info = jpeg.parse(data)
     g = jpeg.geometry(info.h, info.w, info.ncomp, info.hs, info.vs)
     comp, rst = jpeg.unstuff(data[info.offset:info.offset + info.length])
@@ -110,4 +121,4 @@ def sync_decode(data, sbits: int):
         decoded[first + min(seg_total[k], n):first + n] = False
     decoded[cutoff:] = False
     coef[~decoded] = 0
-    return coef, decoded, rounds
+    return coef, decoded, np.array([len(comp), len(rst), len(subs), rounds, cutoff], np.int32)

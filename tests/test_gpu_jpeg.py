@@ -1,12 +1,14 @@
 """JPEG files at ingress (`decode="jpeg"`) on the GPU, bit for bit against the host restatement.
 
-The contract: `defer_k_jpeg_decode` gives the coefficients, planes and RGB of `jpeg.decode_stages` byte for byte (on the
-committed fixtures, on a file with random entropy data and on a never-written sample); a `decode="jpeg"` stage equals the
+The contract: `defer_k_jpeg_decode` gives the coefficients, planes and RGB of `jpeg.decode_stages` byte for byte, and the
+five counters of the restatement in tests/jpeg_check.py (on the committed fixtures, on a file with random entropy data
+and on a never-written sample); a `decode="jpeg"` stage equals the
 `max_image_size` stage fed `decode_jpeg(item)`, in both preprocessing modes, dtypes and stem paths and after lane re-use;
 and `DEFER` over one and two stages returns what the `max_image_size` pipeline returns for the decoded images, in FIFO
 order, and surfaces a refused file as a ValueError.  The fixtures come from tools/make_jpeg_fixtures.py; no Pillow here."""
 import ctypes as C
 import queue
+import re
 import sys
 import threading
 from pathlib import Path
@@ -15,16 +17,19 @@ import numpy as np
 import pytest
 
 ROOT = Path(__file__).resolve().parents[1]
-if str(ROOT) not in sys.path:
-    sys.path.insert(0, str(ROOT))
+for _p in (ROOT, ROOT / "tests"):
+    if str(_p) not in sys.path:
+        sys.path.insert(0, str(_p))
 
 from defer_b200 import _cabi as A  # noqa: E402
 from defer_b200 import applications  # noqa: E402
 from defer_b200 import jpeg  # noqa: E402
+from jpeg_check import sync_stats  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1200)]
 
 GOLDEN = ROOT / "tests" / "golden" / "jpeg"
+SBITS = int(re.search(r"#define DEFER_JPEG_SUBSEQ_BITS (\d+)", (ROOT / "include" / "defer_b200.h").read_text()).group(1))
 
 
 def _bits(a):
@@ -50,9 +55,9 @@ def random_entropy(data, seed):
     return data[:info.offset] + junk.tobytes() + b"\xff\xd9"
 
 
-def _decode_dev(files, H, W):
-    """defer_k_jpeg_decode of ``files`` in slots of the bound (H, W): (coef, planes, rgb, stats) per file; a None file is
-    a never-written sample (zero slot, zero block)."""
+def _decode_dev(files, H, W, timed=False):
+    """defer_k_jpeg_decode of ``files`` in slots of the bound (H, W): (workspace, coef offset, plane offset, images); a
+    None file is a never-written sample (zero slot, zero block).  ``timed``: also the decode's time in ms (CUDA events)."""
     import torch
     lib = A.load()
     n = len(files)
@@ -69,14 +74,19 @@ def _decode_dev(files, H, W):
     x = torch.from_numpy(slots.reshape(-1)).cuda()
     b = torch.from_numpy(blocks.reshape(-1)).cuda()
     y = torch.full((n * slot,), 7, dtype=torch.uint8, device="cuda")
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]      # on the legacy default stream, as the decode
+    torch.cuda.synchronize()
+    ev[0].record(torch.cuda.default_stream())
     A.check(lib.defer_k_jpeg_decode(x.data_ptr(), b.data_ptr(), n, H, W, ws.data_ptr(), y.data_ptr(), None))
+    ev[1].record(torch.cuda.default_stream())
     torch.cuda.synchronize()
     ws = ws.cpu().numpy().reshape(n, stride.value)
     y = y.cpu().numpy().reshape(n, slot)
-    return ws, coef_off.value, plane_off.value, y
+    out = ws, coef_off.value, plane_off.value, y
+    return (out, ev[0].elapsed_time(ev[1])) if timed else out
 
 
-def _check_sample(ws, coef_off, plane_off, y, want, name):
+def _check_sample(ws, coef_off, plane_off, y, want, name, stats=None):
     info, g = want["info"], jpeg.geometry(want["info"].h, want["info"].w, want["info"].ncomp, want["info"].hs,
                                           want["info"].vs)
     coef = ws[coef_off:coef_off + g.blocks * 128].view(np.int16).reshape(g.blocks, 64)
@@ -87,9 +97,11 @@ def _check_sample(ws, coef_off, plane_off, y, want, name):
         assert np.array_equal(got, p), (name, c)
         off += p.size
     assert np.array_equal(y[:info.h * info.w * 3].reshape(info.h, info.w, 3), want["rgb"]), name
-    stats = ws[:20].view(np.int32)
-    assert 0 <= stats[4] <= g.blocks and not want["decoded"][stats[4]:].any(), name   # nothing after the cutoff
-    return stats
+    got = ws[:20].view(np.int32)
+    assert 0 <= got[4] <= g.blocks and not want["decoded"][got[4]:].any(), name   # nothing after the cutoff
+    if stats is not None:
+        assert np.array_equal(got, stats), (name, got.tolist(), stats.tolist())
+    return got
 
 
 def test_k_jpeg_decode_matches_host():
@@ -100,14 +112,12 @@ def test_k_jpeg_decode_matches_host():
          "photo_480x640_422_q90_rr1.jpg"])]
     names += ["random entropy"] * 4
     ws, coef_off, plane_off, y = _decode_dev(files + [None], 1080, 1920)
-    rounds = []
     for i, (nm, d) in enumerate(zip(names, files)):
-        stats = _check_sample(ws[i], coef_off, plane_off, y[i], jpeg.decode_stages(d), nm)
-        rounds.append(int(stats[3]))
+        # all five counters (unstuffed bytes, RST markers, subsequences, rounds, cutoff) equal the restatement's
+        _check_sample(ws[i], coef_off, plane_off, y[i], jpeg.decode_stages(d), nm, sync_stats(d, SBITS)[2])
     # a never-written sample: a 1x1 image of value 128, nothing else written
     assert np.array_equal(y[-1][:3], [128, 128, 128])
     assert (y[-1][3:] == 7).all()
-    print(f"sync rounds: max {max(rounds)}, mean {np.mean(rounds):.2f}")
 
 
 def test_k_jpeg_decode_refuses_bad_arguments():

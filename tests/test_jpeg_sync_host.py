@@ -1,6 +1,9 @@
 """The self-synchronising Huffman decode (tests/jpeg_check.py, as the GPU runs it) against the sequential decoder of
-`jpeg.entropy_decode`, for several subsequence sizes, with and without restart intervals, and on random entropy data; and
-its rounds at the device's subsequence size: a few, however long the file, so no thread decodes a whole file."""
+`jpeg.entropy_decode`, for several subsequence sizes, with and without restart intervals, on random entropy data and on
+the corrupt files of the GPU tests; and its rounds at the device's subsequence size on encoder-made files: a few, however
+long the file, so no thread decodes a whole file.  That bound holds for what encoders write, not for every valid file:
+on a file whose every bit position decodes, the rounds are the most subsequences in one restart interval
+(tests/test_jpeg_craft_host.py), and the GPU tests time that case."""
 import re
 import sys
 from pathlib import Path
@@ -41,11 +44,12 @@ def test_sync_equals_sequential(sbits):
         rounds[name] = _same(data, sbits)
     print(f"sbits {sbits}: sync rounds {rounds}")
     assert all(r >= 1 for r in rounds.values())
-    if sbits >= 4096:             # longer than the distance a decoder needs to find the true path
+    if sbits >= 4096:             # encoder-made files: longer than the distance a decoder needs to find the true path
         assert max(rounds.values()) <= 3, rounds
 
 
 def _bounded(data, name):
+    """An encoder-made file: its decoders resynchronise within a subsequence, so the rounds stay at 3 or fewer."""
     n_subs = -(-jpeg.parse(data).length * 8 // SBITS)
     rounds = _same(data, SBITS)
     print(f"{name}: {rounds} rounds for {n_subs} subsequences of {SBITS} bits")
@@ -74,3 +78,14 @@ def test_random_entropy_is_defined():
         st = jpeg.decode_stages(data)
         assert st["rgb"].shape == (st["info"].h, st["info"].w, 3)
         assert not st["coef"][~st["decoded"]].any()
+
+
+def test_corrupt_corpus_is_defined():
+    """The corrupt files of tests/test_gpu_jpeg_craft.py: each is accepted by the parser, and the restatement of the
+    device decode equals the sequential decoder on it."""
+    from test_gpu_jpeg_craft import corpus
+    for name, data in corpus():
+        want, dec = jpeg.entropy_decode(data)
+        got, gdec, _ = sync_decode(data, SBITS)
+        assert np.array_equal(gdec, dec), name
+        assert np.array_equal(got, want), name
