@@ -1407,6 +1407,15 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
     DEFER_CHECK(jb[6] >= 0 && jb[7] >= 0 && (uint64_t)jb[6] + (uint64_t)jb[7] <= nbytes[i],
                 "submit_jpegs: file %d: entropy data [%d, %d + %d) outside its %llu bytes", i, jb[6], jb[6], jb[7],
                 (unsigned long long)nbytes[i]);
+    DEFER_CHECK(jb[10] >= 0 && jb[10] <= DEFER_JPEG_MAX_SCANS && jb[11] >= 0 && jb[11] <= DEFER_JPEG_MAX_TABLES,
+                "submit_jpegs: file %d: %d scans and %d Huffman tables, at most %d and %d", i, jb[10], jb[11],
+                DEFER_JPEG_MAX_SCANS, DEFER_JPEG_MAX_TABLES);
+    for (int k = 0; k < jb[10]; ++k) {
+      const int32_t* sc = jb + DEFER_JPEG_SCAN_OFF + k * DEFER_JPEG_SCAN_INTS;
+      DEFER_CHECK(sc[9] >= 0 && sc[10] >= 0 && (uint64_t)sc[9] + (uint64_t)sc[10] <= nbytes[i],
+                  "submit_jpegs: file %d: scan %d's entropy data [%d, %d + %d) outside its %llu bytes", i, k, sc[9], sc[9],
+                  sc[10], (unsigned long long)nbytes[i]);
+    }
   }
   DEFER_TRY(set_device(s));
   Lane& L = s->lanes[seq % s->cfg.depth];
@@ -1415,8 +1424,22 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
     DEFER_CUDA(cudaMemcpyAsync(dst + (size_t)(first_index + i) * slot, data[i], nbytes[i], cudaMemcpyHostToDevice, L.stream));
   DEFER_CUDA(cudaMemcpy2DAsync(L.tables + (size_t)first_index * f.block_ints, f.block_ints * 4, blocks, per * 4,
                                f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
-  DEFER_CUDA(cudaMemcpy2DAsync(L.jpeg_blocks + (size_t)first_index * DEFER_JPEG_BLOCK_INTS, DEFER_JPEG_BLOCK_INTS * 4,
-                               blocks + f.block_ints, per * 4, DEFER_JPEG_BLOCK_INTS * 4, n, cudaMemcpyHostToDevice, L.stream));
+  // each JPEG block's prefix that its file uses (a baseline file: DEFER_JPEG_BASE_INTS), in one copy when all are baseline
+  auto used = [&](int i) {
+    const int32_t* jb = blocks + (size_t)i * per + f.block_ints;
+    return jb[10] ? (size_t)DEFER_JPEG_POOL_OFF + (size_t)jb[11] * DEFER_JPEG_HUFF_INTS : (size_t)DEFER_JPEG_BASE_INTS;
+  };
+  bool all_base = true;
+  for (int i = 0; i < n; ++i) all_base &= used(i) == DEFER_JPEG_BASE_INTS;
+  if (all_base) {
+    DEFER_CUDA(cudaMemcpy2DAsync(L.jpeg_blocks + (size_t)first_index * DEFER_JPEG_BLOCK_INTS, DEFER_JPEG_BLOCK_INTS * 4,
+                                 blocks + f.block_ints, per * 4, DEFER_JPEG_BASE_INTS * 4, n, cudaMemcpyHostToDevice,
+                                 L.stream));
+  } else {
+    for (int i = 0; i < n; ++i)
+      DEFER_CUDA(cudaMemcpyAsync(L.jpeg_blocks + (size_t)(first_index + i) * DEFER_JPEG_BLOCK_INTS,
+                                 blocks + (size_t)i * per + f.block_ints, used(i) * 4, cudaMemcpyHostToDevice, L.stream));
+  }
   return DEFER_OK;
 }
 

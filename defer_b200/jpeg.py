@@ -1,4 +1,4 @@
-"""Baseline JPEG files at ingress: the marker parser and per-sample block of ``DEFER(decode="jpeg")``, and ``decode_jpeg``,
+"""Baseline and progressive JPEG files at ingress: the marker parser and per-sample block of ``DEFER(decode="jpeg")``, and ``decode_jpeg``,
 the host restatement that the GPU decode (``DEFER_OP_JPEG_DECODE``) is tested against.
 
 ``decode_jpeg(data)`` equals ``np.asarray(PIL.Image.open(io.BytesIO(data)).convert("RGB"))`` byte for byte for the files
@@ -23,12 +23,31 @@ Accepted: SOF0 / SOF1 with 8-bit samples, one scan holding every component, 1 (g
 luma sampling 1x1, 2x1 or 2x2 with 1x1 chroma (4:4:4, 4:2:2, 4:2:0), restart intervals, any APPn / COM segments.  Anything
 else raises a ``ValueError`` that names the reason.
 
+Progressive files (SOF2) are accepted with the same limits.  Each scan's entropy data ends at the next marker that is not
+stuffing, RSTn or fill; DHT, DRI, DQT, COM and APPn segments may come between scans, and each scan uses the Huffman
+tables and restart interval in force when it starts, while a component's quantisation table is latched at its first
+scan.  The scan script is checked as libjpeg checks it, and what libjpeg only warns about is refused: a DC scan with
+Se != 0, an AC scan of several components or of a component before its DC scan, Ss > Se or Se > 63, Ah != 0 with
+Al != Ah - 1, Al > 13, a refinement whose Ah is not the coefficients' bit state, and a first scan of coefficients already
+sent.  So are DC scans of some but not all of three components, more than ``MAX_SCANS`` scans or ``MAX_TABLES`` distinct
+Huffman tables, and files libjpeg-turbo would decode with block smoothing (every component has had a DC scan and some
+component's zigzag coefficients 1..9 are not fully refined).  Coefficients 10..63 never sent or only partly refined are
+fine: their missing bits are zero.  Bits of a refinement are applied as ``jdphuff.c`` applies them, in int16.
+
 Corrupt entropy data has one defined result here, and the device computes the same (there is no promise to match libjpeg
 on it).  The entropy data is unstuffed byte by byte (``unstuff``); restart interval ``k`` is the bytes between the
 ``k``-th and ``k+1``-th RST marker; bits past an interval's end read as zero; a block is decoded only if it starts before
 the interval's end, and at most the interval's own number of blocks is decoded; an invalid Huffman code, or an AC run
 past coefficient 63, ends the decode of the whole image: that block and every later block are zero.  DC prediction runs
 in int32 per component and restarts with each interval.
+
+A progressive file decodes scan by scan under the same rules for unstuffing, intervals and bits past an interval's end;
+the blocks of a scan are walked in its own order (the MCUs of a scan of all components, else the component's own block
+grid), and restart intervals count units of that order.  A block that is not inside an EOB run is decoded only if it
+starts before its interval's end; the blocks of an EOB run belong to the symbol that starts it, and at most the
+interval's own number of blocks is decoded.  An invalid code, a run past Se (a ZRL included), or a refinement symbol of a
+size other than 0 or 1 ends the decode: that block and every later block of the scan, in scan order, get nothing from
+the scan, no later scan is decoded, and everything the earlier scans and blocks wrote stays.
 """
 from __future__ import annotations
 
@@ -46,23 +65,51 @@ import numpy as np
 #   [Q_END + t * HUFF_INTS ...]         Huffman table t: DC of component 0, 1, 2, then AC of component 0, 1, 2
 # A Huffman table is [lookahead[2^LOOKAHEAD] (len << 8 | symbol for codes of <= LOOKAHEAD bits, else 0),
 #                     maxcode[17] (largest code of length l, -1 if none), valoff[17] (symbol index - code), vals[256]]
+#   [10] scans of a progressive file (0 = baseline)  [11] Huffman tables in its pool
+# A progressive file's block goes on past the baseline part (whose six Huffman tables it leaves zero):
+#   [SCAN_OFF + s * SCAN_INTS ...]      scan s: components in scan, their frame indices [3], Ss, Se, Ah, Al, restart
+#                                       interval (MCUs, or blocks of a one-component scan), entropy offset and length,
+#                                       pool index of each component's DC table [3], pool index of the AC table, 0
+#   [POOL_OFF + t * HUFF_INTS ...]      Huffman table t of the pool
+# Only the prefix a file uses is copied to the GPU: BASE_INTS values for a baseline file (``block_ints``).
 HDR_INTS = 16
 Q_OFF = HDR_INTS
 Q_END = Q_OFF + 3 * 64
 LOOKAHEAD = 9
 HUFF_INTS = (1 << LOOKAHEAD) + 17 + 17 + 256
-BLOCK_INTS = Q_END + 6 * HUFF_INTS
+BASE_INTS = Q_END + 6 * HUFF_INTS
+MAX_SCANS = 32                    # DEFER_JPEG_MAX_SCANS: scans of one progressive file
+MAX_TABLES = 32                   # DEFER_JPEG_MAX_TABLES: distinct Huffman tables of one progressive file
+SCAN_INTS = 16
+SCAN_OFF = BASE_INTS
+POOL_OFF = SCAN_OFF + MAX_SCANS * SCAN_INTS
+BLOCK_INTS = POOL_OFF + MAX_TABLES * HUFF_INTS
 
 #: zigzag position k -> natural (row-major) index
 ZIGZAG = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,
                    7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31,
                    39, 46, 53, 60, 61, 54, 47, 55, 62, 63], np.int32)
 
-_SOF_NAMES = {0xC2: "progressive", 0xC3: "lossless", 0xC5: "differential (hierarchical)",
+_SOF_NAMES = {0xC3: "lossless", 0xC5: "differential (hierarchical)",
               0xC6: "differential progressive", 0xC7: "differential lossless", 0xC9: "arithmetic-coded",
               0xCA: "arithmetic-coded progressive", 0xCB: "arithmetic-coded lossless",
               0xCD: "arithmetic-coded differential", 0xCE: "arithmetic-coded differential progressive",
               0xCF: "arithmetic-coded differential lossless"}
+
+
+@dataclass(frozen=True)
+class Scan:
+    """One scan of a progressive file."""
+    comps: Tuple[int, ...]        # frame indices of its components (all of them, in frame order, or one)
+    ss: int                       # spectral selection Ss..Se (zigzag), successive approximation Ah, Al
+    se: int
+    ah: int
+    al: int
+    restart: int                  # restart interval in force at the scan: MCUs, or blocks of a one-component scan
+    offset: int                   # entropy-coded data: data[offset:offset + length]
+    length: int
+    dc: Tuple[int, ...]           # pool index of each component's DC table (a DC first scan), else -1
+    ac: int                       # pool index of the AC table (an AC scan), else -1
 
 
 @dataclass(frozen=True)
@@ -76,8 +123,14 @@ class JpegInfo:
     offset: int                   # entropy-coded data: data[offset:offset + length] (up to the EOI marker)
     length: int
     quant: Tuple[np.ndarray, ...]  # per component, int32 [64] natural order
-    dc: Tuple[np.ndarray, ...]     # per component, int32 [HUFF_INTS]
+    dc: Tuple[np.ndarray, ...]     # per component, int32 [HUFF_INTS] (baseline)
     ac: Tuple[np.ndarray, ...]
+    scans: Tuple[Scan, ...] = ()   # progressive: its scans in file order, and the Huffman tables they use
+    tables: Tuple[np.ndarray, ...] = ()
+
+    @property
+    def progressive(self) -> bool:
+        return bool(self.scans)
 
 
 def _refuse(why: str):
@@ -171,7 +224,7 @@ def parse(data) -> JpegInfo:
     if n < 4 or d[0] != 0xFF or d[1] != 0xD8:
         _refuse("not a JPEG file (no SOI marker)")
     p = 2
-    qt, ht, frame, restart = {}, {}, None, 0
+    qt, ht, frame, restart, progressive = {}, {}, None, 0, False
     jfif, adobe = False, None
     while True:
         if p >= n or d[p] != 0xFF:
@@ -205,7 +258,8 @@ def parse(data) -> JpegInfo:
             if len(seg) != 2:
                 _refuse("malformed DRI segment")
             restart = (seg[0] << 8) | seg[1]
-        elif m in (0xC0, 0xC1):
+        elif m in (0xC0, 0xC1, 0xC2):
+            progressive = m == 0xC2
             if frame is not None:
                 _refuse("more than one frame")
             if len(seg) < 6:
@@ -222,7 +276,8 @@ def parse(data) -> JpegInfo:
             comps = [(seg[6 + 3 * i], seg[7 + 3 * i] >> 4, seg[7 + 3 * i] & 15, seg[8 + 3 * i]) for i in range(nc)]
             frame = (h, w, comps)
         elif m in _SOF_NAMES:
-            _refuse(f"{_SOF_NAMES[m]} JPEG (only baseline and extended sequential Huffman JPEGs are decoded)")
+            _refuse(f"{_SOF_NAMES[m]} JPEG (only baseline, extended sequential and progressive Huffman JPEGs are "
+                    "decoded)")
         elif m == 0xDA:
             break
         elif 0xE0 <= m <= 0xEF or m == 0xFE:
@@ -230,7 +285,7 @@ def parse(data) -> JpegInfo:
         else:
             _refuse(f"unsupported marker 0xFF{m:02X}")
     if frame is None:
-        _refuse("no SOF0/SOF1 frame before the scan")
+        _refuse("no SOF0/SOF1/SOF2 frame before the scan")
     h, w, comps = frame
     nc = len(comps)
     ids = tuple(c[0] for c in comps)
@@ -238,6 +293,8 @@ def parse(data) -> JpegInfo:
         _refuse("RGB colour transform (Adobe or 'RGB' component ids; only YCbCr is decoded)")
     if nc == 3 and adobe is not None and adobe not in (0, 1) and not jfif:
         _refuse(f"Adobe colour transform {adobe}")
+    if progressive:
+        return _parse_progressive(d, p, seg, h, w, comps, qt, ht, restart)
     ns = seg[0] if seg else 0
     if len(seg) != 4 + 2 * ns:
         _refuse("malformed SOS segment")
@@ -249,13 +306,7 @@ def parse(data) -> JpegInfo:
     ss, se, ahal = seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns]
     if (ss, se, ahal) != (0, 63, 0):
         _refuse("spectral selection or successive approximation in a sequential scan")
-    if nc == 3:
-        hs, vs = comps[0][1], comps[0][2]
-        if (hs, vs) not in ((1, 1), (2, 1), (2, 2)) or any((c[1], c[2]) != (1, 1) for c in comps[1:]):
-            _refuse("sampling factors " + ",".join(f"{c[1]}x{c[2]}" for c in comps)
-                    + " (4:4:4, 4:2:2 and 4:2:0 are decoded)")
-    else:
-        hs = vs = 1
+    hs, vs = _sampling(comps)
     quant, dc, ac = [], [], []
     for (cid, _, _, tq), (_, td, ta) in zip(comps, scan):
         if tq not in qt:
@@ -277,6 +328,142 @@ def parse(data) -> JpegInfo:
     while end > p and d[end - 1] == 0xFF:      # fill bytes before the marker
         end -= 1
     return JpegInfo(h, w, nc, hs, vs, restart, p, end - p, tuple(quant), tuple(dc), tuple(ac))
+
+
+def _sampling(comps) -> Tuple[int, int]:
+    """Luma sampling factors (hs, vs) of the frame's components, or a refusal."""
+    if len(comps) == 1:
+        return 1, 1
+    hs, vs = comps[0][1], comps[0][2]
+    if (hs, vs) not in ((1, 1), (2, 1), (2, 2)) or any((c[1], c[2]) != (1, 1) for c in comps[1:]):
+        _refuse("sampling factors " + ",".join(f"{c[1]}x{c[2]}" for c in comps)
+                + " (4:4:4, 4:2:2 and 4:2:0 are decoded)")
+    return hs, vs
+
+
+def _parse_progressive(d: bytes, p: int, seg: bytes, h: int, w: int, comps, qt: dict, ht: dict, restart: int) -> JpegInfo:
+    """The scans of a progressive file, from its first SOS (payload ``seg``, entropy data from ``p``) to the EOI.  The
+    scan script is checked as libjpeg's ``start_pass_phuff_decoder`` checks it, and what libjpeg only warns about is
+    refused here too; so is a file libjpeg would decode with block smoothing.  Each scan's entropy data ends at the next
+    marker that is not stuffing, RSTn or fill: one vectorised byte search per file."""
+    nc = len(comps)
+    hs, vs = _sampling(comps)
+    b = np.frombuffer(d, np.uint8)
+    nxt = b[1:]
+    ends = np.nonzero((b[:-1] == 0xFF) & (nxt != 0) & ((nxt < 0xD0) | (nxt > 0xD7)) & (nxt != 0xFF))[0]
+    ids = [c[0] for c in comps]
+    bits = [[-1] * 64 for _ in range(nc)]         # libjpeg's coef_bits: -1 = never sent, else the last scan's Al
+    quant: List[Optional[np.ndarray]] = [None] * nc
+    scans, pool, pool_ix = [], [], {}
+
+    def table(key, cid):
+        if key not in ht:
+            _refuse(f"component {cid} uses an undefined Huffman table")
+        t = ht[key]
+        if id(t) not in pool_ix:
+            if len(pool) == MAX_TABLES:
+                _refuse(f"more than {MAX_TABLES} distinct Huffman tables in one progressive file (DEFER_JPEG_MAX_TABLES)")
+            pool_ix[id(t)] = len(pool)
+            pool.append(t)
+        return pool_ix[id(t)]
+
+    while True:                                   # at a scan: seg is its SOS payload, p its first entropy byte
+        if len(scans) == MAX_SCANS:
+            _refuse(f"more than {MAX_SCANS} scans in one progressive file (DEFER_JPEG_MAX_SCANS)")
+        ns = seg[0] if seg else 0
+        if ns < 1 or len(seg) != 4 + 2 * ns:
+            _refuse("malformed SOS segment")
+        sel = [(seg[1 + 2 * i], seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
+        if any(c[0] not in ids for c in sel):
+            _refuse("scan of a component the frame does not have")
+        idx = [ids.index(c[0]) for c in sel]
+        if idx != sorted(set(idx)):
+            _refuse("scan components repeated or out of frame order")
+        ss, se, ah, al = seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns] >> 4, seg[3 + 2 * ns] & 15
+        if ss == 0 and se != 0:
+            _refuse(f"bad progressive scan script: a DC scan with Se = {se}")
+        if ss != 0 and (ss > se or se > 63):
+            _refuse(f"bad progressive scan script: spectral selection {ss}..{se}")
+        if ss != 0 and ns != 1:
+            _refuse(f"bad progressive scan script: an AC scan of {ns} components")
+        if ah != 0 and al != ah - 1:
+            _refuse(f"bad progressive scan script: successive approximation Ah = {ah}, Al = {al}")
+        if al > 13:
+            _refuse(f"bad progressive scan script: Al = {al} > 13")
+        if 1 < ns < nc:
+            _refuse(f"progressive DC scan of {ns} of {nc} components (interleaved scans of all components or "
+                    "scans of one are decoded)")
+        for c in idx:
+            if ss > 0 and bits[c][0] < 0:
+                _refuse(f"bad progressive scan script: an AC scan of component {ids[c]} before its DC scan")
+            for k in range(ss, se + 1):
+                cur = bits[c][k]
+                if ah != max(cur, 0):
+                    _refuse(f"bad progressive scan script: component {ids[c]} coefficient {k} refined with Ah = "
+                            f"{ah}, its bit state is {cur}")
+                if ah == 0 and cur >= 0:
+                    _refuse(f"bad progressive scan script: component {ids[c]} coefficient {k} sent twice")
+                bits[c][k] = al
+            if quant[c] is None:                  # latch_quant_tables: a later DQT does not change it
+                tq = comps[c][3]
+                if tq not in qt:
+                    _refuse(f"component {ids[c]} uses undefined quantisation table {tq}")
+                quant[c] = qt[tq]
+        dc = tuple(table((0, td), cid) for cid, td, _ in sel) if ss == 0 and ah == 0 else (-1,) * ns
+        ac = table((1, sel[0][2]), sel[0][0]) if ss > 0 else -1
+        i = int(np.searchsorted(ends, p))
+        if i == len(ends):
+            _refuse("truncated file (no EOI marker)")
+        end = int(ends[i])
+        e = end
+        while e > p and d[e - 1] == 0xFF:         # fill bytes before the marker
+            e -= 1
+        scans.append(Scan(tuple(idx), ss, se, ah, al, restart, p, e - p, dc + (-1,) * (3 - ns), ac))
+        p = end
+        while True:                               # the markers up to the next scan or the EOI
+            while p < len(d) and d[p] == 0xFF:
+                p += 1
+            if p >= len(d):
+                _refuse("truncated file (no EOI marker)")
+            m = d[p]
+            p += 1
+            if m == 0xD9:
+                break
+            if m == 0xDC:
+                _refuse("DNL marker after the scan")
+            if m in (0x01,) or 0xD0 <= m <= 0xD8 or 0xC0 <= m <= 0xCF and m != 0xC4:
+                _refuse(f"unexpected marker 0xFF{m:02X} between scans")
+            if p + 2 > len(d):
+                _refuse("truncated file (no EOI marker)")
+            ln = (d[p] << 8) | d[p + 1]
+            if ln < 2 or p + ln > len(d):
+                _refuse(f"segment 0xFF{m:02X} of length {ln} runs past the end of the file")
+            seg = d[p + 2:p + ln]
+            p += ln
+            if m == 0xDA:
+                break
+            if m == 0xDB:
+                qt.update(dqt_tables(seg))
+            elif m == 0xC4:
+                ht.update(dht_tables(seg))
+            elif m == 0xDD:
+                if len(seg) != 2:
+                    _refuse("malformed DRI segment")
+                restart = (seg[0] << 8) | seg[1]
+            elif not (0xE0 <= m <= 0xEF or m == 0xFE):
+                _refuse(f"unsupported marker 0xFF{m:02X} between scans")
+        if m == 0xD9:
+            break
+    # libjpeg-turbo 3.1 smooths blocks (smoothing_ok) when every component has had a DC scan, none of its quantisers of
+    # zigzag 0..9 is zero, and some component's coefficients 1..9 are not fully refined
+    if (all(bits[c][0] >= 0 for c in range(nc)) and all(int(q[n]) != 0 for q in quant for n in ZIGZAG[:10])
+            and any(bits[c][k] != 0 for c in range(nc) for k in range(1, 10))):
+        _refuse("incomplete progression: zigzag coefficients 1..9 are not all fully refined, which libjpeg decodes "
+                "with block smoothing (not supported)")
+    q = tuple(x if x is not None else np.zeros(64, np.int32) for x in quant)
+    first = scans[0].offset
+    last = max(s.offset + s.length for s in scans)
+    return JpegInfo(h, w, nc, hs, vs, 0, first, last - first, q, (), (), tuple(scans), tuple(pool))
 
 
 @dataclass(frozen=True)
@@ -305,15 +492,28 @@ def geometry(h: int, w: int, ncomp: int, hs: int, vs: int) -> Geometry:
     return Geometry(mx, my, hs * vs + 2, (0,) * (hs * vs) + (1, 2), (mx * hs, mx, mx), (my * vs, my, my))
 
 
-def pack_block(info: JpegInfo) -> np.ndarray:
-    """One sample's int32 block (layout above)."""
-    b = np.zeros(BLOCK_INTS, np.int32)
+def block_ints(info: JpegInfo) -> int:
+    """How much of its block a file uses: the baseline part, or up to the last Huffman table of its pool."""
+    return POOL_OFF + len(info.tables) * HUFF_INTS if info.progressive else BASE_INTS
+
+
+def pack_block(info: JpegInfo, out: Optional[np.ndarray] = None) -> np.ndarray:
+    """One sample's int32 block (layout above); ``out``: a zeroed int32 [BLOCK_INTS] to write it into."""
+    b = np.zeros(BLOCK_INTS, np.int32) if out is None else out
     g = geometry(info.h, info.w, info.ncomp, info.hs, info.vs)
-    b[:10] = (info.h, info.w, info.ncomp, info.hs, info.vs, info.restart, info.offset, info.length, g.mcux, g.mcuy)
+    b[:12] = (info.h, info.w, info.ncomp, info.hs, info.vs, info.restart, info.offset, info.length, g.mcux, g.mcuy,
+              len(info.scans), len(info.tables))
     for c in range(info.ncomp):
         b[Q_OFF + 64 * c:Q_OFF + 64 * (c + 1)] = info.quant[c]
-        b[Q_END + c * HUFF_INTS:Q_END + (c + 1) * HUFF_INTS] = info.dc[c]
-        b[Q_END + (3 + c) * HUFF_INTS:Q_END + (4 + c) * HUFF_INTS] = info.ac[c]
+        if not info.progressive:
+            b[Q_END + c * HUFF_INTS:Q_END + (c + 1) * HUFF_INTS] = info.dc[c]
+            b[Q_END + (3 + c) * HUFF_INTS:Q_END + (4 + c) * HUFF_INTS] = info.ac[c]
+    for i, sc in enumerate(info.scans):
+        comps = sc.comps + (0,) * (3 - len(sc.comps))
+        b[SCAN_OFF + i * SCAN_INTS:SCAN_OFF + (i + 1) * SCAN_INTS] = (
+            len(sc.comps), *comps, sc.ss, sc.se, sc.ah, sc.al, sc.restart, sc.offset, sc.length, *sc.dc, sc.ac, 0)
+    for t, tab in enumerate(info.tables):
+        b[POOL_OFF + t * HUFF_INTS:POOL_OFF + (t + 1) * HUFF_INTS] = tab
     return b
 
 
@@ -600,19 +800,200 @@ def color_convert(pl: List[np.ndarray], info: JpegInfo) -> np.ndarray:
     return np.ascontiguousarray(np.clip(np.stack([r, g, b], axis=2), 0, 255).astype(np.uint8))
 
 
+# ----------------------------------------------------------------------------------------- progressive files, sequentially
+def _i16(v: int) -> int:
+    return ((v + 32768) & 0xFFFF) - 32768
+
+
+def scan_blocks(info: JpegInfo, scan: Scan) -> Tuple[np.ndarray, int]:
+    """The stream-order block of each block of ``scan`` in scan order, and the blocks per unit (restart intervals count
+    units).  A scan of all components walks the MCUs, as a baseline scan.  A scan of one component walks that
+    component's own grid of ``ceil(w * hc / (hmax * 8)) x ceil(h * vc / (vmax * 8))`` blocks, which can be smaller than
+    its MCU-padded grid: the padding blocks only get a DC value, from interleaved DC scans."""
+    g = geometry(info.h, info.w, info.ncomp, info.hs, info.vs)
+    if len(scan.comps) > 1 or info.ncomp == 1:
+        return np.arange(g.blocks), g.bpm if len(scan.comps) > 1 else 1
+    c = scan.comps[0]
+    hc, vc = (info.hs, info.vs) if c == 0 else (1, 1)
+    cw, ch = -(-info.w * hc // (info.hs * 8)), -(-info.h * vc // (info.vs * 8))
+    by, bx = np.divmod(np.arange(cw * ch), cw)
+    j = (by % vc) * hc + bx % hc if c == 0 else info.hs * info.vs + c - 1
+    return ((by // vc) * g.mcux + bx // hc) * g.bpm + j, 1
+
+
+def _bit(r: BitReader, pos: int) -> int:
+    return r.peek16(pos) >> 15
+
+
+def _decode_interval(r: BitReader, sc: Scan, tabs, zz, blks, comp_of) -> Optional[int]:
+    """Decode one restart interval of scan ``sc`` into the zigzag-order coefficient lists ``zz``: ``blks`` are its
+    stream-order blocks in scan order, ``comp_of`` the scan component of each position in a unit.  Returns the index in
+    ``blks`` of the block whose decode failed (it and every later block get nothing from the scan), else None."""
+    ss, se, al, pos = sc.ss, sc.se, sc.al, 0
+    if ss == 0 and sc.ah == 0:                        # DC first
+        pred = [0, 0, 0]
+        for i, b in enumerate(blks):
+            if pos >= r.nbits:
+                break
+            c = comp_of[i % len(comp_of)]
+            l, s = decode_symbol(tabs[sc.dc[c]], r.peek16(pos))
+            if l == 0:
+                return i
+            s &= 15
+            v = extend(r.peek16(pos + l) >> (16 - s), s) if s else 0
+            pos += l + s
+            pred[c] = ((pred[c] + v + (1 << 31)) & 0xFFFFFFFF) - (1 << 31)
+            zz[b][0] = _i16(pred[c] << al)
+        return None
+    if ss == 0:                                       # DC refinement: one raw bit per block
+        for i, b in enumerate(blks):
+            if pos >= r.nbits:
+                break
+            if _bit(r, pos):
+                zz[b][0] = _i16(zz[b][0] | (1 << al))
+            pos += 1
+        return None
+    t, eob = tabs[sc.ac], 0
+    if sc.ah == 0:                                    # AC first
+        for i, b in enumerate(blks):
+            if eob:
+                eob -= 1
+                continue
+            if pos >= r.nbits:
+                break
+            k, new = ss, {}
+            while k <= se:
+                l, sym = decode_symbol(t, r.peek16(pos))
+                if l == 0:
+                    return i
+                pos += l
+                run, s = sym >> 4, sym & 15
+                if s:
+                    k += run
+                    if k > se:
+                        return i
+                    new[k] = _i16(extend(r.peek16(pos) >> (16 - s), s) << al)
+                    pos += s
+                    k += 1
+                elif run == 15:
+                    if k + 16 > se + 1:
+                        return i
+                    k += 16
+                else:
+                    eob = (1 << run) - 1 + ((r.peek16(pos) >> (16 - run)) if run else 0)
+                    pos += run
+                    break
+            for k, v in new.items():
+                zz[b][k] = v
+        return None
+    p1, m1 = 1 << al, -(1 << al)                      # AC refinement
+
+    def correct(v):
+        return _i16(v + (p1 if v >= 0 else m1)) if (v & p1) == 0 else v
+
+    for i, b in enumerate(blks):
+        if eob == 0 and pos >= r.nbits:
+            break
+        new, k = list(zz[b]), ss
+        if eob == 0:
+            while k <= se:
+                l, sym = decode_symbol(t, r.peek16(pos))
+                if l == 0:
+                    return i
+                pos += l
+                run, s = sym >> 4, sym & 15
+                if s:
+                    if s != 1:
+                        return i
+                    s = p1 if _bit(r, pos) else m1
+                    pos += 1
+                elif run != 15:
+                    eob = (1 << run) + ((r.peek16(pos) >> (16 - run)) if run else 0)
+                    pos += run
+                    break
+                while k <= se:                        # skip `run` zero-history coefficients, correcting the others
+                    if new[k]:
+                        if _bit(r, pos):
+                            new[k] = correct(new[k])
+                        pos += 1
+                    else:
+                        run -= 1
+                        if run < 0:
+                            break
+                    k += 1
+                if k > se:
+                    return i
+                if s:
+                    new[k] = _i16(s)
+                k += 1
+        if eob:
+            while k <= se:
+                if new[k]:
+                    if _bit(r, pos):
+                        new[k] = correct(new[k])
+                    pos += 1
+                k += 1
+            eob -= 1
+        zz[b] = new
+    return None
+
+
+def progressive_decode(data, info: Optional[JpegInfo] = None) -> Tuple[np.ndarray, dict]:
+    """Sequential decode of a progressive file, one scan after another: final int16 coefficients ``[blocks, 64]`` in
+    stream order and natural order, and the counters the device writes (``T`` unstuffed bytes and ``R`` RST markers
+    summed over the scans decoded, ``scans`` completed, ``cutoff`` the scan-order block where the decode failed, else
+    the block count)."""
+    d = _as_bytes(data)
+    info = info or parse(d)
+    g = geometry(info.h, info.w, info.ncomp, info.hs, info.vs)
+    zz = [[0] * 64 for _ in range(g.blocks)]
+    st = {"T": 0, "R": 0, "scans": 0, "cutoff": g.blocks}
+    for sc in info.scans:
+        comp, rst = unstuff(d[sc.offset:sc.offset + sc.length])
+        st["T"] += len(comp)
+        st["R"] += len(rst)
+        blks, per = scan_blocks(info, sc)
+        comp_of = list(g.comp_of) if per > 1 else [0]
+        units = len(blks) // per
+        ri = sc.restart
+        nseg = -(-units // ri) if ri else 1
+        bad = None
+        for k, (s, e) in enumerate(segments(len(comp), rst, nseg)):
+            u0 = k * ri if ri else 0
+            part = blks[u0 * per:(u0 + (min(ri, units - u0) if ri else units)) * per]
+            bad = _decode_interval(BitReader(comp, s, e), sc, info.tables, zz, part, comp_of)
+            if bad is not None:
+                bad += u0 * per
+                break
+        if bad is not None:
+            st["cutoff"] = bad
+            break
+        st["scans"] += 1
+    coef = np.zeros((g.blocks, 64), np.int16)
+    coef[:, ZIGZAG] = np.array(zz, np.int64).astype(np.int16)
+    return coef, st
+
+
 def decode_stages(data) -> dict:
-    """Every stage of ``decode_jpeg``: ``info``, ``coef`` (final, ``[blocks, 64]`` stream order), ``decoded`` (per block),
-    ``planes`` and ``rgb``."""
+    """Every stage of ``decode_jpeg``: ``info``, ``coef`` (final, ``[blocks, 64]`` stream order), ``decoded`` (per block;
+    all of a progressive file's), ``planes`` and ``rgb``; and for a progressive file ``progress``, the counters of
+    ``progressive_decode``."""
     d = _as_bytes(data)
     info = parse(d)
-    raw, decoded = entropy_decode(d, info)
-    coef = dc_predict(raw, decoded, info)
+    out = {"info": info}
+    if info.progressive:
+        coef, out["progress"] = progressive_decode(d, info)
+        decoded = np.ones(len(coef), bool)
+    else:
+        raw, decoded = entropy_decode(d, info)
+        coef = dc_predict(raw, decoded, info)
     pl = planes(coef, info)
-    return {"info": info, "coef": coef, "decoded": decoded, "planes": pl, "rgb": color_convert(pl, info)}
+    out.update(coef=coef, decoded=decoded, planes=pl, rgb=color_convert(pl, info))
+    return out
 
 
 def decode_jpeg(data) -> np.ndarray:
-    """Decode one baseline JPEG file to uint8 RGB ``(h, w, 3)``, byte for byte as Keras' ``load_img`` does through Pillow
+    """Decode one baseline or progressive JPEG file to uint8 RGB ``(h, w, 3)``, byte for byte as Keras' ``load_img`` does through Pillow
     (``np.asarray(Image.open(io.BytesIO(data)).convert("RGB"))``, libjpeg-turbo 3.1).  ``DEFER(decode="jpeg")`` runs the
     same decode on the GPU.  Unsupported files raise a ValueError (see ``parse``)."""
     return decode_stages(data)["rgb"]

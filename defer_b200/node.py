@@ -24,7 +24,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .node_state import NodeState
 from .planner import Plan, plan_stage
-from .jpeg import check_jpeg, pack_block
+from .jpeg import BLOCK_INTS, check_jpeg, pack_block
 from .resize import check_frame, pack_frame_tables
 
 DTYPE_TO_FMT = {
@@ -272,7 +272,11 @@ class StageRunner:
             raise ValueError(f"{self.name}: {n} files from sample {index} do not fit the microbatch of {self.batch}")
         hw = np.array([(i.h, i.w) for i in infos], np.int32).reshape(n, 2)
         tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"])
-        blocks = np.concatenate([tables, np.stack([pack_block(i) for i in infos])], axis=1)
+        nr = tables.shape[1]
+        blocks = np.zeros((n, nr + BLOCK_INTS), np.int32)      # only the prefix each file uses is written and copied
+        blocks[:, :nr] = tables
+        for k, i in enumerate(infos):
+            pack_block(i, blocks[k, nr:])
         sizes = np.array([len(f) for f in files], np.uint64)
         self._tables[seq % self.depth] = (blocks, sizes, files)
         ptrs = (C.c_void_p * n)(*[C.cast(C.c_char_p(f), C.c_void_p).value for f in files])

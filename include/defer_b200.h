@@ -102,20 +102,42 @@ typedef enum defer_op_kind {
  * slots by defer_stage_submit_jpegs after the resize blocks, is DEFER_JPEG_BLOCK_INTS values:
  *   [0] h  [1] w  [2] components (1 | 3)  [3] luma h-sampling  [4] luma v-sampling (1x1, 2x1 or 2x2; chroma 1x1)
  *   [5] restart interval in MCUs (0 = none)  [6] entropy-data offset in the file  [7] its length (up to EOI)
- *   [8] MCUs across  [9] MCUs down  [10..15] 0
+ *   [8] MCUs across  [9] MCUs down  [10] scans of a progressive file (0: baseline)  [11] Huffman tables in its pool
+ *   [12..15] 0
  *   [16 + 64 c ...]  quantisation table of component c, natural order (c < 3)
  *   [16 + 192 + t * DEFER_JPEG_HUFF_INTS ...]  Huffman table t = DC of component 0, 1, 2, then AC of component 0, 1, 2:
  *        lookahead[2^DEFER_JPEG_LOOKAHEAD] (code length << 8 | symbol for codes of <= LOOKAHEAD bits, 0 otherwise),
  *        maxcode[17] (largest code of each length, -1 if none), valoff[17] (symbol index - code), symbols[256]
+ * A progressive file (SOF2) leaves those six tables zero; its block goes on with
+ *   [DEFER_JPEG_SCAN_OFF + s * DEFER_JPEG_SCAN_INTS ...]  scan s < [10], in file order: components in the scan (all, or
+ *        1), their frame indices [3], Ss, Se, Ah, Al, restart interval (MCUs, or blocks of a one-component scan),
+ *        entropy-data offset in the file and length, pool index of each component's DC table [3] (DC first scans),
+ *        pool index of the AC table (AC scans), 0
+ *   [DEFER_JPEG_POOL_OFF + t * DEFER_JPEG_HUFF_INTS ...]  Huffman table t < [11] of the pool, in the layout above
+ * A baseline file uses DEFER_JPEG_BASE_INTS values of its block, a progressive one DEFER_JPEG_POOL_OFF + [11] *
+ * DEFER_JPEG_HUFF_INTS; only that prefix is copied and read.  A progressive file decodes scan by scan on the same CTA:
+ * DC and AC first scans by self-synchronisation, DC refinements one thread per block, AC refinements sequentially, one
+ * thread per restart interval.
  * The decode never trusts the block: h / w are clamped into the slot, sampling into 4:4:4 / 4:2:2 / 4:2:0, the entropy
  * extent into the slot and every table index into its table, so no block content makes it access memory outside the
  * sample's slot, workspace or image.  The blocks are zeroed at create: a never-written sample decodes to a 1x1 image of
- * value 128.  An invalid Huffman code ends the sample's decode (that block and all later ones are zero); the exact rule
- * for corrupt data is defer_b200/jpeg.py's. */
+ * value 128.  An invalid Huffman code ends the sample's decode (that block and all later ones are zero; in a progressive
+ * file, they get nothing from that scan and no later scan is decoded); the exact rule for corrupt data is
+ * defer_b200/jpeg.py's.  Workspace stats: [0] unstuffed bytes, [1] RST markers, [2] subsequences, [3] rounds, [4] the
+ * first block whose decode failed, else the block count; a progressive file sums [0..3] over its scans decoded, gives
+ * [4] in the failing scan's block order and [5] the scans decoded whole. */
 #define DEFER_JPEG_HDR_INTS 16
 #define DEFER_JPEG_LOOKAHEAD 9
 #define DEFER_JPEG_HUFF_INTS ((1 << DEFER_JPEG_LOOKAHEAD) + 17 + 17 + 256)
-#define DEFER_JPEG_BLOCK_INTS (DEFER_JPEG_HDR_INTS + 3 * 64 + 6 * DEFER_JPEG_HUFF_INTS)
+/* the baseline part of a block, all a baseline file uses */
+#define DEFER_JPEG_BASE_INTS (DEFER_JPEG_HDR_INTS + 3 * 64 + 6 * DEFER_JPEG_HUFF_INTS)
+/* a progressive file: at most this many scans and distinct Huffman tables (more are refused by the parser) */
+#define DEFER_JPEG_MAX_SCANS 32
+#define DEFER_JPEG_MAX_TABLES 32
+#define DEFER_JPEG_SCAN_INTS 16
+#define DEFER_JPEG_SCAN_OFF DEFER_JPEG_BASE_INTS
+#define DEFER_JPEG_POOL_OFF (DEFER_JPEG_SCAN_OFF + DEFER_JPEG_MAX_SCANS * DEFER_JPEG_SCAN_INTS)
+#define DEFER_JPEG_BLOCK_INTS (DEFER_JPEG_POOL_OFF + DEFER_JPEG_MAX_TABLES * DEFER_JPEG_HUFF_INTS)
 /* bits per subsequence of the self-synchronising Huffman decode */
 #define DEFER_JPEG_SUBSEQ_BITS 8192
 

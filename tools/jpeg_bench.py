@@ -14,6 +14,7 @@ here with Pillow from seeded synthetic photos (gradients, waves and noise), 4:2:
   card                the GPU's name and power limit (read-only nvidia-smi query)
 
     python tools/jpeg_bench.py --size 480x640 --items 640 --reps 3
+    python tools/jpeg_bench.py --progressive ...    # the same with progressive files (Pillow progressive=True)
 """
 from __future__ import annotations
 
@@ -39,8 +40,8 @@ G = 32
 BOUND = (1080, 1920)
 
 
-def files(size, quality, n=G):
-    return [encode(content("photo", size[0], size[1], seed=i), "420", quality) for i in range(n)]
+def files(size, quality, n=G, progressive=False):
+    return [encode(content("photo", size[0], size[1], seed=i), "420", quality, progressive=progressive) for i in range(n)]
 
 
 def decode_op_times(model, items, iters):
@@ -87,18 +88,20 @@ def main():
     ap.add_argument("--items", type=int, default=640)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--op-iters", type=int, default=20)
+    ap.add_argument("--progressive", action="store_true", help="encode every file progressive")
     args = ap.parse_args()
     model = applications.ResNet50()
-    out = {"card": card(), "model": "resnet50", "mode": "caffe", "microbatch": G, "decode_op_us": {}}
+    out = {"card": card(), "model": "resnet50", "mode": "caffe", "microbatch": G, "progressive": args.progressive,
+           "decode_op_us": {}}
     for size in ((480, 640), (1080, 1920)):
         for q in (75, 90):
-            items = files(size, q)
+            items = files(size, q, progressive=args.progressive)
             key = f"{size[0]}x{size[1]}_q{q}"
             out["decode_op_us"][key] = decode_op_times(model, items, args.op_iters)
             out.setdefault("pillow_decode_ms", {})[key] = pillow_ms(items[:8])
             out.setdefault("feeder_us", {})[key] = feeder_us(model, items)
     size = parse_size(args.size)
-    base = files(size, args.quality, n=64)
+    base = files(size, args.quality, n=64, progressive=args.progressive)
     jp = [base[i % len(base)] for i in range(args.items)]
     u8 = [jpeg.decode_jpeg(d)[None] for d in base]
     f32 = [applications.preprocess_input(applications.resize_image(x, (224, 224), "bilinear").astype(np.float32))
