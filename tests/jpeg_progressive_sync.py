@@ -24,6 +24,11 @@ from defer_b200 import jpeg
 CAP = 1 << 30
 
 
+def _sat(v: int) -> int:
+    """The device's segmented block-offset sum saturates (SegSat)."""
+    return min(v, CAP)
+
+
 def _pstep(r, pos, k, j, sc, tabs, per, comp_of):
     """pstep: (pos, k, z, v, eob) after one symbol, or None."""
     p = r.peek16(pos)
@@ -98,7 +103,7 @@ def _first_scan(comp, rst, sc, info, g, zz, sbits):
         if t == 0 or subs[t - 1][0] != k:
             acc = 0
         pre.append(acc)
-        acc = min(acc + out[t][3], CAP)
+        acc = _sat(acc + out[t][3])
         seg_total[k] = min(acc, exp[k])
     cut = nq
     for t, (k, r, a, b) in enumerate(subs):

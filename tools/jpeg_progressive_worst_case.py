@@ -7,9 +7,15 @@ first scan of zigzag 1..63 at Al = 1 that sends nothing (one EOB run over every 
 -1.  That is 1071 bits per block, 4.3 MB of entropy data in the 6.2 MB slot.  For comparison, 32 Pillow-written
 progressive 480x640 q90 4:2:0 files.
 
-``defer_k_jpeg_decode`` (all three kernels) is timed with CUDA events as tools/jpeg_worst_case.py times it; one JSON line.
+``--sync`` times the worst case of the first-scan self-synchronisation instead (tests/jpeg_craft_progressive.py
+``worst_first``): a valid 1080x1920 grayscale file whose AC first scan of zigzag 1..63 is 1071-bit blocks of 17-bit
+symbols over all-zero bits, so every bit offset starts a valid symbol and the sync takes one round per subsequence.
+
+``defer_k_jpeg_decode`` (all three kernels) is timed with CUDA events as tools/jpeg_worst_case.py times it; one JSON line
+with the card and its power limit.
 
     python tools/jpeg_progressive_worst_case.py --reps 3
+    python tools/jpeg_progressive_worst_case.py --sync --reps 3
 """
 from __future__ import annotations
 
@@ -54,7 +60,16 @@ def refinement_stream(h: int, w: int) -> bytes:
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--sync", action="store_true", help="time the AC first self-synchronisation worst case")
     args = ap.parse_args()
+    if args.sync:
+        from jpeg_craft_progressive import worst_first
+        worst = worst_first(*BOUND, "gray", "ac")[0]
+        out = {"card": card(), "bound": f"{BOUND[0]}x{BOUND[1]}", "ac_first_bytes": jpeg.parse(worst).scans[1].length,
+               "slot_bytes": BOUND[0] * BOUND[1] * 3,
+               "ac_first_sync_1080x1920_x1": summary(*time_decode([worst], args.reps), [worst])}
+        print(json.dumps(out))
+        return
     from jpeg_bench import files as bench_files
     worst = refinement_stream(*BOUND)
     info = jpeg.parse(worst)
