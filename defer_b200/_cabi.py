@@ -24,6 +24,7 @@ OP_JPEG_DECODE = 13
 PRE_CAFFE, PRE_TF = 0, 1
 PRE_MODES = {"caffe": PRE_CAFFE, "tf": PRE_TF}
 RESIZE_SAMPLE_W, RESIZE_SAMPLE_H = 1, 2
+RESIZE_W, RESIZE_H = 4, 5      # fixed tables on the named axis, which may keep its length (a keep_aspect_ratio crop box)
 OK, ERR_INVALID, ERR_CUDA, ERR_TIMEOUT, ERR_STATE = 0, -1, -2, -3, -4
 
 FMT_NAMES = {FMT_F32: "f32", FMT_BF16X2: "bf16x2", FMT_BF16: "bf16"}

@@ -25,7 +25,7 @@ from typing import Dict, List, Optional
 import numpy as np
 
 from . import keras_like as K
-from .resize import INTERPOLATIONS, resize_image  # noqa: F401  (Keras load_img's resize, bit for bit as Pillow)
+from .resize import INTERPOLATIONS, resize_image  # noqa: F401  (Keras load_img's resize, keep_aspect_ratio too, as Pillow)
 from .jpeg import decode_jpeg  # noqa: F401  (Keras load_img's JPEG decode of baseline and progressive files, bit for bit as Pillow)
 from .keras_like import (Activation, Add, BatchNormalization, Conv2D, Dense, Flatten,
                          GlobalAveragePooling2D, Input, MaxPooling2D, Model, ZeroPadding2D)

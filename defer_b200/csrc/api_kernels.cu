@@ -129,7 +129,7 @@ int defer_k_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const in
   DEFER_CHECK(c == 3, "k_resize: the resize takes RGB images (3 channels), got %d", c);
   DEFER_CHECK((h_in != h_out) != (w_in != w_out), "k_resize: exactly one axis must change (%dx%d -> %dx%d)", h_in, w_in,
               h_out, w_out);
-  return launch_resize(x, y, bounds, taps, ksize, n, h_in, w_in, h_out, w_out, (cudaStream_t)stream);
+  return launch_resize(x, y, bounds, taps, ksize, n, h_in, w_in, h_out, w_out, w_in != w_out, (cudaStream_t)stream);
 }
 
 int defer_k_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,

@@ -191,10 +191,10 @@ int launch_f32_to_bf16(const float* x, void* y, size_t n, cudaStream_t st);
 int launch_preprocess(const uint8_t* x, const float* shift, float* y, size_t n_pix, cudaStream_t st);
 // Keras tf preprocess_input: uint8 RGB (n_pix pixels x 3) -> fp32 b / 127.5 - 1, channels kept (DEFER_PRE_TF)
 int launch_preprocess_tf(const uint8_t* x, float* y, size_t n_pix, cudaStream_t st);
-// Keras load_img resize, one axis (DEFER_OP_RESIZE): uint8 RGB (n, h_in, w_in, 3) -> (n, h_out, w_out, 3); the axis that
-// changes is the one resized (w_in != w_out: horizontal, else vertical).  bounds [out, 2] (first, count), taps [out, ksize].
+// Keras load_img resize, one axis (DEFER_OP_RESIZE): uint8 RGB (n, h_in, w_in, 3) -> (n, h_out, w_out, 3), resampling
+// the width (horiz) or the height; the other axis keeps its length.  bounds [out, 2] (first, count), taps [out, ksize].
 int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
-                  int w_in, int h_out, int w_out, cudaStream_t st);
+                  int w_in, int h_out, int w_out, bool horiz, cudaStream_t st);
 // Keras load_img resize of mixed sizes, one pass (DEFER_OP_RESIZE, pass = DEFER_RESIZE_SAMPLE_W | _H): each of the n
 // samples reads its size and tables from its int32 block in `tables` (layout: include/defer_b200.h).
 int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,

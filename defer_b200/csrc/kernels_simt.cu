@@ -1257,8 +1257,7 @@ __global__ void __launch_bounds__(256) resize_u8_kernel(const uint8_t* __restric
   }
 }
 int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int32_t* taps, int ksize, int n, int h_in,
-                  int w_in, int h_out, int w_out, cudaStream_t st) {
-  const bool horiz = w_in != w_out;
+                  int w_in, int h_out, int w_out, bool horiz, cudaStream_t st) {
   const size_t n_out = (size_t)n * h_out * w_out * (horiz ? 1 : 3);
   if (n_out == 0) return DEFER_OK;
   const unsigned grid = (unsigned)((n_out + 255) / 256);

@@ -204,6 +204,12 @@ static size_t elem_bytes(int elem, int fmt) {
 
 static size_t buf_bytes(const Buf& b, int fmt) { return b.elems * elem_bytes(b.elem, fmt); }
 
+// the axis of a fixed-table RESIZE op: named by modes W / H (it may keep its length under a crop box), else the one that
+// changes
+static bool resize_horizontal(const defer_op_desc& d, const Buf& bi, const Buf& bo) {
+  return d.mode == DEFER_RESIZE_W || (d.mode == 0 && bi.w != bo.w);
+}
+
 static int set_device(const defer_stage_s* s) {
   DEFER_CUDA(cudaSetDevice(s->cfg.device));
   return DEFER_OK;
@@ -285,13 +291,14 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
     case DEFER_OP_JPEG_DECODE:
       return launch_jpeg_decode((const uint8_t*)x, L.jpeg_blocks, nb, bi.h, bi.w, L.jpeg_ws, (uint8_t*)y, st);
     case DEFER_OP_RESIZE:
-      if (d.mode != 0) {
+      if (d.mode == DEFER_RESIZE_SAMPLE_W || d.mode == DEFER_RESIZE_SAMPLE_H) {
         const auto& f = s->frames;
         return launch_resize_frames(d.mode, (const uint8_t*)x, (uint8_t*)y, L.tables, nb, f.H, f.W, f.H_out, f.W_out, f.kw_w,
                                     f.kw_h, st);
       }
       return launch_resize((const uint8_t*)x, (uint8_t*)y, (const int32_t*)s->d_weights[d.w_scale],
-                           (const int32_t*)s->d_weights[d.w_kernel], d.kw, nb, bi.h, bi.w, bo.h, bo.w, st);
+                           (const int32_t*)s->d_weights[d.w_kernel], d.kw, nb, bi.h, bi.w, bo.h, bo.w,
+                           resize_horizontal(d, bi, bo), st);
   }
   set_error("launch_op: unknown op kind %d", d.kind);
   return DEFER_ERR_INVALID;
@@ -370,7 +377,8 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
       op.alg_flops = nb * bi.h * bi.w * bi.c;
       break;
     case DEFER_OP_RESIZE:   // + the two int32 tables
-      if (d.mode != 0) {    // an upper bound: every sample at the slot's size, plus its header and its axis' tables
+      if (d.mode == DEFER_RESIZE_SAMPLE_W || d.mode == DEFER_RESIZE_SAMPLE_H) {   // an upper bound: every sample at the
+                                                                                 // slot's size, its header and its axis' tables
         const int out_len = d.mode == DEFER_RESIZE_SAMPLE_W ? bo.w : bo.h;
         op.alg_bytes = in_b + out_b + nb * (2.0 + out_len * (2.0 + d.kw)) * 4.0;
         op.alg_flops = 2.0 * nb * bo.h * bo.w * bo.c * d.kw;
@@ -711,17 +719,18 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
           }
           break;
         }
-        if (d.mode != 0) {
-          set_error("op %d (resize): unknown mode %d (0, SAMPLE_W %d, SAMPLE_H %d)", i, d.mode, DEFER_RESIZE_SAMPLE_W,
-                    DEFER_RESIZE_SAMPLE_H);
+        if (d.mode != 0 && d.mode != DEFER_RESIZE_W && d.mode != DEFER_RESIZE_H) {
+          set_error("op %d (resize): unknown mode %d (0, SAMPLE_W %d, SAMPLE_H %d, W %d, H %d)", i, d.mode,
+                    DEFER_RESIZE_SAMPLE_W, DEFER_RESIZE_SAMPLE_H, DEFER_RESIZE_W, DEFER_RESIZE_H);
           return fail(DEFER_ERR_INVALID);
         }
-        if ((bi.h != bo.h) == (bi.w != bo.w) || d.in1 >= 0 || d.flags || d.w_shift >= 0) {
-          set_error("op %d (resize): exactly one axis must change (%dx%d -> %dx%d), no in1 / flags / w_shift", i, bi.h, bi.w,
-                    bo.h, bo.w);
+        if (d.in1 >= 0 || d.flags || d.w_shift >= 0 ||
+            (d.mode == 0 ? (bi.h != bo.h) == (bi.w != bo.w) : d.mode == DEFER_RESIZE_W ? bi.h != bo.h : bi.w != bo.w)) {
+          set_error("op %d (resize): mode 0 needs exactly one axis to change, mode W / H only its axis (%dx%d -> %dx%d, mode "
+                    "%d), no in1 / flags / w_shift", i, bi.h, bi.w, bo.h, bo.w, d.mode);
           return fail(DEFER_ERR_INVALID);
         }
-        const bool horiz = bi.w != bo.w;
+        const bool horiz = resize_horizontal(d, bi, bo);
         const int in_len = horiz ? bi.w : bi.h, out_len = horiz ? bo.w : bo.h, ksize = d.kw;
         if (ksize < 1 || d.w_scale < 0 || d.w_kernel < 0 || s->weight_bytes[d.w_scale] != (size_t)out_len * 2 * 4 ||
             s->weight_bytes[d.w_kernel] != (size_t)out_len * ksize * 4) {

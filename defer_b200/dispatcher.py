@@ -14,7 +14,7 @@ What changed underneath:
 
 Non-reference additions: ``close()`` / context manager (the reference can only be killed), keyword-only
 ``dtype``, ``depth`` (in-flight microbatches per stage), ``batch`` (samples per queue item; reference: 1),
-``coalesce``, ``preprocess``, ``image_size``, ``max_image_size``, ``interpolation`` and ``decode``.
+``coalesce``, ``preprocess``, ``image_size``, ``max_image_size``, ``interpolation``, ``keep_aspect_ratio`` and ``decode``.
 
 Preprocessing: the reference's driver runs Keras' ``preprocess_input`` on the host before every ``input_q.put``
 (``test/test.py:19-23``).  With ``preprocess="caffe"`` queue items are the uint8 images themselves
@@ -34,7 +34,10 @@ queue item is a uint8 image ``(batch, h, w, 3)`` of its own size with ``h <= H``
 share a microbatch, and each gives exactly what ``image_size=(h, w)`` would.  Only the image's own bytes cross PCIe.
 With ``decode="jpeg"`` as well, each queue item is a baseline JPEG file (``open(path, "rb").read()``); the first GPU
 decodes it exactly as ``load_img`` does with Pillow (``jpeg.decode_jpeg``), so only the compressed file crosses PCIe
-and the host only parses its markers.
+and the host only parses its markers.  ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``, and with
+``decode="jpeg"``) resizes each image's centred crop with the model input's aspect ratio instead of squashing the whole
+image, as ``load_img(..., keep_aspect_ratio=True)`` does: ``applications.resize_image(item, (H, W), interpolation,
+keep_aspect_ratio=True)``.
 
 Coalescing: the reference's queue items are single images and every node runs them one at a time
 (``src/node.py:103-108``), re-reading its weights per image.  Here up to ``coalesce`` in-flight queue items are
@@ -55,7 +58,7 @@ import numpy as np
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
 from .jpeg import check_decode, check_jpeg
-from .resize import check_frame, check_interpolation, check_size
+from .resize import check_frame, check_interpolation, check_keep_aspect_ratio, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
 
@@ -65,7 +68,8 @@ class DEFER:
                  coalesce: int = 1, linger_us: float = 200.0, conv_backend: int = 0, dist=None,
                  wait_timeout_ms: int = 0, max_inflight: int = 0, preprocess: Optional[str] = None,
                  image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
-                 max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None) -> None:
+                 max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
+                 keep_aspect_ratio: bool = False) -> None:
         check_decode(decode, preprocess, image_size, max_image_size)
         if decode is not None and batch not in (None, 1):
             raise ValueError(f"decode={decode!r}: a queue item is one JPEG file, so batch must be 1, got {batch}")
@@ -85,10 +89,12 @@ class DEFER:
             if image_size is not None:
                 raise ValueError(f"max_image_size={max_image_size} and image_size={image_size}: give one (image_size: "
                                  "every image has that size; max_image_size: each image has its own size up to that bound)")
+        keep_aspect_ratio = check_keep_aspect_ratio(keep_aspect_ratio, image_size, max_image_size)
         self.computeNodes = list(computeNodes)
         self.preprocess = preprocess        # None | "caffe" | "tf": uint8 queue items, preprocessed on stage 0's GPU
         self.image_size = image_size        # None | (h, w) of the uint8 queue items, resized on stage 0's GPU
         self.interpolation = interpolation
+        self.keep_aspect_ratio = keep_aspect_ratio  # resize Keras' centred crop of each image (load_img keep_aspect_ratio)
         self.max_image_size = max_image_size  # None | (H, W): uint8 queue items of any size up to it, resized on stage 0
         self.decode = decode                # None | "jpeg": queue items are JPEG files, decoded on stage 0
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
@@ -154,7 +160,8 @@ class DEFER:
                                          "image_size": self.image_size if i == 0 else None,
                                          "interpolation": self.interpolation,
                                          "max_image_size": self.max_image_size if i == 0 else None,
-                                         "decode": self.decode if i == 0 else None})
+                                         "decode": self.decode if i == 0 else None,
+                                         "keep_aspect_ratio": self.keep_aspect_ratio and i == 0})
             self.dist.wait_all_ready()      # the 1-byte ACK of dispatcher.py:64-65
             return
         runners = []
@@ -169,7 +176,8 @@ class DEFER:
                                       image_size=self.image_size if i == 0 else None,
                                       interpolation=self.interpolation,
                                       max_image_size=self.max_image_size if i == 0 else None,
-                                      decode=self.decode if i == 0 else None)
+                                      decode=self.decode if i == 0 else None,
+                                      keep_aspect_ratio=self.keep_aspect_ratio and i == 0)
             r.name = f"part{i+1}"
             runners.append(r)
         for i in range(n - 1):              # next hop = nodeIPs[i+1] (dispatcher.py:51-55)

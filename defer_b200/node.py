@@ -117,7 +117,7 @@ class StageRunner:
                    is_first: bool = True, is_last: bool = True, finalize: bool = True, preprocess: Optional[str] = None,
                    image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
                    max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
-                   **kw) -> "StageRunner":
+                   keep_aspect_ratio: bool = False, **kw) -> "StageRunner":
         """``preprocess="caffe"`` or ``"tf"`` (first stage only): inputs are uint8 RGB images ``(batch, h, w, 3)`` and the
         stage applies Keras' ``preprocess_input`` in that mode on the GPU (``"tf"`` for the ResNet V2 family).
         ``image_size=(h, w)`` (with ``preprocess``): inputs are uint8 RGB images of that size, resized on the GPU to the
@@ -126,9 +126,12 @@ class StageRunner:
         ``(H, W)``, each resized from its own size; feed them with ``submit_frames`` / ``predict_frames``.
         ``decode="jpeg"`` (with ``preprocess`` and ``max_image_size``): inputs are baseline JPEG files of images up to
         ``(H, W)``, decoded on the GPU as Keras' ``load_img`` does (``jpeg.decode_jpeg``); feed them with
-        ``submit_jpegs`` / ``predict_jpegs``."""
+        ``submit_jpegs`` / ``predict_jpegs``.
+        ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``): each image's centred crop with the model
+        input's aspect ratio is resized, as ``load_img(..., keep_aspect_ratio=True)`` does (``resize.keras_crop_box``)."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
-                          interpolation=interpolation, max_image_size=max_image_size, decode=decode)
+                          interpolation=interpolation, max_image_size=max_image_size, decode=decode,
+                          keep_aspect_ratio=keep_aspect_ratio)
         fmt = dtype if isinstance(dtype, int) else DTYPE_TO_FMT[dtype]
         r = cls(plan, device=parse_device(device), fmt=fmt, batch=max_batch, depth=depth, is_first=is_first,
                 is_last=is_last, name=model.name, **kw)
@@ -240,7 +243,8 @@ class StageRunner:
         if not 0 <= index <= self.batch - n:
             raise ValueError(f"{self.name}: {n} images from sample {index} do not fit the microbatch of {self.batch}")
         hw = np.array([im.shape[:2] for im in images], np.int32).reshape(n, 2)
-        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"])
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"],
+                                   self.frames.get("keep_aspect_ratio", False))
         self._tables[seq % self.depth] = (tables, hw, images)
         ptrs = (C.c_void_p * n)(*[im.__array_interface__["data"][0] for im in images])
         A.check(self.lib.defer_stage_submit_frames(self.handle, seq, index, n, ptrs, hw.ctypes.data, tables.ctypes.data,
@@ -271,7 +275,8 @@ class StageRunner:
         if not 1 <= n <= self.batch - index or index < 0:
             raise ValueError(f"{self.name}: {n} files from sample {index} do not fit the microbatch of {self.batch}")
         hw = np.array([(i.h, i.w) for i in infos], np.int32).reshape(n, 2)
-        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"])
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"],
+                                   self.frames.get("keep_aspect_ratio", False))
         nr = tables.shape[1]
         blocks = np.zeros((n, nr + BLOCK_INTS), np.int32)      # only the prefix each file uses is written and copied
         blocks[:, :nr] = tables
@@ -473,7 +478,8 @@ class Node:
                                        image_size=msg.get("image_size") if rank == 0 else None,
                                        interpolation=msg.get("interpolation", "nearest"),
                                        max_image_size=msg.get("max_image_size") if rank == 0 else None,
-                                       decode=msg.get("decode") if rank == 0 else None)
+                                       decode=msg.get("decode") if rank == 0 else None,
+                                       keep_aspect_ratio=msg.get("keep_aspect_ratio", False) if rank == 0 else False)
         ns.model = runner                               # src/node.py:38
         self.runner = runner
         # wire the hop: my consumer gives me its input-side token, I give it my output-side token

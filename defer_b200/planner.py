@@ -25,6 +25,10 @@ With ``max_image_size=(H, W)`` instead, the stage input is a uint8 slot of that 
 (``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.  With
 ``decode="jpeg"`` as well, the stage input is a byte slot of ``H * W * 3`` per sample holding one JPEG file, and a
 ``JPEG_DECODE`` op in front of the resize pair decodes it into the uint8 slot (``jpeg.pack_block``).
+``keep_aspect_ratio=True`` resizes Keras' centred crop of each image instead (``resize.keras_crop_box``): with
+``image_size`` the two ``RESIZE`` ops carry box tables, and an axis that keeps its length under a partial box is
+resampled by an op whose ``mode`` names its axis (``RESIZE_W`` / ``_H``); with ``max_image_size`` the feeder packs each
+image's box tables (``Plan.frames["keep_aspect_ratio"]``).
 """
 from __future__ import annotations
 
@@ -37,7 +41,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
 from .jpeg import check_decode
-from .resize import check_interpolation, check_size, kcap, resize_tables
+from .resize import check_interpolation, check_keep_aspect_ratio, check_size, crop_boxes, kcap, resize_tables
 
 
 def same_pad(size: int, k: int, s: int) -> Tuple[int, int]:
@@ -80,7 +84,8 @@ class Plan:
     output_shape: Tuple[int, ...]
     tensor_buf: Dict[str, int]                        # layer name -> buffer id holding its output (if materialised)
     # max_image_size=: {"max_image_size": (H, W), "target": (H_out, W_out), "kw": (kw_w, kw_h), "interpolation": name},
-    # what the stage's feeder needs to pack each image's table block (resize.pack_frame_tables); None otherwise
+    # plus "keep_aspect_ratio": True when that is on, what the stage's feeder needs to pack each image's table block
+    # (resize.pack_frame_tables); None otherwise
     frames: Optional[dict] = None
     # decode="jpeg": the stage takes JPEG files (each with its jpeg.pack_block block after its table block); None otherwise
     decode: Optional[str] = None
@@ -104,7 +109,8 @@ def _hwc(shape) -> Tuple[int, int, int]:
 
 def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Optional[str] = None,
                image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
-               max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None) -> Plan:
+               max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
+               keep_aspect_ratio: bool = False) -> Plan:
     check_decode(decode, preprocess, image_size, max_image_size)
     if preprocess is not None:
         check_preprocess(preprocess)
@@ -125,6 +131,7 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         if image_size is not None:
             raise ValueError(f"max_image_size={max_image_size} and image_size={image_size}: give one (image_size: every "
                              "image has that size; max_image_size: each image has its own size up to that bound)")
+    keep = check_keep_aspect_ratio(keep_aspect_ratio, image_size, max_image_size)
     nodes = list(model.iter_nodes())
     # names as recorded at map time (tensor histories may be re-tagged later by Input(tensor=...))
     order = [l.name for l, _ in nodes]
@@ -229,20 +236,28 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
                               layers=[f"load_img(decode {decode} <={h}x{w})"])).out
         if max_image_size is not None:
             # images of mixed sizes up to (h, w): both passes always, the tables come with each image
+            # a crop box's scale is at most the axis' own, so kcap bounds the taps with keep_aspect_ratio as well
             kw = (kcap(w, W, interpolation), kcap(h, H, interpolation))
+            how = interpolation + (", keep_aspect_ratio" if keep else "")
             op_w = emit(PlanOp(A.OP_RESIZE, img, new_buf((None, h, W, 3), A.BUF_U8), kw=kw[0], mode=A.RESIZE_SAMPLE_W,
-                               layers=[f"load_img(width <={w}->{W}, {interpolation})"]))
+                               layers=[f"load_img(width <={w}->{W}, {how})"]))
             img = emit(PlanOp(A.OP_RESIZE, op_w.out, new_buf((None, H, W, 3), A.BUF_U8), kw=kw[1], mode=A.RESIZE_SAMPLE_H,
-                              layers=[f"load_img(height <={h}->{H}, {interpolation})"])).out
+                              layers=[f"load_img(height <={h}->{H}, {how})"])).out
             frames = {"max_image_size": (h, w), "target": (H, W), "kw": kw, "interpolation": interpolation}
-        # Pillow resizes the width first and skips an axis whose size does not change (so does Keras: no resize at all
-        # when the image is already at target_size)
-        for axis, n_in, n_out, shape in (("width", w, W, (h, W, 3)), ("height", h, H, (H, W, 3))):
-            if n_in == n_out or frames is not None:
+            if keep:
+                frames["keep_aspect_ratio"] = True
+        # Pillow resizes the width first and skips an axis whose size does not change and whose box is the whole axis
+        # (so does Keras: no resize at all when the image is already at target_size).  An axis that keeps its size under
+        # a partial box is resampled; its op names the axis in `mode`, as its shapes cannot.
+        box_w, box_h = crop_boxes(h, w, (H, W), keep)
+        for axis, n_in, n_out, shape, box in (("width", w, W, (h, W, 3), box_w), ("height", h, H, (H, W, 3), box_h)):
+            if (n_in == n_out and box is None) or frames is not None:
                 continue
-            first, count, coef = resize_tables(n_in, n_out, interpolation)
-            op = emit(PlanOp(A.OP_RESIZE, img, new_buf((None,) + shape, A.BUF_U8), kw=coef.shape[1],
-                             layers=[f"load_img({axis} {n_in}->{n_out}, {interpolation})"]))
+            first, count, coef = resize_tables(n_in, n_out, interpolation, box)
+            crop = "" if box is None else f" box {box[0]}..{box[1]}"
+            mode = 0 if n_in != n_out else (A.RESIZE_W if axis == "width" else A.RESIZE_H)
+            op = emit(PlanOp(A.OP_RESIZE, img, new_buf((None,) + shape, A.BUF_U8), kw=coef.shape[1], mode=mode,
+                             layers=[f"load_img({axis} {n_in}->{n_out}{crop}, {interpolation})"]))
             op.w_scale = add_table(np.stack([first, count], axis=1))
             op.w_kernel = add_table(coef)
             img = op.out

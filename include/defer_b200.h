@@ -74,6 +74,7 @@ typedef enum defer_op_kind {
                          /*   w_kernel = [out_len, kw] fixed-point taps, 22 fractional bits;  kw = ksize          */
                          /*   y[i] = clamp((2^21 + sum_{k < count} x[first + k] * tap[k]) >> 22, 0, 255) per     */
                          /*   channel; 0 <= first, 1 <= count <= kw, first + count <= in_len (checked at create)  */
+                         /* `mode` DEFER_RESIZE_W / _H: the same on the named axis, which may keep its length    */
                          /* `mode` DEFER_RESIZE_SAMPLE_W / _H: images of mixed sizes, tables per sample (below)   */
   DEFER_OP_JPEG_DECODE = 13 /* baseline JPEG files -> images (below): in0 = the stage input, a DEFER_BUF_JPEG (H, W, 3)    */
                          /*   slot per sample; out = U8 (H, W, 3), each image packed (h, w, 3) at the start of its sample;  */
@@ -95,6 +96,11 @@ typedef enum defer_op_kind {
  * planned, even when an axis of the bound already equals the target, as the axis cannot be told from the shapes then. */
 #define DEFER_RESIZE_SAMPLE_W 1
 #define DEFER_RESIZE_SAMPLE_H 2
+/* Modes W / H: mode 0's fixed tables on the named axis, the other axis keeping its length.  The named axis may keep its
+ * length too: Keras' load_img(keep_aspect_ratio=True) resamples an axis of the target's length when its crop box does
+ * not cover it (Pillow's resize with box=), which mode 0 cannot tell from the shapes. */
+#define DEFER_RESIZE_W 4
+#define DEFER_RESIZE_H 5
 
 /* DEFER_OP_JPEG_DECODE decodes each sample's JPEG file on the GPU, bit for bit as libjpeg-turbo 3.1 does through Pillow
  * (defer_b200/jpeg.py restates it).  It is planned before the DEFER_RESIZE_SAMPLE_W / _H pair, whose table blocks keep

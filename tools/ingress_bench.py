@@ -27,12 +27,14 @@ device time of the fp32 fused stem, the uint8 fused stem of the mode and its sta
 L2 flushed), the host time of one preprocessing call, and the card's name and power limit (read-only nvidia-smi query);
 with --image-size also the host time of one Pillow resize and the time_op of each RESIZE op at 32 frames; with
 --mixed-sizes the time_op of the two per-sample RESIZE ops at 32 mixed frames and at 32 frames of the first size (under
-a bound of that size), and arm f's H2D bytes per item (the image's own bytes plus its table block).
+a bound of that size), and arm f's H2D bytes per item (the image's own bytes plus its table block).  With --crop-sizes
+HxW,HxW,... the time_op of each RESIZE op at 32 frames of each size, with keep_aspect_ratio off and on (the crop arm).
 
     python tools/ingress_bench.py [--model resnet50 --preprocess caffe] [--items 640] [--reps 3]
     python tools/ingress_bench.py --model resnet50v2 --preprocess tf
     python tools/ingress_bench.py --image-size 480x640 --interpolation bilinear
     python tools/ingress_bench.py --image-size 480x640 --mixed-sizes 480x640,720x1280,1080x1920
+    python tools/ingress_bench.py --crop-sizes 480x640,640x480,1080x1920,1920x1080 --interpolation bilinear
 """
 from __future__ import annotations
 
@@ -155,10 +157,10 @@ def pillow_resize(size, interpolation):
     return fn
 
 
-def resize_times(model, mode, image_size, interpolation, iters):
+def resize_times(model, mode, image_size, interpolation, iters, keep_aspect_ratio=False):
     """time_op (us) of each RESIZE op at the benchmarked microbatch (32 frames), L2 flushed."""
     r = StageRunner.from_model(model, device=0, dtype="float32", max_batch=G, depth=1, preprocess=mode,
-                               image_size=image_size, interpolation=interpolation)
+                               image_size=image_size, interpolation=interpolation, keep_aspect_ratio=keep_aspect_ratio)
     out = {}
     try:
         r.predict(applications.synthetic_image(G, image_size + (3,), seed=1))
@@ -207,6 +209,8 @@ def main():
     ap.add_argument("--image-size", default=None, help="HxW of uint8 frames for arms d and e, e.g. 480x640")
     ap.add_argument("--interpolation", choices=applications.INTERPOLATIONS, default="nearest")
     ap.add_argument("--mixed-sizes", default=None, help="HxW,HxW,... of uint8 frames for arm f, e.g. 480x640,720x1280")
+    ap.add_argument("--crop-sizes", default=None,
+                    help="HxW,HxW,...: time the RESIZE ops of each size with keep_aspect_ratio off and on, then exit")
     args = ap.parse_args()
     if args.reps < 3:
         ap.error("--reps must be >= 3")
@@ -226,6 +230,20 @@ def main():
         bound = (max(h for h, _ in mixed), max(w for _, w in mixed))
 
     model = MODELS[args.model]()
+    if args.crop_sizes:
+        try:
+            crops = [parse_size(v) for v in args.crop_sizes.split(",")]
+        except ValueError:
+            ap.error(f"--crop-sizes {args.crop_sizes!r}: expected HxW,HxW,..., e.g. 480x640,1080x1920")
+        res = {"metric": f"{args.model}_resize_time_op_us", "preprocess": args.preprocess, "frames": G,
+               "interpolation": args.interpolation,
+               "crop_time_op": {f"{h}x{w}": {k: resize_times(model, args.preprocess, (h, w), args.interpolation,
+                                                             args.op_iters, keep_aspect_ratio=keep)
+                                             for k, keep in (("off", False), ("keep_aspect_ratio", True))}
+                                for h, w in crops}}
+        res.update(card())
+        print(json.dumps(res), flush=True)
+        return
     host_fn = HOST_PREPROCESS[args.preprocess]
     imgs = [applications.synthetic_image(1, seed=i) for i in range(args.items)]
     pre = [host_fn(x) for x in imgs]
