@@ -7,10 +7,13 @@ triangular upsampling, fixed-point YCbCr->RGB of ``jdcolor.c``).  Other libjpeg 
 differently and can give other pixels.
 
 That holds while every output of the IDCT stays within +-512 of 128, as it does for the blocks encoders write from 8-bit
-images.  Beyond that range the samples are defined by ``jidctint.c``: the output wraps to 10 bits before the clamp to
-0..255 (``idct_range_limit[x & 1023]``), so 128 + 1100 gives 204, not 255.  Only hand-made or corrupt files get there
-(large coefficients or quantisers), and there no single Pillow result exists: libjpeg-turbo's SIMD IDCT, which Pillow
-uses on x86, does not wrap, while a build without SIMD runs ``jidctint.c``.
+images.  Beyond that range the samples are those of libjpeg's C code: ``jidctint.c`` wraps each output to 10 bits
+before the clamp to 0..255 (``idct_range_limit[x & 1023]``), so 128 + 1100 gives 204, not 255, and coefficients are
+int16 as ``jdhuff.c`` / ``jdphuff.c`` store them (a DC predictor past 32767, ``v << Al`` of a first scan).  Only
+hand-made or corrupt files get there (large coefficients or quantisers).  There the decode equals Pillow whose
+libjpeg-turbo 3.1 runs its C path (``JSIMD_FORCENONE=1``, or a build without SIMD), checked against libjpeg-turbo 3.1's
+C path on files that cross every edge of the wrap and the clamp (tests/test_jpeg_idct_range_host.py); Pillow's default
+on x86, the SIMD IDCT, saturates instead of wrapping and gives other pixels.
 
 The feeder only walks the markers (``parse``) and decodes no Huffman code: past the scan header, byte searches find the
 EOI that ends the entropy-coded data.  Tables derived from DQT and DHT segments are memoised on the segment bytes,

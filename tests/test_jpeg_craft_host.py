@@ -6,8 +6,8 @@
   intervals of one MCU and of more than one MCU row, and the stream of all-zero bits, whose blocks are 127 bits each.
   The coefficients come from a forward DCT of 8-bit blocks, so any encoder may emit them.
 - 0xFF fill bytes before every RSTn marker decode as Pillow does.
-- Out of range, ``jpeg.idct_islow`` wraps as jidctint.c's ``idct_range_limit[x & 1023]``: checked against hand-computed
-  values, not against Pillow, whose SIMD IDCT does not wrap.
+- Out of range, ``jpeg.idct_islow`` wraps as jidctint.c's ``idct_range_limit[x & 1023]``: a few hand-computed values
+  here; tests/test_jpeg_idct_range_host.py checks the whole out-of-range decode against libjpeg-turbo 3.1's C path.
 - The closed form of the rounds of the self-synchronising decode on files whose every bit position decodes (the worst
   case the GPU tests use) equals ``jpeg_check.sync_stats`` at 8, 32 and the device's subsequence size.
 """

@@ -36,7 +36,7 @@ def test_valid_edges_decode_as_written_and_as_pillow(case):
     assert st["progress"]["scans"] == len(st["info"].scans) and st["progress"]["cutoff"] == len(st["coef"])
     assert np.array_equal(st["coef"], want), name
     raw = idct_raw(st["coef"].astype(np.int64), np.ones(64, np.int64))
-    if np.abs(raw).max() > 512:                  # beyond the IDCT range no single Pillow result exists (jpeg.py)
+    if np.abs(raw).max() > 512:      # beyond the IDCT range: against the C path in test_jpeg_idct_range_host.py
         assert name.startswith("al 13")
         return
     Image = pytest.importorskip("PIL.Image")
