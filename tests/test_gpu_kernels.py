@@ -19,7 +19,8 @@ def torch_cuda():
     return torch, lib
 
 
-# the distinct conv shapes of ResNet50 at batch 1 (SURVEY.md 8d) + batch / edge variants
+# most of ResNet50's distinct conv shapes at batch 1 (SURVEY.md 8d; not res4a_branch1) + batch / edge variants.  The
+# complete list of the applications' conv geometries, derived from their plans, is tests/app_convs.py
 RESNET_SHAPES = [
     # n, h, w, cin, cout, k, s, pad
     (1, 56, 56, 64, 64, 1, 1, 0), (1, 56, 56, 64, 64, 3, 1, 1), (1, 56, 56, 64, 256, 1, 1, 0),
