@@ -23,27 +23,36 @@ _HDR_WORDS = 16     # uint64 header: [0] submitted, [1] stop, [2] done (publishe
 
 
 class DistContext:
-    def __init__(self, backend: Optional[str] = None, ring: int = 64, out_elems: int = 1000, batch: int = 1):
+    """``device``: the GPU this rank's stage runs on (default: its local rank).  Ranks that share a GPU (CUDA IPC works
+    between processes on one device) need ``backend="gloo"``: NCCL refuses two ranks on one device."""
+
+    def __init__(self, backend: Optional[str] = None, ring: int = 64, out_elems: int = 1000, batch: int = 1,
+                 device: Optional[int] = None):
         import torch
         import torch.distributed as dist
         self.torch, self.dist = torch, dist
         self.rank = int(os.environ.get("RANK", "0"))
         self.world = int(os.environ.get("WORLD_SIZE", "1"))
         self.local_rank = int(os.environ.get("LOCAL_RANK", str(self.rank)))
+        self.device = self.local_rank if device is None else int(device)
         self.ring = int(ring)
         self.out_elems = int(out_elems) * int(batch)
         self._runner = None
         self._owns_group = False
         # a gloo-only world may have more ranks than the host has GPUs: those ranks stay on the CPU
-        self.cuda = torch.cuda.is_available() and self.local_rank < torch.cuda.device_count()
+        self.cuda = torch.cuda.is_available() and self.device < torch.cuda.device_count()
         if not dist.is_initialized():
             use_cuda = self.cuda
             if backend is None:
                 backend = "cpu:gloo,cuda:nccl" if use_cuda else "gloo"
             if use_cuda:
-                torch.cuda.set_device(self.local_rank)
+                torch.cuda.set_device(self.device)
             dist.init_process_group(backend=backend, rank=self.rank, world_size=self.world)
             self._owns_group = True
+        else:
+            backend = str(dist.get_backend())
+        # collectives run on the GPU only where NCCL carries them; under gloo they stay on the host
+        self.nccl = self.cuda and "nccl" in str(backend)
         # control block in POSIX shared memory (single node by construction: NVLink domain of one box)
         port = os.environ.get("MASTER_PORT", "0")
         self.shm_name = f"defer_b200_{port}_{os.environ.get('TORCHELASTIC_RUN_ID', 'x')}"[:60]
@@ -68,15 +77,15 @@ class DistContext:
     # ------------------------------------------------------------------ collectives (control plane only)
     def barrier(self):
         if self.world > 1:
-            if self.cuda:
-                self.dist.barrier(device_ids=[self.local_rank])
+            if self.nccl:
+                self.dist.barrier(device_ids=[self.device])
             else:
                 self.dist.barrier()
 
     def max_over_ranks(self, value: float) -> float:
         if self.world == 1:
             return float(value)
-        dev = f"cuda:{self.local_rank}" if self.cuda else "cpu"
+        dev = f"cuda:{self.device}" if self.nccl else "cpu"
         t = self.torch.tensor([float(value)], dtype=self.torch.float64, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.MAX)
         return float(t.item())
@@ -84,7 +93,7 @@ class DistContext:
     def sum_over_ranks(self, value: float) -> float:
         if self.world == 1:
             return float(value)
-        dev = f"cuda:{self.local_rank}" if self.cuda else "cpu"
+        dev = f"cuda:{self.device}" if self.nccl else "cpu"
         t = self.torch.tensor([float(value)], dtype=self.torch.float64, device=dev)
         self.dist.all_reduce(t, op=self.dist.ReduceOp.SUM)
         return float(t.item())

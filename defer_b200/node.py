@@ -468,7 +468,7 @@ class Node:
         ctx = self.ctx
         ns = self.state = NodeState(chunk_size=512 * 1000)  # src/node.py:111 (kept for interface parity)
         msg = self._receive_stage(ns)
-        dev = self.device if self.device is not None else ctx.local_rank
+        dev = self.device if self.device is not None else ctx.device
         rank, world = ctx.rank, ctx.world
         runner = StageRunner.from_wire(msg["json"], ns.weights, device=dev, dtype=msg["fmt"], max_batch=msg["batch"],
                                        depth=msg["depth"], is_first=(rank == 0), is_last=(rank == world - 1),

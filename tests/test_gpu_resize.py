@@ -3,12 +3,8 @@
 The contract: a uint8 image of `image_size` in a resizing pipeline gives exactly the result of
 `applications.resize_image(image, model input, interpolation)` in the same pipeline without the option - for
 `defer_k_resize` alone, for the `RESIZE` ops of a stage in both preprocessing modes, dtypes and stem paths, and for
-`DEFER` end to end over one and two stages and one process per GPU.  Run as a script under torchrun, this file is the
-worker of the one-process-per-GPU test."""
-import os
+`DEFER` end to end over one and two stages (one process per GPU: the `image-size` case of tests/test_gpu_dist.py)."""
 import queue
-import socket
-import subprocess
 import sys
 import threading
 from pathlib import Path
@@ -237,79 +233,3 @@ def test_resnet50v2_defer_frames_tf_bilinear(monkeypatch):
     y0, _, _ = _run_defer(m, [resize_image(x, (224, 224), "bilinear") for x in items], 1, preprocess="tf")
     assert kernels[:2] == ["resize_u8_kernel"] * 2
     assert np.array_equal(_bits(y), _bits(y0))
-
-
-# ------------------------------------------------------------------------------------------------ one process per GPU
-def _n_gpus():
-    try:
-        return A.device_count()
-    except Exception:
-        return 0
-
-
-def test_one_process_per_gpu_with_image_size():
-    if _n_gpus() < 2:
-        pytest.skip("needs 2 GPUs")
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    env = dict(os.environ)
-    env.pop("CUDA_VISIBLE_DEVICES", None)
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), str(Path(__file__).resolve())]
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=540, env=env, cwd=str(ROOT))
-    assert r.returncode == 0 and "RESIZE_DIST_OK" in r.stdout, r.stdout[-3000:] + "\n--- stderr ---\n" + r.stderr[-3000:]
-
-
-def _dist_worker():
-    """Every rank runs `Node.run`; rank 0 is also the dispatcher and checks each result against one stage on its GPU fed
-    the host-resized image, bitwise."""
-    A.load()
-    import torch
-    from defer_b200.dispatcher import DEFER
-    from defer_b200.dist import DistContext
-    from defer_b200.node import Node, StageRunner
-    rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    G, n_items = 4, 10
-    torch.cuda.set_device(local_rank)
-    ctx = DistContext(ring=64, out_elems=1000, batch=G)
-    node = Node(dist_ctx=ctx, device=local_rank)
-    nt = threading.Thread(target=node.run, daemon=True)
-    nt.start()
-    ok = True
-    if rank == 0:
-        model = applications.ResNet50()
-        defer = DEFER(list(range(world)), depth=3, coalesce=G, linger_us=2000, dist=ctx, wait_timeout_ms=20000,
-                      preprocess="caffe", image_size=(480, 640), interpolation="bilinear")
-        in_q, out_q = queue.Queue(), queue.Queue()
-        t = threading.Thread(target=defer.run_defer, args=(model, applications.default_cuts(model, world), in_q, out_q),
-                             daemon=True)
-        t.start()
-        assert defer.wait_ready(600), "pipeline did not come up"
-        frames = _frames(n_items, 480, 640, seed=51)
-        for i in range(n_items):
-            in_q.put(frames[i:i + 1])
-        outs = [out_q.get(timeout=120) for _ in range(n_items)]
-        single = StageRunner.from_model(model, device=local_rank, max_batch=G, depth=1, preprocess="caffe")
-        try:
-            for g in range(0, n_items, G):
-                group = resize_image(frames[g:g + G], (224, 224), "bilinear")
-                group = np.concatenate([group] + [group[:1]] * (G - len(group)))
-                want = single.predict(group)
-                for i in range(min(G, n_items - g)):
-                    if not np.array_equal(outs[g + i], want[i:i + 1]):
-                        ok = False
-                        print(f"item {g + i}: differs from one stage fed the host-resized image", flush=True)
-        finally:
-            single.close()
-        defer.close()
-        t.join(timeout=30)
-    ctx.shutdown(nt)
-    if rank == 0:
-        print("RESIZE_DIST_OK" if ok else "RESIZE_DIST_FAIL", flush=True)
-        sys.exit(0 if ok else 1)
-
-
-if __name__ == "__main__":
-    _dist_worker()

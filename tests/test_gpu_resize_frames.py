@@ -3,16 +3,11 @@
 The contract: each uint8 image of its own size up to the bound gives exactly `applications.resize_image(image, model
 input, interpolation)` fed to the same pipeline without the option - for `defer_k_resize_frames` against the numpy
 restatement of the kernel, for the two per-sample RESIZE ops of a stage in both preprocessing modes, dtypes and stem paths,
-after re-use of a lane, and for `DEFER` end to end over one and two stages and one process per GPU.  Run as a script under
-torchrun, this file is the worker of the one-process-per-GPU test."""
+after re-use of a lane, and for `DEFER` end to end over one and two stages (one process per GPU: the `max-image-size` case
+of tests/test_gpu_dist.py)."""
 import copy
 import ctypes as C
-import os
-import socket
-import subprocess
 import sys
-import threading
-import queue
 from pathlib import Path
 
 import numpy as np
@@ -287,74 +282,3 @@ def test_resnet50v2_defer_mixed_frames_tf_bilinear(monkeypatch):
     y0, _, _ = _run_defer(m, [resize_image(x, (224, 224), "bilinear") for x in items], 1, preprocess="tf")
     assert kernels[:2] == ["resize_frames_u8_kernel"] * 2
     assert np.array_equal(_bits(y), _bits(y0))
-
-
-# ------------------------------------------------------------------------------------------------ one process per GPU
-def test_one_process_per_gpu_with_max_image_size():
-    from test_gpu_resize import _n_gpus
-    if _n_gpus() < 2:
-        pytest.skip("needs 2 GPUs")
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    env = dict(os.environ)
-    env.pop("CUDA_VISIBLE_DEVICES", None)
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), str(Path(__file__).resolve())]
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=540, env=env, cwd=str(ROOT))
-    assert r.returncode == 0 and "FRAMES_DIST_OK" in r.stdout, r.stdout[-3000:] + "\n--- stderr ---\n" + r.stderr[-3000:]
-
-
-def _dist_worker():
-    """Every rank runs `Node.run`; rank 0 is also the dispatcher and checks each result against one stage on its GPU fed
-    the host-resized images, bitwise."""
-    sys.path.insert(0, str(Path(__file__).resolve().parent))
-    A.load()
-    import torch
-    from defer_b200.dispatcher import DEFER
-    from defer_b200.dist import DistContext
-    from defer_b200.node import Node, StageRunner
-    rank, world, local_rank = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    G, n_items = 4, 10
-    torch.cuda.set_device(local_rank)
-    ctx = DistContext(ring=64, out_elems=1000, batch=G)
-    node = Node(dist_ctx=ctx, device=local_rank)
-    nt = threading.Thread(target=node.run, daemon=True)
-    nt.start()
-    ok = True
-    if rank == 0:
-        model = applications.ResNet50()
-        defer = DEFER(list(range(world)), depth=3, coalesce=G, linger_us=2000, dist=ctx, wait_timeout_ms=20000,
-                      preprocess="caffe", max_image_size=(720, 1280), interpolation="bilinear")
-        in_q, out_q = queue.Queue(), queue.Queue()
-        t = threading.Thread(target=defer.run_defer, args=(model, applications.default_cuts(model, world), in_q, out_q),
-                             daemon=True)
-        t.start()
-        assert defer.wait_ready(600), "pipeline did not come up"
-        items = _items(n_items, seed=51)
-        for x in items:
-            in_q.put(x)
-        outs = [out_q.get(timeout=120) for _ in range(n_items)]
-        single = StageRunner.from_model(model, device=local_rank, max_batch=G, depth=1, preprocess="caffe")
-        try:
-            for g in range(0, n_items, G):
-                group = np.concatenate([resize_image(x, (224, 224), "bilinear") for x in items[g:g + G]])
-                group = np.concatenate([group] + [group[:1]] * (G - len(group)))
-                want = single.predict(group)
-                for i in range(min(G, n_items - g)):
-                    if not np.array_equal(outs[g + i], want[i:i + 1]):
-                        ok = False
-                        print(f"item {g + i}: differs from one stage fed the host-resized image", flush=True)
-        finally:
-            single.close()
-        defer.close()
-        t.join(timeout=30)
-    ctx.shutdown(nt)
-    if rank == 0:
-        print("FRAMES_DIST_OK" if ok else "FRAMES_DIST_FAIL", flush=True)
-        sys.exit(0 if ok else 1)
-
-
-if __name__ == "__main__":
-    _dist_worker()
