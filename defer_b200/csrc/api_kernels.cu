@@ -31,7 +31,7 @@ int defer_k_conv(int fmt, int backend, const void* x, int x_is_f32, const float*
                                /*mega=*/backend == 3, stream_bn);
     args.direct_out = backend >= 6;
     if (rc == DEFER_OK) rc = umma_conv_bind(plan, &args, x, residual, y);
-    const int n_tiles = plan.tiles_n * plan.tiles_h * plan.tiles_w * (cout / plan.bn);
+    const int n_tiles = plan.m_tiles * (cout / plan.bn);
     if (backend == 2) {
       if (rc == DEFER_OK) rc = launch_conv_umma(plan, args, st);
     } else {

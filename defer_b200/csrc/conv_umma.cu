@@ -3,10 +3,13 @@
 // The contraction of every Conv2D whose C_in is a multiple of 64 (all ResNet / VGG convs but the
 // RGB stem).  GEMM view: M = output pixels, N = C_out, K = taps x C_in.
 //
-//   * A (activations, NHWC bf16 planes) is never im2col'ed: for tap (kh, kw) the 128-row A tile is a
-//     4-D TMA box {64 channels, tile_w, tile_h, tile_n} of the input tensor shifted by (kh-pad, kw-pad);
-//     TMA zero-fills out-of-bounds elements, which IS the 'same' / ZeroPadding2D border, and its
-//     element strides do stride-2 sub-sampling.  1x1/stride-1 convs use the flat [M, C] view.
+//   * A (activations, NHWC bf16 planes) is never im2col'ed in memory: TMA does it.  M tile t is the 128
+//     consecutive output pixels [128 t, 128 t + 128) in (n, ho, wo) order, across rows and images.  For tap
+//     (kh, kw) and a 64-channel block its A tile is one im2col load: the pixel walk starts at the input corner of
+//     the tile's first output pixel and steps by the conv stride through a bounding box whose corners are the
+//     padding, and each pixel is read at the tap offset (kw, kh) from its corner.  TMA zero-fills out-of-bounds
+//     pixels, which IS the 'same' / ZeroPadding2D border and the rows past the batch.  1x1/stride-1 convs load
+//     the flat [M, C] view with a tiled load instead.
 //   * B (weights) is pre-arranged once as [tap][C_out][C_in] bf16 (K-major), a 3-D TMA box.
 //   * Both land in 128B-swizzled shared memory (a ring of stages guarded by mbarriers) and feed
 //     wgmma.mma_async m64nBNk16 issued by two consumer warpgroups (rows 0-63 and 64-127 of the tile);
@@ -59,8 +62,8 @@ constexpr int STG_BYTES = BM * STG_COLS * 4;   // 32 KB, after the operand ring
 struct KParams {
   // geometry
   int n, ho, wo, cout;
-  int tile_n, tile_h, tile_w, tiles_h, tiles_w;   // M tile = tile_n x tile_h x tile_w output pixels
-  int flat;                                       // flat [M, C] view: rows = consecutive pixels
+  int tile_h, tile_w, tiles_h, tiles_w;           // fused stem: M tile = tile_h x tile_w pixels of one image
+  int im2col;                                     // A tile: 1 = im2col load, 0 = tiled load of the [M, C] view
   int m_total;                                    // n*ho*wo
   int kh, kw, sh, sw, pad_t, pad_l;
   int cblocks;                                    // cin / 64
@@ -176,6 +179,15 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// im2col load: (c0, w, h, n) is the input corner of the first pixel of the walk, (ow, oh) the tap offset of every pixel
+__device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int w, int h,
+                                                   int n, uint16_t ow, uint16_t oh) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
+      "[%2], {%7, %8};"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh)
+      : "memory");
+}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -270,20 +282,19 @@ __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t a, uint
       : "l"(a), "l"(b), "r"(1));
 }
 
-// accumulator row r of the tile at (n0, h0, w0) -> output pixel (linear NHW index) and whether it exists
+// accumulator row r of the tile at (n0, h0, w0) -> output pixel (linear NHW index) and whether it exists.  A conv tile
+// starts at pixel w0; a fused stem tile (STEM) is tile_h x tile_w pixels of image n0.
+template <bool STEM>
 __device__ __forceinline__ void row_to_pixel(const KParams& p, int r, int n0, int h0, int w0, bool& valid, size_t& pix) {
-  if (p.flat) {
+  if (!STEM) {
     const int m = w0 + r;
     valid = m < p.m_total;
     pix = (size_t)m;
   } else {
-    const int tw = r % p.tile_w;
-    const int t2 = r / p.tile_w;
-    const int th = t2 % p.tile_h;
-    const int tn = t2 / p.tile_h;
-    const int nn = n0 + tn, oh = h0 + th, ow = w0 + tw;
-    valid = (tn < p.tile_n) && nn < p.n && oh < p.ho && ow < p.wo;
-    pix = ((size_t)nn * p.ho + oh) * p.wo + ow;
+    const int th = r / p.tile_w;
+    const int oh = h0 + th, ow = w0 + r % p.tile_w;
+    valid = th < p.tile_h && oh < p.ho && ow < p.wo;
+    pix = ((size_t)n0 * p.ho + oh) * p.wo + ow;
   }
 }
 
@@ -356,7 +367,7 @@ __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 
 // what eltwise_kernel<FMT, DEFER_OP_AFFINE> reads back - with the same fmaf, ReLU and split, into y2.  The folded result is
 // therefore bit-identical to the conv followed by the standalone affine op.
 // qmask: the 8-column groups q (acc[4q .. 4q + 3]) this CTA stores (cluster split-K: those it reduced; otherwise all).
-template <int NPLANES, int BN, bool AFF>
+template <int NPLANES, int BN, bool AFF, bool STEM = false>
 __device__ __forceinline__ void epi_tile(const KParams& p, const EpiArgs& e, uint32_t stg, const float (&acc)[BN / 2],
                                          uint32_t qmask, int c_base, int n0, int h0, int w0) {
   const int tid = threadIdx.x;
@@ -374,7 +385,7 @@ __device__ __forceinline__ void epi_tile(const KParams& p, const EpiArgs& e, uin
   for (int k = 0; k < 4; ++k) {
     bool v;
     size_t pix;
-    row_to_pixel(p, rb + 32 * k, n0, h0, w0, v, pix);
+    row_to_pixel<STEM>(p, rb + 32 * k, n0, h0, w0, v, pix);
     orow[k] = pix * (size_t)e.cout;
     vmask |= (uint32_t)v << k;
   }
@@ -544,23 +555,16 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
     const int kb_end = ((split + 1) * p.k_blocks) / p.splits;
 
     for (int t = t_first; t < total; t += t_step) {
-      const int m_tile = t % op.m_tiles;
+      const int m0 = (t % op.m_tiles) * BM;   // first output pixel of the tile
       const int c_base = (t / op.m_tiles) * BN;
-      int n0 = 0, h0 = 0, w0 = 0;
-      if (p.flat) {
-        w0 = m_tile * BM;
-      } else {
-        const int tw = m_tile % p.tiles_w;
-        const int t2 = m_tile / p.tiles_w;
-        n0 = (t2 / p.tiles_h) * p.tile_n;
-        h0 = (t2 % p.tiles_h) * p.tile_h;
-        w0 = tw * p.tile_w;
-      }
 
       if (tid >= CONS_THREADS) {
         // =================================================================== producer
         if (tid == CONS_THREADS) {
-          const uint32_t a_rows = p.flat ? (uint32_t)BM : (uint32_t)(p.tile_n * p.tile_h * p.tile_w);
+          // im2col: input corner of pixel m0 = (n, oh, ow), the start of the tile's pixel walk
+          const int ow = m0 % p.wo;
+          const int oh = (m0 / p.wo) % p.ho;
+          const int cw = ow * p.sw - p.pad_l, ch = oh * p.sh - p.pad_t, cn = m0 / (p.wo * p.ho);
           uint32_t i2 = it;
           for (int kb = kb_begin; kb < kb_end; ++kb, ++i2) {
             const int stage = (int)(i2 % (uint32_t)stages);
@@ -570,20 +574,17 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
             const uint32_t b_dst = a_dst + NPLANES * L::A_PLANE;
             const int tap = kb / p.cblocks;
             const int cb = kb - tap * p.cblocks;
-            const int khi = tap / p.kw;
-            const int kwi = tap - khi * p.kw;
-            int cw = w0, ch = 0, cn = 0;
-            if (!p.flat) {
-              cw = w0 * p.sw + kwi - p.pad_l;
-              ch = h0 * p.sh + khi - p.pad_t;
-              cn = n0;
-            }
-            mbar_arrive_expect_tx(full_bar(stage), NPLANES * (a_rows * 128u + (uint32_t)L::B_PLANE));
-            tma_load_4d(a_dst, &op.tmx[0], full_bar(stage), cb * BK, cw, ch, cn);
-            tma_load_3d(b_dst, &op.tmw[0], full_bar(stage), cb * BK, c_base, tap);
-            if (NPLANES == 2) {
-              tma_load_4d(a_dst + L::A_PLANE, &op.tmx[1], full_bar(stage), cb * BK, cw, ch, cn);
-              tma_load_3d(b_dst + L::B_PLANE, &op.tmw[1], full_bar(stage), cb * BK, c_base, tap);
+            const uint16_t khi = (uint16_t)(tap / p.kw);
+            const uint16_t kwi = (uint16_t)(tap - khi * p.kw);
+            // every A load fills all 128 rows (zeros past the batch), so the byte count is the same for every tile
+            mbar_arrive_expect_tx(full_bar(stage), NPLANES * (uint32_t)(L::A_PLANE + L::B_PLANE));
+#pragma unroll
+            for (int pl = 0; pl < NPLANES; ++pl) {
+              if (p.im2col)
+                tma_load_im2col_4d(a_dst + pl * L::A_PLANE, &op.tmx[pl], full_bar(stage), cb * BK, cw, ch, cn, kwi, khi);
+              else
+                tma_load_4d(a_dst + pl * L::A_PLANE, &op.tmx[pl], full_bar(stage), cb * BK, m0, 0, 0);
+              tma_load_3d(b_dst + pl * L::B_PLANE, &op.tmw[pl], full_bar(stage), cb * BK, c_base, tap);
             }
           }
         }
@@ -668,22 +669,12 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
           }
         }
       }
-      epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, 0xffffu, c_base, n0, h0, w0);
+      epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, 0xffffu, c_base, 0, 0, m0);
     }
 
     if (MODE == 0 && p.cluster) {
       cluster_sync_all();
       if (tid < CONS_THREADS) {
-        const int m_tile = blockIdx.x;
-        int n0 = 0, h0 = 0, w0 = 0;
-        if (p.flat) {
-          w0 = m_tile * BM;
-        } else {
-          const int t2 = m_tile / p.tiles_w;
-          n0 = (t2 / p.tiles_h) * p.tile_n;
-          h0 = (t2 % p.tiles_h) * p.tile_h;
-          w0 = (m_tile % p.tiles_w) * p.tile_w;
-        }
         // this CTA reduces and stores the column groups q = rank, rank + S, ...; the partials it reads over DSMEM sit at
         // the start of each peer's ring, the staging tile after it, so peers may still be reading while this CTA stages
         const int S = p.splits;
@@ -704,7 +695,7 @@ __device__ __forceinline__ void conv_body(const MegaOp* ops, int n_ops, int stag
           }
           acc[4 * q] = a.x; acc[4 * q + 1] = a.y; acc[4 * q + 2] = a.z; acc[4 * q + 3] = a.w;
         }
-        epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, qmask, (int)blockIdx.y * BN, n0, h0, w0);
+        epi_tile<NPLANES, BN, AFF>(p, epi_args(op), stg, acc, qmask, (int)blockIdx.y * BN, 0, 0, (int)blockIdx.x * BM);
       }
       cluster_sync_all();   // no CTA may leave (and free its shared memory) while a peer still reads it
     }
@@ -807,7 +798,7 @@ __device__ __forceinline__ StemGeo stem_geo(const MegaOp& op) {
   return g;
 }
 
-// output pixel of row 0 of stem tile m_tile (tile_n = 1: a tile never spans two images)
+// output pixel of row 0 of stem tile m_tile (a stem tile never spans two images)
 __device__ __forceinline__ void stem_tile_origin(const KParams& p, int m_tile, int& n0, int& h0, int& w0) {
   const int t2 = m_tile / p.tiles_w;
   n0 = t2 / p.tiles_h;
@@ -1004,7 +995,7 @@ __device__ __forceinline__ void stem_body(const MegaOp* ops, int stages, int pdl
     if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
     int n0, h0, w0;
     stem_tile_origin(p, t % op.m_tiles, n0, h0, w0);
-    epi_tile<NPLANES, 64, false>(p, epi_args(op), stg, acc, 0xffffu, (t / op.m_tiles) * 64, n0, h0, w0);
+    epi_tile<NPLANES, 64, false, true>(p, epi_args(op), stg, acc, 0xffffu, (t / op.m_tiles) * 64, n0, h0, w0);
   }
 }
 
@@ -1078,6 +1069,67 @@ int encode_map(CUtensorMap* map, void* base, int rank, const uint64_t* dims, con
   return DEFER_OK;
 }
 
+typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                     const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*,
+                                     CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                     CUtensorMapFloatOOBfill);
+
+PFN_encodeIm2col get_encode_im2col() {
+  static PFN_encodeIm2col fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = (PFN_encodeIm2col)p;
+  }
+  return fn;
+}
+
+// The im2col bounding box of a conv over an h x w input, in (W, H) order.  The pixel walk of a tile visits the input
+// corners (ow * sw - pad_l, oh * sh - pad_t) of its output pixels in (n, oh, ow) order: in a row it steps by the stride up
+// to the corner of the last output column, then goes on at the lower corner of the next row (and of the next image after
+// the last row).  So the box runs from (-pad_l, -pad_t) to the corner of the last output pixel; TMA takes its lower
+// corner as an offset from input pixel (0, 0) and its upper corner as an offset from pixel (w - 1, h - 1).
+void im2col_corners(int h, int w, int ho, int wo, int sh, int sw, int pad_t, int pad_l, int lower[2], int upper[2]) {
+  lower[0] = -pad_l;
+  lower[1] = -pad_t;
+  upper[0] = (wo - 1) * sw - pad_l - (w - 1);
+  upper[1] = (ho - 1) * sh - pad_t - (h - 1);
+}
+
+// a rank-4 im2col tensor map holds each corner in [-128, 127] (the tap offsets of kernels up to 7 x 7 are far inside
+// what the load instruction takes)
+bool im2col_corners_encodable(const int lower[2], const int upper[2]) {
+  for (int i = 0; i < 2; ++i)
+    if (lower[i] < -128 || lower[i] > 127 || upper[i] < -128 || upper[i] > 127) return false;
+  return true;
+}
+
+// A operand of a non-flat conv: the NHWC plane at `base` as (C, W, H, N), walked 128 pixels x 64 channels per load
+int encode_im2col_map(CUtensorMap* map, void* base, const UmmaConvPlan& P) {
+  PFN_encodeIm2col enc = get_encode_im2col();
+  if (!enc) {
+    set_error("cuTensorMapEncodeIm2col entry point not available");
+    return DEFER_ERR_CUDA;
+  }
+  const uint64_t dims[4] = {(uint64_t)P.cin, (uint64_t)P.w, (uint64_t)P.h, (uint64_t)P.n};
+  const uint64_t strides[3] = {(uint64_t)P.cin * 2, (uint64_t)P.w * P.cin * 2, (uint64_t)P.h * P.w * P.cin * 2};
+  const uint32_t es[4] = {1, (uint32_t)P.sw, (uint32_t)P.sh, 1};
+  int lower[2], upper[2];
+  im2col_corners(P.h, P.w, P.ho, P.wo, P.sh, P.sw, P.pad_t, P.pad_l, lower, upper);
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, (const cuuint64_t*)dims, (const cuuint64_t*)strides, lower,
+                   upper, (cuuint32_t)BK, (cuuint32_t)BM, (const cuuint32_t*)es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeIm2col failed (CUresult %d): dims [%llu,%llu,%llu,%llu] corners (%d,%d)..(%d,%d) stride %dx%d",
+              (int)r, (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)dims[2],
+              (unsigned long long)dims[3], lower[0], lower[1], upper[0], upper[1], P.sh, P.sw);
+    return DEFER_ERR_CUDA;
+  }
+  return DEFER_OK;
+}
+
 template <auto kernel>
 int set_smem_attr(bool cluster16 = false) {
   static bool attr_set[64] = {false};   // one flag array per kernel instantiation
@@ -1109,8 +1161,7 @@ void fill_op(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, MegaOp* out) {
   op.tmw[1] = P.tmap_w[1];
   KParams& kp = op.p;
   kp.n = P.n; kp.ho = P.ho; kp.wo = P.wo; kp.cout = P.cout;
-  kp.tile_n = P.tile_n; kp.tile_h = P.tile_h; kp.tile_w = P.tile_w; kp.tiles_h = P.tiles_h; kp.tiles_w = P.tiles_w;
-  kp.flat = P.flat;
+  kp.im2col = P.im2col;
   kp.m_total = P.n * P.ho * P.wo;
   kp.kh = P.kh; kp.kw = P.kw; kp.sh = P.sh; kp.sw = P.sw; kp.pad_t = P.pad_t; kp.pad_l = P.pad_l;
   kp.cblocks = P.cin / 64;
@@ -1124,7 +1175,7 @@ void fill_op(const UmmaConvPlan& P, const UmmaConvLaneArgs& a, MegaOp* out) {
   kp.partial = a.partial;
   kp.counters = a.counters;
   kp.plane_out = (size_t)P.n * P.ho * P.wo * P.cout;
-  op.m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
+  op.m_tiles = P.m_tiles;
   op.n_tiles = P.cout / P.bn;
   op.scale2 = P.scale2;
   op.shift2 = P.shift2;
@@ -1262,8 +1313,9 @@ bool umma_conv_supported(int fmt, int n, int h, int w, int cin, int ho, int wo, 
   if (kh > 7 || kw > 7) return false;
   if (n < 1 || ho < 1 || wo < 1 || h < 1 || w < 1) return false;
   if ((size_t)n * ho * wo * cout >= (1ull << 40)) return false;
-  (void)pad_t; (void)pad_l;
-  return true;
+  int lower[2], upper[2];
+  im2col_corners(h, w, ho, wo, sh, sw, pad_t, pad_l, lower, upper);
+  return im2col_corners_encodable(lower, upper);
 }
 
 int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int kw,
@@ -1281,36 +1333,20 @@ int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin,
   const int taps = kh * kw;
   P.k_blocks = taps * (cin / 64);
 
-  // ---- M tiling
-  // flat [M, C] view only when the output grid IS the input grid (a fused asymmetric ZeroPadding2D gives ho != h even
-  // with pad_t == pad_l == 0; that case takes the 4-D box path, whose out-of-bounds zero fill is the padding)
-  P.flat = (kh == 1 && kw == 1 && sh == 1 && sw == 1 && pad_t == 0 && pad_l == 0 && ho == h && wo == w) ? 1 : 0;
-  if (P.flat) {
-    long long m = (long long)n * ho * wo;
-    P.tile_n = 1; P.tile_h = 1; P.tile_w = BM;
-    P.tiles_n = 1; P.tiles_h = 1; P.tiles_w = (int)((m + BM - 1) / BM);
-  } else {
-    int parts_w = (wo + BM - 1) / BM;                 // split very wide rows evenly
-    P.tile_w = (wo + parts_w - 1) / parts_w;
-    P.tiles_w = (wo + P.tile_w - 1) / P.tile_w;
-    P.tile_h = BM / P.tile_w;
-    if (P.tile_h > ho) P.tile_h = ho;
-    // balance rows across tiles (e.g. 14 rows: 7+7 instead of 9+5)
-    P.tiles_h = (ho + P.tile_h - 1) / P.tile_h;
-    P.tile_h = (ho + P.tiles_h - 1) / P.tiles_h;
-    P.tile_n = 1;
-    if (P.tile_h == ho && P.tiles_w == 1) {
-      P.tile_n = BM / (P.tile_h * P.tile_w);
-      if (P.tile_n > n) P.tile_n = n;
-      if (P.tile_n < 1) P.tile_n = 1;
-    }
-    P.tiles_n = (n + P.tile_n - 1) / P.tile_n;
-    if (P.tile_w * sw > 256 || P.tile_h * sh > 256) {
-      set_error("umma conv: TMA box too large (tile %dx%d stride %dx%d)", P.tile_h, P.tile_w, sh, sw);
+  // ---- M tiling: 128 consecutive output pixels per tile.  A 1x1/stride-1 conv whose output grid IS the input grid reads
+  // them as 128 consecutive rows of the [M, C] view; every other conv through TMA im2col (a fused asymmetric ZeroPadding2D
+  // gives ho != h even with pad_t == pad_l == 0: the bounding box and its out-of-bounds zero fill are the padding).
+  P.im2col = (kh == 1 && kw == 1 && sh == 1 && sw == 1 && pad_t == 0 && pad_l == 0 && ho == h && wo == w) ? 0 : 1;
+  P.m_tiles = (int)(((long long)n * ho * wo + BM - 1) / BM);
+  if (P.im2col) {
+    int lower[2], upper[2];
+    im2col_corners(h, w, ho, wo, sh, sw, pad_t, pad_l, lower, upper);
+    if (!im2col_corners_encodable(lower, upper)) {
+      set_error("umma conv: im2col box corners (%d,%d)..(%d,%d) outside [-128, 127]", lower[0], lower[1], upper[0], upper[1]);
       return DEFER_ERR_INVALID;
     }
   }
-  const int m_tiles = P.tiles_n * P.tiles_h * P.tiles_w;
+  const int m_tiles = P.m_tiles;
 
   // ---- N tile, split-K and ring depth.  The A tile is re-read once per N tile and the weights once per M tile, so
   // wide N tiles cut L2 -> SM traffic; split-K adds partial-tile traffic and is kept for launches of very few CTAs.
@@ -1399,18 +1435,14 @@ int umma_conv_bind(const UmmaConvPlan& P, UmmaConvLaneArgs* a, const void* x, co
   size_t xelems = (size_t)P.n * P.h * P.w * P.cin;
   for (int pl = 0; pl < P.nplanes; ++pl) {
     uint8_t* base = (uint8_t*)x + pl * xelems * 2;
-    if (P.flat) {
+    if (P.im2col) {
+      DEFER_TRY(encode_im2col_map(&a->tmap_x[pl], base, P));
+    } else {
       uint64_t m = (uint64_t)P.n * P.h * P.w;
       uint64_t dims[4] = {(uint64_t)P.cin, m, 1, 1};
       uint64_t strides[3] = {(uint64_t)P.cin * 2, m * P.cin * 2, m * P.cin * 2};
       uint32_t box[4] = {64, BM, 1, 1};
       uint32_t es[4] = {1, 1, 1, 1};
-      DEFER_TRY(encode_map(&a->tmap_x[pl], base, 4, dims, strides, box, es));
-    } else {
-      uint64_t dims[4] = {(uint64_t)P.cin, (uint64_t)P.w, (uint64_t)P.h, (uint64_t)P.n};
-      uint64_t strides[3] = {(uint64_t)P.cin * 2, (uint64_t)P.w * P.cin * 2, (uint64_t)P.h * P.w * P.cin * 2};
-      uint32_t box[4] = {64, (uint32_t)(P.tile_w * P.sw), (uint32_t)(P.tile_h * P.sh), (uint32_t)P.tile_n};
-      uint32_t es[4] = {1, (uint32_t)P.sw, (uint32_t)P.sh, 1};
       DEFER_TRY(encode_map(&a->tmap_x[pl], base, 4, dims, strides, box, es));
     }
   }
@@ -1420,7 +1452,7 @@ int umma_conv_bind(const UmmaConvPlan& P, UmmaConvLaneArgs* a, const void* x, co
   a->partial = nullptr;
   a->counters = nullptr;
   if (P.splits > 1 && !P.cluster) {
-    size_t tiles = (size_t)P.tiles_n * P.tiles_h * P.tiles_w * (P.cout / P.bn);
+    size_t tiles = (size_t)P.m_tiles * (P.cout / P.bn);
     DEFER_CUDA(cudaMalloc((void**)&a->partial, tiles * P.splits * BM * P.bn * sizeof(float)));
     DEFER_CUDA(cudaMalloc((void**)&a->counters, tiles * sizeof(unsigned int)));
     DEFER_CUDA(cudaMemset(a->counters, 0, tiles * sizeof(unsigned int)));
@@ -1523,10 +1555,8 @@ int umma_mega_set_stem(void* host_op, const float* x, int h, int w, int cin, int
   op->stem_kh = kh; op->stem_kw = kw; op->stem_sh = sh; op->stem_sw = sw;
   op->stem_pad_t = pad_t; op->stem_pad_l = pad_l;
   op->stem_K = kh * kw * cin;
-  // the real output map replaces the plan's flat view of the patch matrix: tile_n = 1, tile_h x tile_w pixels
+  // the real output map replaces the plan's flat view of the patch matrix: tile_h x tile_w pixels of one image
   stem_tile(p.ho, p.wo, kh, kw, sh, sw, cin, &p.tile_h, &p.tile_w, &op->stem_win_rows, &op->stem_win_cols);
-  p.flat = 0;
-  p.tile_n = 1;
   p.tiles_h = (p.ho + p.tile_h - 1) / p.tile_h;
   p.tiles_w = (p.wo + p.tile_w - 1) / p.tile_w;
   op->m_tiles = p.n * p.tiles_h * p.tiles_w;

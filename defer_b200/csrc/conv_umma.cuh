@@ -13,9 +13,9 @@ struct UmmaConvPlan {
   int n = 0, h = 0, w = 0, cin = 0, ho = 0, wo = 0, cout = 0;
   int kh = 1, kw = 1, sh = 1, sw = 1, pad_t = 0, pad_l = 0;
   uint32_t flags = 0;
-  // M tile = box of (tile_n images) x (tile_h rows) x (tile_w cols) output pixels, <= 128 rows
-  int tile_n = 1, tile_h = 1, tile_w = 1, tiles_n = 1, tiles_h = 1, tiles_w = 1;
-  int flat = 0;            // 1: 1x1/stride-1 conv treated as a plain [M, K] GEMM (tile_w = 128 rows)
+  // M tile t = the 128 consecutive output pixels [128 t, 128 t + 128) in (n, ho, wo) order
+  int m_tiles = 0;         // ceil(n * ho * wo / 128)
+  int im2col = 0;          // A tile: 1 = TMA im2col load of the NHWC input; 0 = tiled load of the [M, C] view (1x1, stride 1)
   int bn = 64;             // N tile (cout per CTA)
   int k_blocks = 0;        // taps * cin / 64
   int splits = 1;          // split-K factor (grid.z)
@@ -46,6 +46,7 @@ struct UmmaConvLaneArgs {
   unsigned int* counters = nullptr;  // split-K arrival counters, one per output tile
 };
 
+// false also when the corners of the shape's im2col bounding box are outside what TMA encodes for a rank-4 tensor
 bool umma_conv_supported(int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int kw, int sh, int sw,
                          int pad_t, int pad_l);
 int umma_conv_prepare(UmmaConvPlan* plan, int fmt, int n, int h, int w, int cin, int ho, int wo, int cout, int kh, int kw,

@@ -237,7 +237,7 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       if (op.backend == 2 || op.backend == 4) {
         if (op.stream)
           return launch_conv_stream(op.umma.nplanes, op.umma.bn, L.persist_op[oi],
-                                    op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w * (op.umma.cout / op.umma.bn),
+                                    op.umma.m_tiles * (op.umma.cout / op.umma.bn),
                                     op.umma.k_blocks, op.aff_op >= 0, st);
         if (op.persist) return launch_conv_persistent(op.umma.nplanes, L.persist_op[oi], op.n_tiles64, op.aff_op >= 0, st);
         return launch_conv_umma(op.umma, L.umma[oi], st);
@@ -963,8 +963,8 @@ int defer_stage_describe(defer_stage_t s, char* buf, size_t buf_len) {
     if ((op.backend == 2 || op.backend == 4) && op.umma.ready) {
       const UmmaConvPlan& u = op.umma;
       snprintf(line, sizeof line, "       wgmma tiles: m=%d x n=%d (BN %d) x k-splits %d%s, %d k-blocks, ring %d -> %d CTAs\n",
-               u.tiles_n * u.tiles_h * u.tiles_w, u.cout / u.bn, u.bn, u.splits, u.cluster ? " (cluster, DSMEM reduce)" : "",
-               u.k_blocks, u.stages, u.tiles_n * u.tiles_h * u.tiles_w * (u.cout / u.bn) * u.splits);
+               u.m_tiles, u.cout / u.bn, u.bn, u.splits, u.cluster ? " (cluster, DSMEM reduce)" : "",
+               u.k_blocks, u.stages, u.m_tiles * (u.cout / u.bn) * u.splits);
       o += line;
     }
   }
@@ -1165,7 +1165,7 @@ int defer_stage_finalize(defer_stage_t s) {
                                   d.sw, d.pad_t, d.pad_l, d.flags, (const float*)s->d_weights[d.w_kernel],
                                   d.w_scale >= 0 ? (const float*)s->d_weights[d.w_scale] : nullptr,
                                   d.w_shift >= 0 ? (const float*)s->d_weights[d.w_shift] : nullptr, mega_plan, stream_bn));
-      const int m_tiles = op.umma.tiles_n * op.umma.tiles_h * op.umma.tiles_w;
+      const int m_tiles = op.umma.m_tiles;
       op.n_tiles64 = m_tiles * (bo.c / 64);
       op.persist = (mega_plan || stream_bn > 0) && s->op_group[oi] < 0;
       if (attempt == 0 && !mega_plan) {
