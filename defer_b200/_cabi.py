@@ -19,8 +19,8 @@ LINK_TOKEN_BYTES = 256
 FMT_F32, FMT_BF16X2, FMT_BF16 = 0, 1, 2
 OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS, OP_RESIZE = range(1, 13)
 FLAG_RELU, FLAG_RESIDUAL = 1, 2
-BUF_ACT, BUF_F32, BUF_U8, BUF_JPEG = 0, 1, 2, 3
-OP_JPEG_DECODE = 13
+BUF_ACT, BUF_F32, BUF_U8, BUF_JPEG, BUF_PNG = 0, 1, 2, 3, 4
+OP_JPEG_DECODE, OP_PNG_DECODE = 13, 14
 PRE_CAFFE, PRE_TF = 0, 1
 PRE_MODES = {"caffe": PRE_CAFFE, "tf": PRE_TF}
 RESIZE_SAMPLE_W, RESIZE_SAMPLE_H = 1, 2
@@ -32,7 +32,7 @@ OP_NAMES = {OP_CONV: "conv", OP_MAXPOOL: "maxpool", OP_GAP: "gap", OP_DENSE: "de
             OP_AFFINE: "affine", OP_RELU: "relu", OP_ADD: "add", OP_PAD: "pad", OP_COPY: "copy",
             OP_PREPROCESS: "preprocess"}
 #: OP_NAMES covers the ops of a model and of its preprocess_input; KIND_NAMES adds RESIZE, the load_img resize in front
-KIND_NAMES = {**OP_NAMES, OP_RESIZE: "resize", OP_JPEG_DECODE: "jpeg_decode"}
+KIND_NAMES = {**OP_NAMES, OP_RESIZE: "resize", OP_JPEG_DECODE: "jpeg_decode", OP_PNG_DECODE: "png_decode"}
 
 
 class BufDesc(C.Structure):
@@ -77,6 +77,7 @@ PROTOTYPES = {
     "defer_stage_submit_parts": (_i, [_vp, _u64, _i, _i, _i, C.POINTER(_vp), _u64]),
     "defer_stage_submit_frames": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_submit_jpegs": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
+    "defer_stage_submit_pngs": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_step": (_i, [_vp, _u64]),
     "defer_stage_result": (_i, [_vp, _u64, _vp, _u64]),
     "defer_stage_predict": (_i, [_vp, _vp, _u64, _vp, _u64]),
@@ -110,6 +111,8 @@ PROTOTYPES = {
     "defer_k_resize_frames": (_i, [_i, _vp, _vp, _vp] + [_i] * 8 + [_vp]),
     "defer_k_jpeg_workspace": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
     "defer_k_jpeg_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "defer_k_png_workspace": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "defer_k_png_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 _LIB = None

@@ -206,6 +206,13 @@ size_t jpeg_workspace_bytes(int H, int W, int n);
 bool jpeg_bound_ok(int H, int W);
 int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
                        cudaStream_t st);
+// DEFER_OP_PNG_DECODE (png.cu): n PNG files in DEFER_PNG_SLOT_BYTES(H, W)-byte slots, with their blocks -> n U8 (H, W, 3)
+// images, through a workspace of png_workspace_bytes(H, W, n) (256-byte aligned)
+size_t png_workspace_bytes(int H, int W, int n);
+// the bounds (H, W) the decode takes: the slot fits the blocks' int32 offsets
+bool png_bound_ok(int H, int W);
+int launch_png_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
+                      cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

@@ -12,6 +12,7 @@
 #include <unistd.h>
 
 #include <mutex>
+#include <algorithm>
 #include <set>
 #include <utility>
 #include <stdlib.h>
@@ -118,8 +119,8 @@ struct Lane {
   bool timed = false;
   void* peer_out = nullptr;   // HOP_COPY: this lane's input slot on the consumer GPU (destination of the hop copy)
   int32_t* tables = nullptr;  // DEFER_RESIZE_SAMPLE_*: `batch` table blocks, next to the lane's input slot in the arena
-  int32_t* jpeg_blocks = nullptr;  // DEFER_OP_JPEG_DECODE: `batch` JPEG blocks, after the table blocks
-  void* jpeg_ws = nullptr;         // ... and its decode workspace (coefficients, planes, sync state)
+  int32_t* dec_blocks = nullptr;   // DEFER_OP_JPEG_DECODE / _PNG_DECODE: `batch` JPEG or PNG blocks, after the table blocks
+  void* dec_ws = nullptr;          // ... and its decode workspace
   // the microbatch the lane ran last (last stage: the one out_host is filled with); result() refuses any other
   bool stepped = false;
   uint64_t last_seq = 0;
@@ -182,12 +183,15 @@ struct defer_stage_s {
     size_t block_ints = 0;        // int32 values per sample block
     size_t tables_off = 0;        // offset of a lane's blocks from its input slot
   } frames;
-  // JPEG files at ingress: the DEFER_OP_JPEG_DECODE op (-1 = none) in front of the per-sample resize pair
-  struct Jpeg {
+  // JPEG or PNG files at ingress: the DEFER_OP_JPEG_DECODE or _PNG_DECODE op (-1 = none) in front of the per-sample
+  // resize pair
+  struct Decode {
     int op = -1;
-    size_t blocks_off = 0;        // offset of a lane's JPEG blocks from its input slot
+    int kind = 0;                 // its op kind
+    size_t block_ints = 0;        // DEFER_JPEG_BLOCK_INTS or DEFER_PNG_BLOCK_INTS
+    size_t blocks_off = 0;        // offset of a lane's blocks from its input slot
     size_t ws_bytes = 0;          // decode workspace per lane
-  } jpeg;
+  } dec;
 
   uint32_t* ctrl_u32(size_t off) { return reinterpret_cast<uint32_t*>(arena + off); }
   uint32_t* ready_flag(int d) { return ctrl_u32(OFF_READY + d * FLAG_STRIDE); }
@@ -199,10 +203,15 @@ struct defer_stage_s {
 namespace defer {
 
 static size_t elem_bytes(int elem, int fmt) {
-  return elem == DEFER_BUF_U8 || elem == DEFER_BUF_JPEG ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
+  return elem == DEFER_BUF_U8 || elem == DEFER_BUF_JPEG || elem == DEFER_BUF_PNG ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
 }
 
 static size_t buf_bytes(const Buf& b, int fmt) { return b.elems * elem_bytes(b.elem, fmt); }
+
+// the files a stage with a decode op takes, for messages: "JPEG" / "jpeg" or "PNG" / "png"
+static const char* dec_name(const defer_stage_s* s, bool upper) {
+  return s->dec.kind == DEFER_OP_PNG_DECODE ? (upper ? "PNG" : "png") : (upper ? "JPEG" : "jpeg");
+}
 
 // the axis of a fixed-table RESIZE op: named by modes W / H (it may keep its length under a crop box), else the one that
 // changes
@@ -289,7 +298,9 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       if (d.mode == DEFER_PRE_TF) return launch_preprocess_tf((const uint8_t*)x, (float*)y, (size_t)nb * bi.h * bi.w, st);
       return launch_preprocess((const uint8_t*)x, wptr(d.w_shift), (float*)y, (size_t)nb * bi.h * bi.w, st);
     case DEFER_OP_JPEG_DECODE:
-      return launch_jpeg_decode((const uint8_t*)x, L.jpeg_blocks, nb, bi.h, bi.w, L.jpeg_ws, (uint8_t*)y, st);
+      return launch_jpeg_decode((const uint8_t*)x, L.dec_blocks, nb, bi.h, bi.w, L.dec_ws, (uint8_t*)y, st);
+    case DEFER_OP_PNG_DECODE:
+      return launch_png_decode((const uint8_t*)x, L.dec_blocks, nb, bi.h, bi.w, L.dec_ws, (uint8_t*)y, st);
     case DEFER_OP_RESIZE:
       if (d.mode == DEFER_RESIZE_SAMPLE_W || d.mode == DEFER_RESIZE_SAMPLE_H) {
         const auto& f = s->frames;
@@ -393,6 +404,11 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
       op.alg_flops = 0;
       break;
     }
+    case DEFER_OP_PNG_DECODE:   // an upper bound: the slot read, gathered and read again, the scanlines written and
+                                // unfiltered at the slot's size, and the image
+      op.alg_bytes = 3.0 * (double)bi.bytes + 3.0 * nb * bi.h * (1.0 + 8.0 * bi.w) + out_b;
+      op.alg_flops = 0;
+      break;
     default:
       op.alg_bytes = in_b + out_b;
       op.alg_flops = 0;
@@ -471,17 +487,19 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     Buf b;
     b.h = bufs[i].h; b.w = bufs[i].w; b.c = bufs[i].c; b.elem = bufs[i].elem;
     if (b.h < 1 || b.w < 1 || b.c < 1 ||
-        (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8 && b.elem != DEFER_BUF_JPEG)) {
+        (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8 && b.elem != DEFER_BUF_JPEG &&
+         b.elem != DEFER_BUF_PNG)) {
       set_error("buffer %d: bad descriptor (%d,%d,%d,elem %d)", i, b.h, b.w, b.c, b.elem);
       return fail(DEFER_ERR_INVALID);
     }
     if (b.elem == DEFER_BUF_U8) {   // the first stage's image, or that image resized
       bool resized = false;
       for (int j = 0; j < n_ops; ++j)
-        resized |= ops[j].out == i && (ops[j].kind == DEFER_OP_RESIZE || ops[j].kind == DEFER_OP_JPEG_DECODE);
+        resized |= ops[j].out == i && (ops[j].kind == DEFER_OP_RESIZE || ops[j].kind == DEFER_OP_JPEG_DECODE ||
+                                       ops[j].kind == DEFER_OP_PNG_DECODE);
       if (!cfg->is_first || (i != cfg->input_buf && !resized)) {
-        set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE or "
-                  "JPEG_DECODE op", i);
+        set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE, "
+                  "JPEG_DECODE or PNG_DECODE op", i);
         return fail(DEFER_ERR_INVALID);
       }
     }
@@ -491,8 +509,14 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
                 "H * W * 24 + %d < 2^31", i, DEFER_JPEG_SUBSEQ_BITS);
       return fail(DEFER_ERR_INVALID);
     }
+    if (b.elem == DEFER_BUF_PNG && (!cfg->is_first || i != cfg->input_buf || b.c != 3 || !png_bound_ok(b.h, b.w))) {
+      set_error("buffer %d: a PNG buffer is legal only as the first stage's input buffer, (H, W, 3) with "
+                "DEFER_PNG_SLOT_BYTES(H, W) < 2^31", i);
+      return fail(DEFER_ERR_INVALID);
+    }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;
-    b.bytes = buf_bytes(b, cfg->fmt);
+    b.bytes = b.elem == DEFER_BUF_PNG ? (size_t)cfg->batch * DEFER_PNG_SLOT_BYTES((size_t)b.h, (size_t)b.w)
+                                      : buf_bytes(b, cfg->fmt);
     s->bufs.push_back(b);
   }
   if (cfg->is_first && s->bufs[cfg->input_buf].elem == DEFER_BUF_ACT) {
@@ -561,6 +585,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     if ((bi.elem == DEFER_BUF_JPEG) != (d.kind == DEFER_OP_JPEG_DECODE) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_JPEG)) {
       set_error("op %d: a JPEG buffer is read only by a JPEG_DECODE op (as in0), which reads nothing else", i);
+      return fail(DEFER_ERR_INVALID);
+    }
+    if ((bi.elem == DEFER_BUF_PNG) != (d.kind == DEFER_OP_PNG_DECODE) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_PNG)) {
+      set_error("op %d: a PNG buffer is read only by a PNG_DECODE op (as in0), which reads nothing else", i);
       return fail(DEFER_ERR_INVALID);
     }
     if (d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE && d.mode != 0) {
@@ -697,7 +725,7 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
             set_error("op %d (resize, per sample): takes no weights, in1 or flags (its tables come with each microbatch)", i);
             return fail(DEFER_ERR_INVALID);
           }
-          const bool from_input = d.in0 == cfg->input_buf || (s->jpeg.op >= 0 && d.in0 == ops[s->jpeg.op].out);
+          const bool from_input = d.in0 == cfg->input_buf || (s->dec.op >= 0 && d.in0 == ops[s->dec.op].out);
           if (horiz ? (!from_input || bo.h != bi.h || f.op_w >= 0) : (bo.w != bi.w || f.op_h >= 0)) {
             set_error("op %d (resize, per sample): SAMPLE_W maps the stage input (H, W) to (H, W_out), SAMPLE_H maps (H, W_out) "
                       "to (H_out, W_out), one of each per stage (got %dx%d -> %dx%d, mode %d)", i, bi.h, bi.w, bo.h, bo.w, d.mode);
@@ -753,12 +781,27 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         op.kname = "jpeg_entropy_kernel+jpeg_idct_kernel+jpeg_color_kernel";
         op.n_kernels = 3;
         if (d.in0 != cfg->input_buf || bo.elem != DEFER_BUF_U8 || bo.h != bi.h || bo.w != bi.w || bo.c != 3 || d.in1 >= 0 ||
-            d.flags || d.mode || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0 || s->jpeg.op >= 0) {
+            d.flags || d.mode || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0 || s->dec.op >= 0) {
           set_error("op %d (jpeg decode): maps the stage's JPEG input (H, W, 3) to a U8 (H, W, 3) buffer, once, with no weights, "
                     "in1, flags or mode", i);
           return fail(DEFER_ERR_INVALID);
         }
-        s->jpeg.op = i;
+        s->dec.op = i;
+        s->dec.kind = d.kind;
+        s->dec.block_ints = DEFER_JPEG_BLOCK_INTS;
+        break;
+      case DEFER_OP_PNG_DECODE:
+        op.kname = "png_inflate_kernel+png_unfilter_kernel+png_expand_kernel";
+        op.n_kernels = 3;
+        if (d.in0 != cfg->input_buf || bo.elem != DEFER_BUF_U8 || bo.h != bi.h || bo.w != bi.w || bo.c != 3 || d.in1 >= 0 ||
+            d.flags || d.mode || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0 || s->dec.op >= 0) {
+          set_error("op %d (png decode): maps the stage's PNG input (H, W, 3) to a U8 (H, W, 3) buffer, once, with no weights, "
+                    "in1, flags or mode (and no other decode op)", i);
+          return fail(DEFER_ERR_INVALID);
+        }
+        s->dec.op = i;
+        s->dec.kind = d.kind;
+        s->dec.block_ints = DEFER_PNG_BLOCK_INTS;
         break;
       default:
         set_error("op %d: unknown kind %d", i, d.kind);
@@ -780,8 +823,9 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     f.block_ints = 2 + (size_t)f.W_out * (2 + f.kw_w) + (size_t)f.H_out * (2 + f.kw_h);
   }
-  if (s->jpeg.op >= 0 && (s->frames.op_w < 0 || ops[s->frames.op_w].in0 != ops[s->jpeg.op].out)) {
-    set_error("the JPEG_DECODE op (op %d) feeds the per-sample resize pair: its output is SAMPLE_W's input", s->jpeg.op);
+  if (s->dec.op >= 0 && (s->frames.op_w < 0 || ops[s->frames.op_w].in0 != ops[s->dec.op].out)) {
+    set_error("the %s_DECODE op (op %d) feeds the per-sample resize pair: its output is SAMPLE_W's input", dec_name(s, true),
+              s->dec.op);
     return fail(DEFER_ERR_INVALID);
   }
   for (int i = 0; i < n_ops; ++i)
@@ -828,10 +872,12 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     s->frames.tables_off = s->slot_stride;
     s->slot_stride += ((size_t)cfg->batch * s->frames.block_ints * 4 + 1023) / 1024 * 1024;
   }
-  if (s->jpeg.op >= 0) {       // then the JPEG blocks (zeroed with the arena too)
-    s->jpeg.blocks_off = s->slot_stride;
-    s->slot_stride += ((size_t)cfg->batch * DEFER_JPEG_BLOCK_INTS * 4 + 1023) / 1024 * 1024;
-    s->jpeg.ws_bytes = jpeg_workspace_bytes(s->bufs[cfg->input_buf].h, s->bufs[cfg->input_buf].w, cfg->batch);
+  if (s->dec.op >= 0) {       // then the JPEG or PNG blocks (zeroed with the arena too)
+    const Buf& bi = s->bufs[cfg->input_buf];
+    s->dec.blocks_off = s->slot_stride;
+    s->slot_stride += ((size_t)cfg->batch * s->dec.block_ints * 4 + 1023) / 1024 * 1024;
+    s->dec.ws_bytes = s->dec.kind == DEFER_OP_PNG_DECODE ? png_workspace_bytes(bi.h, bi.w, cfg->batch)
+                                                         : jpeg_workspace_bytes(bi.h, bi.w, cfg->batch);
   }
   s->arena_bytes = CTRL_BYTES + s->slot_stride * cfg->depth;
   if (cudaMalloc((void**)&s->arena, s->arena_bytes) != cudaSuccess) {
@@ -857,13 +903,13 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     L.buf.assign(n_bufs, nullptr);
     L.buf[cfg->input_buf] = s->arena + CTRL_BYTES + s->slot_stride * l;
     if (s->frames.op_w >= 0) L.tables = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->frames.tables_off);
-    if (s->jpeg.op >= 0) {
-      L.jpeg_blocks = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->jpeg.blocks_off);
-      if (cudaMalloc(&L.jpeg_ws, s->jpeg.ws_bytes) != cudaSuccess) {
-        set_error("cudaMalloc JPEG decode workspace (%zu bytes) failed", s->jpeg.ws_bytes);
+    if (s->dec.op >= 0) {
+      L.dec_blocks = reinterpret_cast<int32_t*>(s->arena + CTRL_BYTES + s->slot_stride * l + s->dec.blocks_off);
+      if (cudaMalloc(&L.dec_ws, s->dec.ws_bytes) != cudaSuccess) {
+        set_error("cudaMalloc %s decode workspace (%zu bytes) failed", dec_name(s, true), s->dec.ws_bytes);
         return fail(DEFER_ERR_CUDA);
       }
-      s->workspace.push_back(L.jpeg_ws);
+      s->workspace.push_back(L.dec_ws);
     }
     for (int b = 0; b < n_bufs; ++b) {
       if (b == cfg->input_buf) continue;
@@ -1309,7 +1355,8 @@ int defer_stage_finalize(defer_stage_t s) {
 int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit: null");
   DEFER_CHECK(s->cfg.is_first, "submit: only the first stage takes host input");
-  DEFER_CHECK(s->jpeg.op < 0, "submit: this stage takes JPEG files (defer_stage_submit_jpegs)");
+  DEFER_CHECK(s->dec.op < 0, "submit: this stage takes %s files (defer_stage_submit_%ss)", dec_name(s, true),
+              dec_name(s, false));
   DEFER_CHECK(s->frames.op_w < 0, "submit: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   DEFER_CHECK(nbytes == b.bytes, "submit: got %llu bytes, stage input is %zu", (unsigned long long)nbytes, b.bytes);
@@ -1322,7 +1369,8 @@ int defer_stage_submit(defer_stage_t s, uint64_t seq, const void* host_in, uint6
 int defer_stage_submit_part(defer_stage_t s, uint64_t seq, int index, int count, const void* host_in, uint64_t nbytes) {
   DEFER_CHECK(s && host_in, "submit_part: null");
   DEFER_CHECK(s->cfg.is_first, "submit_part: only the first stage takes host input");
-  DEFER_CHECK(s->jpeg.op < 0, "submit_part: this stage takes JPEG files (defer_stage_submit_jpegs)");
+  DEFER_CHECK(s->dec.op < 0, "submit_part: this stage takes %s files (defer_stage_submit_%ss)", dec_name(s, true),
+              dec_name(s, false));
   DEFER_CHECK(s->frames.op_w < 0, "submit_part: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;       // first-stage input is plain fp32 NHWC: samples are contiguous
@@ -1341,7 +1389,8 @@ int defer_stage_submit_parts(defer_stage_t s, uint64_t seq, int first_index, int
                              const void* const* host_ptrs, uint64_t nbytes_per_item) {
   DEFER_CHECK(s && host_ptrs && n_items >= 1 && samples_per_item >= 1, "submit_parts: bad arguments");
   DEFER_CHECK(s->cfg.is_first, "submit_parts: only the first stage takes host input");
-  DEFER_CHECK(s->jpeg.op < 0, "submit_parts: this stage takes JPEG files (defer_stage_submit_jpegs)");
+  DEFER_CHECK(s->dec.op < 0, "submit_parts: this stage takes %s files (defer_stage_submit_%ss)", dec_name(s, true),
+              dec_name(s, false));
   DEFER_CHECK(s->frames.op_w < 0, "submit_parts: this stage takes images of mixed sizes (defer_stage_submit_frames)");
   const Buf& b = s->bufs[s->cfg.input_buf];
   const size_t sample = b.bytes / (size_t)s->cfg.batch;
@@ -1366,7 +1415,8 @@ int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, in
   DEFER_CHECK(s->cfg.is_first, "submit_frames: only the first stage takes host input");
   const auto& f = s->frames;
   DEFER_CHECK(f.op_w >= 0, "submit_frames: the stage takes one image size (no DEFER_RESIZE_SAMPLE_* ops); use defer_stage_submit*");
-  DEFER_CHECK(s->jpeg.op < 0, "submit_frames: this stage takes JPEG files (defer_stage_submit_jpegs)");
+  DEFER_CHECK(s->dec.op < 0, "submit_frames: this stage takes %s files (defer_stage_submit_%ss)", dec_name(s, true),
+              dec_name(s, false));
   DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_frames: samples [%d, %d) outside the microbatch of %d",
               first_index, first_index + n, s->cfg.batch);
   DEFER_CHECK(table_bytes == (uint64_t)n * f.block_ints * 4, "submit_frames: got %llu table bytes, %d blocks are %zu",
@@ -1395,7 +1445,7 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes) {
   DEFER_CHECK(s && data && nbytes && blocks && n >= 1, "submit_jpegs: bad arguments");
   DEFER_CHECK(s->cfg.is_first, "submit_jpegs: only the first stage takes host input");
-  DEFER_CHECK(s->jpeg.op >= 0, "submit_jpegs: the stage has no DEFER_OP_JPEG_DECODE op");
+  DEFER_CHECK(s->dec.kind == DEFER_OP_JPEG_DECODE, "submit_jpegs: the stage has no DEFER_OP_JPEG_DECODE op");
   const auto& f = s->frames;
   DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_jpegs: samples [%d, %d) outside the microbatch of %d",
               first_index, first_index + n, s->cfg.batch);
@@ -1441,13 +1491,70 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
   bool all_base = true;
   for (int i = 0; i < n; ++i) all_base &= used(i) == DEFER_JPEG_BASE_INTS;
   if (all_base) {
-    DEFER_CUDA(cudaMemcpy2DAsync(L.jpeg_blocks + (size_t)first_index * DEFER_JPEG_BLOCK_INTS, DEFER_JPEG_BLOCK_INTS * 4,
+    DEFER_CUDA(cudaMemcpy2DAsync(L.dec_blocks + (size_t)first_index * DEFER_JPEG_BLOCK_INTS, DEFER_JPEG_BLOCK_INTS * 4,
                                  blocks + f.block_ints, per * 4, DEFER_JPEG_BASE_INTS * 4, n, cudaMemcpyHostToDevice,
                                  L.stream));
   } else {
     for (int i = 0; i < n; ++i)
-      DEFER_CUDA(cudaMemcpyAsync(L.jpeg_blocks + (size_t)(first_index + i) * DEFER_JPEG_BLOCK_INTS,
+      DEFER_CUDA(cudaMemcpyAsync(L.dec_blocks + (size_t)(first_index + i) * DEFER_JPEG_BLOCK_INTS,
                                  blocks + (size_t)i * per + f.block_ints, used(i) * 4, cudaMemcpyHostToDevice, L.stream));
+  }
+  return DEFER_OK;
+}
+
+int defer_stage_submit_pngs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                            const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes) {
+  DEFER_CHECK(s && data && nbytes && blocks && n >= 1, "submit_pngs: bad arguments");
+  DEFER_CHECK(s->cfg.is_first, "submit_pngs: only the first stage takes host input");
+  DEFER_CHECK(s->dec.kind == DEFER_OP_PNG_DECODE, "submit_pngs: the stage has no DEFER_OP_PNG_DECODE op");
+  const auto& f = s->frames;
+  DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_pngs: samples [%d, %d) outside the microbatch of %d",
+              first_index, first_index + n, s->cfg.batch);
+  const size_t per = f.block_ints + DEFER_PNG_BLOCK_INTS;      // one file's resize block, then its PNG block
+  DEFER_CHECK(block_bytes == (uint64_t)n * per * 4, "submit_pngs: got %llu block bytes, %d files take %zu",
+              (unsigned long long)block_bytes, n, (size_t)n * per * 4);
+  const uint64_t slot = DEFER_PNG_SLOT_BYTES((uint64_t)f.H, (uint64_t)f.W);
+  for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
+    const int32_t* rb = blocks + (size_t)i * per;
+    const int32_t* pb = rb + f.block_ints;
+    DEFER_CHECK(data[i], "submit_pngs: file %d is null", i);
+    DEFER_CHECK(nbytes[i] >= 8 && nbytes[i] <= slot, "submit_pngs: file %d has %llu bytes, the slot takes 8..%llu", i,
+                (unsigned long long)nbytes[i], (unsigned long long)slot);
+    DEFER_CHECK(pb[0] >= 1 && pb[0] <= f.H && pb[1] >= 1 && pb[1] <= f.W, "submit_pngs: file %d is %dx%d, the slot takes 1..%d x "
+                "1..%d", i, pb[0], pb[1], f.H, f.W);
+    DEFER_CHECK(rb[0] == pb[0] && rb[1] == pb[1], "submit_pngs: resize block %d is for %dx%d, PNG block %d for %dx%d", i, rb[0],
+                rb[1], i, pb[0], pb[1]);
+    const int ct = pb[2], d = pb[3];
+    const int ch = ct == 0 ? 1 : ct == 2 ? 3 : ct == 3 ? 1 : ct == 4 ? 2 : ct == 6 ? 4 : 0;
+    const bool depth_ok = d == 8 || (d == 16 && ct != 3) || ((d == 1 || d == 2 || d == 4) && (ct == 0 || ct == 3));
+    DEFER_CHECK(ch && depth_ok && pb[4] == (int)(((int64_t)pb[1] * ch * d + 7) / 8) && pb[5] == std::max(1, ch * d / 8),
+                "submit_pngs: file %d: colour type %d, depth %d, %d bytes per row and filter unit %d do not match", i, ct, d,
+                pb[4], pb[5]);
+    DEFER_CHECK(pb[6] >= 1 && pb[6] <= DEFER_PNG_MAX_IDAT && pb[8] >= 0 && pb[8] <= 256,
+                "submit_pngs: file %d: %d IDAT chunks (1..%d) and %d palette entries (0..256)", i, pb[6], DEFER_PNG_MAX_IDAT,
+                pb[8]);
+    int64_t total = 0;
+    for (int k = 0; k < pb[6]; ++k) {
+      const int32_t off = pb[DEFER_PNG_IDAT_OFF + 2 * k], len = pb[DEFER_PNG_IDAT_OFF + 2 * k + 1];
+      DEFER_CHECK(off >= 0 && len >= 0 && (uint64_t)off + (uint64_t)len <= nbytes[i],
+                  "submit_pngs: file %d: IDAT chunk %d [%d, %d + %d) outside its %llu bytes", i, k, off, off, len,
+                  (unsigned long long)nbytes[i]);
+      total += len;
+    }
+    DEFER_CHECK(total == pb[7], "submit_pngs: file %d: its IDAT chunks hold %lld bytes, its block says %d", i, (long long)total,
+                pb[7]);
+  }
+  DEFER_TRY(set_device(s));
+  Lane& L = s->lanes[seq % s->cfg.depth];
+  uint8_t* dst = (uint8_t*)L.buf[s->cfg.input_buf];
+  for (int i = 0; i < n; ++i)   // the file's own bytes only, at the start of its sample slot
+    DEFER_CUDA(cudaMemcpyAsync(dst + (size_t)(first_index + i) * slot, data[i], nbytes[i], cudaMemcpyHostToDevice, L.stream));
+  DEFER_CUDA(cudaMemcpy2DAsync(L.tables + (size_t)first_index * f.block_ints, f.block_ints * 4, blocks, per * 4,
+                               f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
+  for (int i = 0; i < n; ++i) {   // each PNG block's prefix that its file uses: header, palette and its IDAT ranges
+    const int32_t* pb = blocks + (size_t)i * per + f.block_ints;
+    DEFER_CUDA(cudaMemcpyAsync(L.dec_blocks + (size_t)(first_index + i) * DEFER_PNG_BLOCK_INTS, pb,
+                               ((size_t)DEFER_PNG_IDAT_OFF + 2 * (size_t)pb[6]) * 4, cudaMemcpyHostToDevice, L.stream));
   }
   return DEFER_OK;
 }
@@ -1625,6 +1732,13 @@ int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_o
                 op.aff_op, buf_id);
   }
   DEFER_CUDA(cudaStreamSynchronize(s->lanes[lane].stream));
+  if (b.elem == DEFER_BUF_PNG) {   // the first h * w * 3 bytes of each sample's slot
+    const size_t per = (size_t)b.h * b.w * b.c, slot = b.bytes / s->cfg.batch;
+    std::vector<uint8_t> raw(b.elems);
+    DEFER_CUDA(cudaMemcpy2D(raw.data(), per, src, slot, per, s->cfg.batch, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < b.elems; ++i) host_out[i] = (float)raw[i];
+    return DEFER_OK;
+  }
   if (b.elem == DEFER_BUF_U8 || b.elem == DEFER_BUF_JPEG) {
     std::vector<uint8_t> raw(b.elems);
     DEFER_CUDA(cudaMemcpy(raw.data(), src, b.elems, cudaMemcpyDeviceToHost));

@@ -34,7 +34,8 @@ queue item is a uint8 image ``(batch, h, w, 3)`` of its own size with ``h <= H``
 share a microbatch, and each gives exactly what ``image_size=(h, w)`` would.  Only the image's own bytes cross PCIe.
 With ``decode="jpeg"`` as well, each queue item is a baseline JPEG file (``open(path, "rb").read()``); the first GPU
 decodes it exactly as ``load_img`` does with Pillow (``jpeg.decode_jpeg``), so only the compressed file crosses PCIe
-and the host only parses its markers.  ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``, and with
+and the host only parses its markers.  ``decode="png"`` does the same for non-interlaced PNG files (``png.decode_png``);
+the host only walks their chunk headers.  A pipeline decodes one of the two formats.  ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``, and with
 ``decode="jpeg"``) resizes each image's centred crop with the model input's aspect ratio instead of squashing the whole
 image, as ``load_img(..., keep_aspect_ratio=True)`` does: ``applications.resize_image(item, (H, W), interpolation,
 keep_aspect_ratio=True)``.
@@ -58,6 +59,7 @@ import numpy as np
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
 from .jpeg import check_decode, check_jpeg
+from .png import DECODES, check_png
 from .resize import check_frame, check_interpolation, check_keep_aspect_ratio, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
@@ -70,9 +72,9 @@ class DEFER:
                  image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
                  max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
                  keep_aspect_ratio: bool = False) -> None:
-        check_decode(decode, preprocess, image_size, max_image_size)
+        check_decode(decode, preprocess, image_size, max_image_size, DECODES)
         if decode is not None and batch not in (None, 1):
-            raise ValueError(f"decode={decode!r}: a queue item is one JPEG file, so batch must be 1, got {batch}")
+            raise ValueError(f"decode={decode!r}: a queue item is one {decode.upper()} file, so batch must be 1, got {batch}")
         if preprocess is not None:
             check_preprocess(preprocess)
         check_interpolation(interpolation)
@@ -96,7 +98,7 @@ class DEFER:
         self.interpolation = interpolation
         self.keep_aspect_ratio = keep_aspect_ratio  # resize Keras' centred crop of each image (load_img keep_aspect_ratio)
         self.max_image_size = max_image_size  # None | (H, W): uint8 queue items of any size up to it, resized on stage 0
-        self.decode = decode                # None | "jpeg": queue items are JPEG files, decoded on stage 0
+        self.decode = decode                # None | "jpeg" | "png": queue items are JPEG / PNG files, decoded on stage 0
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -202,10 +204,13 @@ class DEFER:
         if bound is not None:                # each image with its own size and tables, one C call per group
             def submit_items(seq, group):
                 first.submit_frames(seq, 0, group)
-        jpeg = self.decode == "jpeg"
-        if jpeg:                             # the files, parsed here, decoded on the GPU
+        files = self.decode is not None      # JPEG or PNG files
+        check_file = check_png if self.decode == "png" else check_jpeg
+        if files:                            # the files, parsed here, decoded on the GPU
+            submit_files = first.submit_pngs if self.decode == "png" else first.submit_jpegs
+
             def submit_items(seq, group):
-                first.submit_jpegs(seq, 0, [d for d, _ in group], [i for _, i in group])
+                submit_files(seq, 0, [d for d, _ in group], [i for _, i in group])
         try:
             while not self._stop.is_set():
                 try:
@@ -222,8 +227,8 @@ class DEFER:
                 in_shape = None
                 while True:
                     x = model_input
-                    if jpeg:                         # (file bytes, header): refused files raise here, as bad items do
-                        x = check_jpeg(x, bound)
+                    if files:                        # (file bytes, header): refused files raise here, as bad items do
+                        x = check_file(x, bound)
                     elif bound is not None:          # any size up to the bound: no same-shape rule within a group
                         x = check_frame(x, bound)
                     elif u8:
@@ -234,9 +239,9 @@ class DEFER:
                         x = np.ascontiguousarray(x)
                     elif not (isinstance(x, np.ndarray) and x.dtype == np.float32 and x.flags["C_CONTIGUOUS"]):
                         x = np.ascontiguousarray(x, dtype=np.float32)
-                    if not jpeg and x.shape[0] != B:
+                    if not files and x.shape[0] != B:
                         raise ValueError(f"queue item has batch {x.shape[0]}, DEFER was built for batch {B}")
-                    if jpeg or bound is not None:
+                    if files or bound is not None:
                         pass
                     elif in_shape is None:
                         in_shape = x.shape

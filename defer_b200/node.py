@@ -24,6 +24,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .node_state import NodeState
 from .planner import Plan, plan_stage
+from . import png
 from .jpeg import BLOCK_INTS, check_jpeg, pack_block
 from .resize import check_frame, pack_frame_tables
 
@@ -85,7 +86,7 @@ class StageRunner:
         self.resizes = any(o.kind == A.OP_RESIZE for o in plan.ops)
         # planned with max_image_size=: images of mixed sizes, fed by submit_frames with their table blocks
         self.frames = plan.frames
-        self.decode = plan.decode                    # "jpeg": fed by submit_jpegs, files with their JPEG blocks
+        self.decode = plan.decode                    # "jpeg" / "png": fed by submit_jpegs / submit_pngs, files with blocks
         self._tables: Dict[int, tuple] = {}          # per lane: blocks, sizes and images of its latest microbatch (kept alive)
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
@@ -126,7 +127,8 @@ class StageRunner:
         ``(H, W)``, each resized from its own size; feed them with ``submit_frames`` / ``predict_frames``.
         ``decode="jpeg"`` (with ``preprocess`` and ``max_image_size``): inputs are baseline JPEG files of images up to
         ``(H, W)``, decoded on the GPU as Keras' ``load_img`` does (``jpeg.decode_jpeg``); feed them with
-        ``submit_jpegs`` / ``predict_jpegs``.
+        ``submit_jpegs`` / ``predict_jpegs``.  ``decode="png"``: the same for non-interlaced PNG files (``png.decode_png``),
+        fed with ``submit_pngs`` / ``predict_pngs``.
         ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``): each image's centred crop with the model
         input's aspect ratio is resized, as ``load_img(..., keep_aspect_ratio=True)`` does (``resize.keras_crop_box``)."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
@@ -233,7 +235,8 @@ class StageRunner:
         if self.frames is None:
             raise ValueError(f"{self.name}: submit_frames needs a stage planned with max_image_size=")
         if self.decode is not None:
-            raise ValueError(f"{self.name}: this stage takes JPEG files; feed them with submit_jpegs / predict_jpegs")
+            raise ValueError(f"{self.name}: this stage takes {self.decode.upper()} files; feed them with "
+                             f"submit_{self.decode}s / predict_{self.decode}s")
         bound = self.frames["max_image_size"]
         images = []
         for x in frames:
@@ -291,6 +294,39 @@ class StageRunner:
     def predict_jpegs(self, items) -> np.ndarray:
         """Single-stage ``model.predict`` of a ``decode="jpeg"`` stage: the outputs of the JPEG files ``items``, in order."""
         self.submit_jpegs(0, 0, items)
+        self.step(0)
+        return self.result(0)[:len(items)]
+
+    def submit_pngs(self, seq: int, index: int, items, infos=None) -> None:
+        """Ingress of a ``decode="png"`` stage, as ``submit_jpegs``: ``items`` are PNG files, their chunks are walked here
+        (``png.check_png``: a refused file raises a ValueError and nothing is copied), and one C call copies each file's
+        own bytes and then its resize block and the part of its PNG block it uses."""
+        if self.decode != "png":
+            raise ValueError(f"{self.name}: submit_pngs needs a stage planned with decode='png'")
+        bound = self.frames["max_image_size"]
+        if infos is None:
+            items, infos = zip(*[png.check_png(x, bound) for x in items]) if items else ((), ())
+        files = items
+        n = len(files)
+        if not 1 <= n <= self.batch - index or index < 0:
+            raise ValueError(f"{self.name}: {n} files from sample {index} do not fit the microbatch of {self.batch}")
+        hw = np.array([(i.h, i.w) for i in infos], np.int32).reshape(n, 2)
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"],
+                                   self.frames.get("keep_aspect_ratio", False))
+        nr = tables.shape[1]
+        blocks = np.zeros((n, nr + png.BLOCK_INTS), np.int32)  # only the prefix each file uses is written and copied
+        blocks[:, :nr] = tables
+        for k, i in enumerate(infos):
+            png.pack_block(i, blocks[k, nr:])
+        sizes = np.array([len(f) for f in files], np.uint64)
+        self._tables[seq % self.depth] = (blocks, sizes, files)
+        ptrs = (C.c_void_p * n)(*[C.cast(C.c_char_p(f), C.c_void_p).value for f in files])
+        A.check(self.lib.defer_stage_submit_pngs(self.handle, seq, index, n, ptrs, sizes.ctypes.data, blocks.ctypes.data,
+                                                 blocks.nbytes))
+
+    def predict_pngs(self, items) -> np.ndarray:
+        """Single-stage ``model.predict`` of a ``decode="png"`` stage: the outputs of the PNG files ``items``, in order."""
+        self.submit_pngs(0, 0, items)
         self.step(0)
         return self.result(0)[:len(items)]
 

@@ -24,7 +24,8 @@ With ``max_image_size=(H, W)`` instead, the stage input is a uint8 slot of that 
 ``RESIZE`` ops (``RESIZE_SAMPLE_W``, then ``_H``) read each image's size and tables from a block that comes with it
 (``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.  With
 ``decode="jpeg"`` as well, the stage input is a byte slot of ``H * W * 3`` per sample holding one JPEG file, and a
-``JPEG_DECODE`` op in front of the resize pair decodes it into the uint8 slot (``jpeg.pack_block``).
+``JPEG_DECODE`` op in front of the resize pair decodes it into the uint8 slot (``jpeg.pack_block``); with ``decode="png"``
+the slot holds one PNG file (``png.slot_bytes(H, W)`` bytes) and a ``PNG_DECODE`` op takes that place (``png.pack_block``).
 ``keep_aspect_ratio=True`` resizes Keras' centred crop of each image instead (``resize.keras_crop_box``): with
 ``image_size`` the two ``RESIZE`` ops carry box tables, and an axis that keeps its length under a partial box is
 resampled by an op whose ``mode`` names its axis (``RESIZE_W`` / ``_H``); with ``max_image_size`` the feeder packs each
@@ -41,6 +42,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
 from .jpeg import check_decode
+from .png import DECODES
 from .resize import check_interpolation, check_keep_aspect_ratio, check_size, crop_boxes, kcap, resize_tables
 
 
@@ -87,7 +89,8 @@ class Plan:
     # plus "keep_aspect_ratio": True when that is on, what the stage's feeder needs to pack each image's table block
     # (resize.pack_frame_tables); None otherwise
     frames: Optional[dict] = None
-    # decode="jpeg": the stage takes JPEG files (each with its jpeg.pack_block block after its table block); None otherwise
+    # decode="jpeg" / "png": the stage takes JPEG / PNG files (each with its jpeg.pack_block / png.pack_block block after its
+    # table block); None otherwise
     decode: Optional[str] = None
 
     def describe(self) -> str:
@@ -111,7 +114,7 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
                image_size: Optional[Tuple[int, int]] = None, interpolation: str = "nearest",
                max_image_size: Optional[Tuple[int, int]] = None, decode: Optional[str] = None,
                keep_aspect_ratio: bool = False) -> Plan:
-    check_decode(decode, preprocess, image_size, max_image_size)
+    check_decode(decode, preprocess, image_size, max_image_size, DECODES)
     if preprocess is not None:
         check_preprocess(preprocess)
         if not is_first:
@@ -229,10 +232,12 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         H, W, _ = _hwc(shapes[in_name])
         h, w = image_size or max_image_size or (H, W)
         input_shape = (h, w, 3)
-        input_buf = img = new_buf((None,) + input_shape, A.BUF_JPEG if decode else A.BUF_U8)
+        files, op_decode = {None: (A.BUF_U8, None), "jpeg": (A.BUF_JPEG, A.OP_JPEG_DECODE),
+                            "png": (A.BUF_PNG, A.OP_PNG_DECODE)}[decode]
+        input_buf = img = new_buf((None,) + input_shape, files)
         if decode is not None:
-            # the JPEG files decode into the image slot the per-sample resize reads (jpeg.pack_block per file)
-            img = emit(PlanOp(A.OP_JPEG_DECODE, img, new_buf((None,) + input_shape, A.BUF_U8),
+            # the files decode into the image slot the per-sample resize reads (jpeg.pack_block / png.pack_block per file)
+            img = emit(PlanOp(op_decode, img, new_buf((None,) + input_shape, A.BUF_U8),
                               layers=[f"load_img(decode {decode} <={h}x{w})"])).out
         if max_image_size is not None:
             # images of mixed sizes up to (h, w): both passes always, the tables come with each image

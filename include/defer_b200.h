@@ -76,9 +76,11 @@ typedef enum defer_op_kind {
                          /*   channel; 0 <= first, 1 <= count <= kw, first + count <= in_len (checked at create)  */
                          /* `mode` DEFER_RESIZE_W / _H: the same on the named axis, which may keep its length    */
                          /* `mode` DEFER_RESIZE_SAMPLE_W / _H: images of mixed sizes, tables per sample (below)   */
-  DEFER_OP_JPEG_DECODE = 13 /* baseline JPEG files -> images (below): in0 = the stage input, a DEFER_BUF_JPEG (H, W, 3)    */
+  DEFER_OP_JPEG_DECODE = 13, /* baseline JPEG files -> images (below): in0 = the stage input, a DEFER_BUF_JPEG (H, W, 3)   */
                          /*   slot per sample; out = U8 (H, W, 3), each image packed (h, w, 3) at the start of its sample;  */
                          /*   read by the DEFER_RESIZE_SAMPLE_W op.  No weights, mode 0.                                     */
+  DEFER_OP_PNG_DECODE = 14 /* non-interlaced PNG files -> images (below): as DEFER_OP_JPEG_DECODE, from a DEFER_BUF_PNG  */
+                         /*   (H, W, 3) input of DEFER_PNG_SLOT_BYTES(H, W) bytes per sample                                 */
 } defer_op_kind;
 
 /* defer_op_desc.mode of a DEFER_OP_RESIZE op.  0: the fixed-size resize above (one image size per stage).
@@ -147,6 +149,38 @@ typedef enum defer_op_kind {
 /* bits per subsequence of the self-synchronising Huffman decode */
 #define DEFER_JPEG_SUBSEQ_BITS 8192
 
+/* DEFER_OP_PNG_DECODE decodes each sample's PNG file on the GPU, bit for bit as Pillow's convert("RGB") gives it
+ * (defer_b200/png.py restates it, with its one defined result for corrupt data).  It is planned before the
+ * DEFER_RESIZE_SAMPLE_W / _H pair, exactly where DEFER_OP_JPEG_DECODE is.  The sample's file sits at the start of its
+ * DEFER_PNG_SLOT_BYTES(H, W)-byte slot, room for the stored (level 0) encoding of any accepted image up to (H, W); its
+ * int32 block, written next to the slots by defer_stage_submit_pngs after the resize blocks, is DEFER_PNG_BLOCK_INTS
+ * values:
+ *   [0] h  [1] w  [2] colour type (0, 2, 3, 4, 6)  [3] bit depth  [4] bytes per row (without the filter byte)
+ *   [5] filter unit (bytes per complete pixel, at least 1)  [6] IDAT chunks  [7] their total payload bytes
+ *   [8] PLTE entries  [9..15] 0
+ *   [DEFER_PNG_PAL_OFF + i]           palette entry i < 256: r | g << 8 | b << 16, zero past the PLTE length
+ *   [DEFER_PNG_IDAT_OFF + 2 k, + 1]   IDAT chunk k < [6]: payload offset in the file, payload length
+ * Only the prefix a file uses, DEFER_PNG_IDAT_OFF + 2 * [6] values, is copied and read.  The device gathers the IDAT
+ * payloads into one zlib stream, inflates it (stored, fixed and dynamic Huffman blocks), unfilters the scanlines in a
+ * wavefront and converts them to RGB as Pillow does for the file's mode and depth.
+ * The decode never trusts the block: h / w are clamped into the slot, colour type and depth to a valid pair (from which
+ * it derives the row length itself), every IDAT range into the slot and the stream into its workspace, so no block
+ * content makes it access memory outside the sample's slot, workspace or image.  The blocks are zeroed at create: a
+ * never-written sample decodes to a 1x1 black image.  Corrupt compressed data ends the stream; the scanline bytes not
+ * produced are zero, and a filter type above 4 unfilters its row as None (defer_b200/png.py gives the exact rule).
+ * Workspace stats: [0] status (0 complete, 1 final block before the end, 2 input exhausted, 3 bad block type or stored
+ * length, 4 bad dynamic header, 5 bad code or symbol, 6 distance too far back), [1] scanline bytes produced, [2] rows
+ * with an unknown filter type. */
+#define DEFER_PNG_HDR_INTS 16
+#define DEFER_PNG_PAL_OFF DEFER_PNG_HDR_INTS
+#define DEFER_PNG_IDAT_OFF (DEFER_PNG_PAL_OFF + 256)
+/* IDAT chunks of one file (more are refused by the parser; libpng writes 8 KiB chunks) */
+#define DEFER_PNG_MAX_IDAT 4096
+#define DEFER_PNG_BLOCK_INTS (DEFER_PNG_IDAT_OFF + 2 * DEFER_PNG_MAX_IDAT)
+/* one sample's file slot: the stored encoding of RGBA at 16 bits, H * (1 + 8 W) scanline bytes, 1/64 more for block and
+ * chunk headers, and 64 KiB for the other chunks */
+#define DEFER_PNG_SLOT_BYTES(H, W) ((H) * (1 + 8 * (W)) + (H) * (1 + 8 * (W)) / 64 + 65536)
+
 /* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
 #define DEFER_PRE_CAFFE 0   /* keras_applications imagenet_utils mode='caffe' (ResNet50/101/152, VGG16) */
 #define DEFER_PRE_TF    1   /* mode='tf' (ResNet50V2/101V2/152V2): fl32(fl32(x / 127.5) - 1), bit for bit */
@@ -162,11 +196,13 @@ typedef enum defer_op_kind {
                           /* (or of a DEFER_OP_JPEG_DECODE)                                                                */
 #define DEFER_BUF_JPEG 3  /* bytes of one JPEG file per sample, h * w * c of them: the first stage's input buffer only,   */
                           /* read only by DEFER_OP_JPEG_DECODE                                                             */
+#define DEFER_BUF_PNG 4   /* bytes of one PNG file per sample, DEFER_PNG_SLOT_BYTES(h, w) of them (c = 3): the first      */
+                          /* stage's input buffer only, read only by DEFER_OP_PNG_DECODE                                   */
 
 /* One logical tensor of the plan.  Shapes are per sample, NHWC; vectors use h = w = 1. */
 typedef struct defer_buf_desc {
   int32_t h, w, c;
-  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 | DEFER_BUF_JPEG */
+  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 | DEFER_BUF_JPEG | DEFER_BUF_PNG */
 } defer_buf_desc;
 
 /* One fused op of the plan.  Buffer ids index the defer_buf_desc array; weight ids index the
@@ -268,6 +304,13 @@ DEFER_API int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first
  * stream.  defer_stage_submit / _part / _parts / _frames refuse such a stage. */
 DEFER_API int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes);
+/* First stage with a DEFER_OP_PNG_DECODE op: the same contract as defer_stage_submit_jpegs, with PNG files of at most
+ * DEFER_PNG_SLOT_BYTES(H, W) bytes and DEFER_PNG_BLOCK_INTS-value blocks; each block's IDAT count must be at most
+ * DEFER_PNG_MAX_IDAT, its ranges inside the file, and its row length and filter unit those of its size, colour type and
+ * depth.  Only the block prefix a file uses is copied.  defer_stage_submit / _part / _parts / _frames / _jpegs refuse
+ * such a stage. */
+DEFER_API int defer_stage_submit_pngs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                             const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes);
 /* Enqueue microbatch `seq` on lane seq % depth: wait-input -> kernel chain -> hop -> flags. Async. */
 DEFER_API int defer_stage_step(defer_stage_t s, uint64_t seq);
 /* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host.  A lane keeps only the output
@@ -365,6 +408,14 @@ DEFER_API int defer_k_jpeg_workspace(int H, int W, int n, uint64_t* bytes, uint6
                                      uint64_t* plane_off);
 DEFER_API int defer_k_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace,
                                   uint8_t* y, void* stream);
+
+/* The whole DEFER_OP_PNG_DECODE of n samples: files = n slots of DEFER_PNG_SLOT_BYTES(H, W) bytes, blocks = n PNG blocks
+ * (layout above, 4-byte aligned), y = n U8 (H, W, 3) images; workspace of defer_k_png_workspace bytes, 256-byte aligned,
+ * caller-owned.  Per sample (sample_stride apart) the workspace holds the three stats above as its first int32 values,
+ * and from raw_off the scanlines, h * (1 + bytes per row), unfiltered (each row's filter type byte kept). */
+DEFER_API int defer_k_png_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* raw_off);
+DEFER_API int defer_k_png_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace,
+                                 uint8_t* y, void* stream);
 
 #ifdef __cplusplus
 }
