@@ -40,6 +40,18 @@ stream, and everything the stream produced before it stays:
     is then not applied (bits past the end read as zero while a code is looked up).
 The stream also ends, normally, when the output holds ``h * (1 + bytes per row)`` bytes: a match is cut there and
 whatever follows is not read, as Pillow stops reading once the image is full.  The Adler-32 trailer is not checked.
+Against zlib's ``inflate()`` given the same input and room for the image, this result differs in four cases only
+(tests/test_png_zlib_host.py checks that nothing else differs):
+  (a) a stored block whose data runs past the end of the input produces none of its bytes here (EXHAUSTED); zlib
+      produces the bytes that are there, and so fills the image when they reach its end;
+  (b) a dynamic header whose code-length code has no codes at all is refused at once (BAD_HEADER); zlib decodes each
+      of the HLIT + HDIST lengths as 0 from one bit and refuses the header for its missing end-of-block code;
+  (c) a repeat code 16 as the first code length is refused before its two extra bits are read (BAD_HEADER); zlib reads
+      them first;
+  (d) a distance code with no codes is refused when used, before any bit of the distance is read (BAD_SYMBOL); zlib
+      reads one bit first.
+In (b), (c) and (d) the bytes produced are the same and the status differs only when the input ends first, where zlib
+still waits for input (EXHAUSTED).
 The scanline bytes not produced are zero, and the unfilter and the conversion run over them as over the others.  A
 filter type byte above 4 makes its row unfiltered as type 0 (None).
 

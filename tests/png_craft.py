@@ -4,8 +4,10 @@
 ``BitWriter`` writes deflate blocks bit by bit (stored, fixed Huffman, dynamic Huffman with any code lengths, and raw
 header fields), so a test can build what zlib never emits: empty stored blocks, stored blocks that cross IDAT chunk
 boundaries, matches at distance 32768 and length 258, an overlapping match, a dynamic header whose repeat codes span the
-literal/length and distance lengths, one-code distance trees, and every corruption of the decode's defined result
-(defer_b200/png.py)."""
+literal/length and distance lengths, one-code distance trees, codes that use every length from 1 to 15, a one-bit
+end-of-block-only code, every corruption of the decode's defined result and each case where that result deviates from
+zlib (defer_b200/png.py).  ``filter_rows`` filters image rows forward, so a test can build a file of any size whose
+expected scanlines are known without an unfilter."""
 from __future__ import annotations
 
 import struct
@@ -183,6 +185,38 @@ def lit_lengths_for(symbols: Sequence[int], n: int = 286) -> List[int]:
     return lens
 
 
+# ------------------------------------------------------------------------------------------------- forward filters
+def filter_rows(x: np.ndarray, bpp: int, types: np.ndarray) -> bytes:
+    """The scanlines of image rows ``x`` (uint8 [h, bytes per row]) filtered forward with filter type ``types[r]`` on row
+    r, filter unit ``bpp``: each row's type byte and its bytes minus the predictor of the PNG specification.  Every
+    neighbour is known on this side, so all four predictors are whole-array operations (no unfilter is run)."""
+    h, bpr = x.shape
+    xi = x.astype(np.int16)
+    a = np.zeros_like(xi)
+    a[:, bpp:] = xi[:, :-bpp]
+    b = np.zeros_like(xi)
+    b[1:] = xi[:-1]
+    c = np.zeros_like(xi)
+    c[1:, bpp:] = xi[:-1, :-bpp]
+    p = a + b - c
+    pa, pb, pc = np.abs(p - a), np.abs(p - b), np.abs(p - c)
+    paeth = np.where((pa <= pb) & (pa <= pc), a, np.where(pb <= pc, b, c))
+    t = np.asarray(types, np.uint8)
+    rows = xi.copy()
+    for k, pred in ((1, a), (2, b), (3, (a + b) >> 1), (4, paeth)):
+        rows[t == k] -= pred[t == k]
+    return np.concatenate([t[:, None], (rows & 255).astype(np.uint8)], axis=1).tobytes()
+
+
+def encode(x: np.ndarray, w: int, depth: int, ctype: int, types, level: int = 1, chunk_bytes: int = 8192,
+           palette: Optional[bytes] = None) -> bytes:
+    """A PNG of scanline bytes ``x`` (uint8 [h, bytes per row]): ``filter_rows`` with per-row ``types``, zlib at
+    ``level``, IDAT chunks of ``chunk_bytes``."""
+    raw = filter_rows(x, max(1, CHANNELS[ctype] * depth // 8), types)
+    z = zlib.compress(raw, level)
+    return png_file(w, x.shape[0], depth, ctype, z, idat_sizes=[chunk_bytes] * (len(z) // chunk_bytes), palette=palette)
+
+
 # ------------------------------------------------------------------------------------------------- the corpus
 def _scan(w: int, h: int, depth: int, ctype: int, seed: int) -> bytes:
     """Scanlines with random filter types 0..4 and random bytes."""
@@ -260,7 +294,115 @@ def valid_cases() -> Dict[str, bytes]:
     data = bytes([1, 2, 1, 2])
     assert zlib.decompress(w.zlib(data)) == data
     out["dyn_empty_dist"] = png_file(3, 1, 8, 0, w.zlib(data))
+    out["dyn_lengths_1_to_15"] = lengths_1_to_15()
+    # a literal/length code whose only code is end-of-block, of one bit (incomplete, valid as in zlib), then the data
+    w = BitWriter()
+    w.huffman([], lit_lens=EOB_ONLY, dist_lens=[0])
+    w.huffman([], lit_lens=EOB_ONLY, dist_lens=[1])
+    w.stored(raw[:121], final=True)
+    assert zlib.decompress(w.zlib(raw[:121])) == raw[:121]
+    out["dyn_eob_only"] = png_file(40, 1, 8, 2, w.zlib(raw[:121]))
     return out
+
+
+EOB_ONLY = [0] * 256 + [1]                                            # HLIT = 257: end-of-block alone, code "0"
+
+# lengths_1_to_15: literal/length and distance codes, each complete and using every code length from 1 to 15 (lengths
+# 1..14 once and 15 twice); a literal, a length symbol and two distance symbols have 15-bit codes
+_LIT_1_15 = {0: 1, 257: 2, 1: 3, 265: 4, 2: 5, 269: 6, 3: 7, 273: 8, 4: 9, 277: 10, 7: 11, 281: 12, 100: 13, 256: 14,
+             255: 15, 285: 15}
+_DIST_1_15 = {27: 1, 3: 2, 26: 3, 8: 4, 28: 5, 11: 6, 15: 7, 14: 8, 17: 9, 20: 10, 23: 11, 5: 12, 4: 13, 2: 14,
+              0: 15, 29: 15}
+
+
+def lengths_1_to_15(seed: int = 5) -> bytes:
+    """An 8-bit grey 255x130 file of one dynamic block in the codes above, whose data uses every symbol of both codes:
+    the 10-bit lookup and the canonical walk of longer codes run in one table.  Filter type bytes (every 256th) are
+    0..4: a match that covers one has a distance that is a multiple of 256, so it copies another."""
+    assert sum(2.0 ** -v for v in _LIT_1_15.values()) == 1 and sum(2.0 ** -v for v in _DIST_1_15.values()) == 1
+    rng = np.random.default_rng(seed)
+    lits = [s for s in _LIT_1_15 if s < 256]
+    lsyms = [s - 257 for s in _LIT_1_15 if s > 256]
+    dsyms = list(_DIST_1_15)
+    n, out, items = 256 * 130, bytearray(), []
+    todo_l, todo_d = set(lsyms), set(dsyms)
+    used_lit = set()
+    while len(out) < n:
+        p = len(out)
+        item = None
+        if p % 256 and rng.random() < 0.6:
+            ls = int(rng.choice(sorted(todo_l) if todo_l and rng.random() < 0.5 else lsyms))
+            near = [d for d in (sorted(todo_d) if todo_d and rng.random() < 0.5 else dsyms) if png.DBASE[d] <= p]
+            ds = int(rng.choice(near)) if near else -1
+            if ds >= 0:
+                length = png.LBASE[ls] + int(rng.integers(0, 1 << png.LEXT[ls]))
+                lo, hi = png.DBASE[ds], min(p, png.DBASE[ds] + (1 << png.DEXT[ds]) - 1)
+                crosses = (p + length - 1) // 256 > p // 256
+                if crosses:                                           # a multiple of 256 in [lo, hi]
+                    lo, hi = -(-lo // 256), hi // 256
+                step = 256 if crosses else 1
+                if lo <= hi and p + length <= n:
+                    d = step * int(rng.integers(lo, hi + 1))
+                    item = ("m", length, d)
+                    todo_l.discard(ls)
+                    todo_d.discard(ds)
+                    for _ in range(length):
+                        out.append(out[-d])
+        if item is None:
+            v = int(rng.integers(0, 5)) if p % 256 == 0 else int(rng.choice(lits))
+            used_lit.add(v)
+            item = v
+            out.append(v)
+        items.append(item)
+    assert not todo_l and not todo_d and used_lit == set(lits), (todo_l, todo_d, used_lit)
+    lit = [0] * 286
+    for s, v in _LIT_1_15.items():
+        lit[s] = v
+    dist = [0] * 30
+    for s, v in _DIST_1_15.items():
+        dist[s] = v
+    w = BitWriter()
+    w.huffman(items, final=True, lit_lens=lit, dist_lens=dist)
+    data = bytes(out)
+    z = w.zlib(data)
+    assert zlib.decompress(z) == data and all(v <= 4 for v in data[::256])
+    return png_file(255, 130, 8, 0, z)
+
+
+def _ends_at_byte(body) -> BitWriter:
+    """A writer holding a non-final fixed block of j 9-bit literals (200) and then ``body(writer)``, with j in 0..7
+    chosen so that the bits end on a byte boundary: nothing past ``body`` for a decoder to read."""
+    for j in range(8):
+        w = BitWriter()
+        w.huffman([200] * j)
+        body(w)
+        if len(w.bits) % 8 == 0:
+            return w
+    raise AssertionError("no prefix aligns the body")
+
+
+def _empty_cl_header(w: BitWriter, zero_lengths: int):
+    """A final dynamic block header whose code-length code has no codes (HLIT 257, HDIST 1, HCLEN 4, all lengths 0),
+    then ``zero_lengths`` zero bits (zlib decodes each bit as code length 0)."""
+    w.put(1, 1)
+    w.put(2, 2)
+    w.put(0, 5)
+    w.put(0, 5)
+    w.put(0, 4)
+    w.put(0, 12)
+    w.put(0, zero_lengths)
+
+
+def _sixteen_first(w: BitWriter):
+    """A final dynamic block header whose first code length is repeat code 16, its 2 extra bits not written."""
+    w.put(1, 1)
+    w.put(2, 2)
+    w.put(0, 5)
+    w.put(0, 5)
+    w.put(0, 4)
+    for v in (1, 0, 0, 1):                                            # CL_ORDER 16, 17, 18, 0: codes 0 -> "0", 16 -> "1"
+        w.put(v, 3)
+    w.put_code(1, 1)
 
 
 def corrupt_cases() -> Dict[str, Tuple[bytes, int]]:
@@ -343,6 +485,28 @@ def corrupt_cases() -> Dict[str, Tuple[bytes, int]]:
     w.put(1, 1)
     w.put(0, 16)
     out["dyn_one_code_dist_unused"] = (f(w.zlib()), S.STATUS_BAD_SYMBOL)
+    w = BitWriter()                                                   # the one-code (end-of-block) tree fed code "1"
+    w.huffman([], lit_lens=EOB_ONLY, dist_lens=[0])
+    w.huffman(["noeob"], lit_lens=EOB_ONLY, dist_lens=[0], final=True)
+    w.put(1, 1)
+    w.put(0, 16)
+    out["dyn_eob_only_unused"] = (f(w.zlib()), S.STATUS_BAD_SYMBOL)
+    # the restatement's deviations from zlib (module docstring of defer_b200/png.py)
+    w = BitWriter()                                                   # a code-length code with no codes at all
+    w.stored(good[:10])
+    _empty_cl_header(w, 400)
+    out["dyn_empty_cl_code"] = (f(w.zlib()), S.STATUS_BAD_HEADER)
+    w = _ends_at_byte(lambda w: _empty_cl_header(w, 100))             # ... cut before its 258 code lengths
+    out["dyn_empty_cl_code_cut"] = (f(w.zlib()), S.STATUS_BAD_HEADER)
+    w = _ends_at_byte(_sixteen_first)                                 # repeat code 16 first, cut before its extra bits
+    out["dyn_16_first_cut"] = (f(w.zlib()), S.STATUS_BAD_HEADER)
+    w = _ends_at_byte(lambda w: w.huffman([1, 2, 3, ("sym", 257), "noeob"], lit_lens=lit_lengths_for([1, 2, 3, 257]),
+                                          dist_lens=[0], final=True))
+    out["dyn_empty_dist_used_at_end"] = (f(w.zlib()), S.STATUS_BAD_SYMBOL)   # an empty distance code, cut where used
+    w = BitWriter()                                                   # a stored block whose data runs past the input
+    w.stored(good[:10])
+    w.stored(good[10:50], final=True)
+    out["stored_truncated"] = (f(w.zlib()[:-15]), S.STATUS_EXHAUSTED)
     # scanlines with an unknown filter type: the stream is valid, the row unfilters as None
     raw = b"".join(bytes([ft]) + bytes(range(i, i + 19)) for i, ft in enumerate((7, 1, 200)))
     out["unknown_filter"] = (f(zlib.compress(raw)), S.STATUS_OK)

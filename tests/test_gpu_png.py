@@ -35,9 +35,10 @@ def _fixtures():
     return sorted(p.name for p in GOLDEN.glob("*.png"))
 
 
-def decode_dev(files, H, W, timed=False):
+def decode_dev(files, H, W, timed=False, fill=0x5A):
     """defer_k_png_decode of ``files`` in slots of the bound (H, W): (workspace [n, stride], raw offset, images [n, H*W*3]);
-    a None file is a never-written sample (zero slot, zero block).  ``timed``: also the decode's time in ms."""
+    a None file is a never-written sample (zero slot, zero block).  ``timed``: also the decode's time in ms; ``fill``: the
+    stale byte the workspace holds before the decode."""
     import torch
     lib = A.load()
     n = len(files)
@@ -50,7 +51,7 @@ def decode_dev(files, H, W, timed=False):
             png.pack_block(png.parse(d), blocks[i])
     total, stride, raw_off = (C.c_uint64() for _ in range(3))
     A.check(lib.defer_k_png_workspace(H, W, n, C.byref(total), C.byref(stride), C.byref(raw_off)))
-    ws = torch.full((total.value,), 0x5A, dtype=torch.uint8, device="cuda")        # stale bytes everywhere
+    ws = torch.full((total.value,), fill, dtype=torch.uint8, device="cuda")        # stale bytes everywhere
     x = torch.from_numpy(slots.reshape(-1)).cuda()
     b = torch.from_numpy(blocks.reshape(-1)).cuda()
     y = torch.full((n * H * W * 3,), 7, dtype=torch.uint8, device="cuda")
