@@ -12,15 +12,15 @@ from pathlib import Path
 
 import numpy as np
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 LINK_TOKEN_BYTES = 256
 
 # enums (include/defer_b200.h)
 FMT_F32, FMT_BF16X2, FMT_BF16 = 0, 1, 2
 OP_CONV, OP_MAXPOOL, OP_GAP, OP_DENSE, OP_SOFTMAX, OP_AFFINE, OP_RELU, OP_ADD, OP_PAD, OP_COPY, OP_PREPROCESS, OP_RESIZE = range(1, 13)
 FLAG_RELU, FLAG_RESIDUAL = 1, 2
-BUF_ACT, BUF_F32, BUF_U8, BUF_JPEG, BUF_PNG = 0, 1, 2, 3, 4
-OP_JPEG_DECODE, OP_PNG_DECODE = 13, 14
+BUF_ACT, BUF_F32, BUF_U8, BUF_JPEG, BUF_PNG, BUF_IMAGE = 0, 1, 2, 3, 4, 5
+OP_JPEG_DECODE, OP_PNG_DECODE, OP_IMAGE_DECODE = 13, 14, 15
 PRE_CAFFE, PRE_TF = 0, 1
 PRE_MODES = {"caffe": PRE_CAFFE, "tf": PRE_TF}
 RESIZE_SAMPLE_W, RESIZE_SAMPLE_H = 1, 2
@@ -32,7 +32,8 @@ OP_NAMES = {OP_CONV: "conv", OP_MAXPOOL: "maxpool", OP_GAP: "gap", OP_DENSE: "de
             OP_AFFINE: "affine", OP_RELU: "relu", OP_ADD: "add", OP_PAD: "pad", OP_COPY: "copy",
             OP_PREPROCESS: "preprocess"}
 #: OP_NAMES covers the ops of a model and of its preprocess_input; KIND_NAMES adds RESIZE, the load_img resize in front
-KIND_NAMES = {**OP_NAMES, OP_RESIZE: "resize", OP_JPEG_DECODE: "jpeg_decode", OP_PNG_DECODE: "png_decode"}
+KIND_NAMES = {**OP_NAMES, OP_RESIZE: "resize", OP_JPEG_DECODE: "jpeg_decode", OP_PNG_DECODE: "png_decode",
+              OP_IMAGE_DECODE: "image_decode"}
 
 
 class BufDesc(C.Structure):
@@ -78,6 +79,7 @@ PROTOTYPES = {
     "defer_stage_submit_frames": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_submit_jpegs": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_submit_pngs": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
+    "defer_stage_submit_images": (_i, [_vp, _u64, _i, _i, C.POINTER(_vp), _vp, _vp, _u64]),
     "defer_stage_step": (_i, [_vp, _u64]),
     "defer_stage_result": (_i, [_vp, _u64, _vp, _u64]),
     "defer_stage_predict": (_i, [_vp, _vp, _u64, _vp, _u64]),
@@ -113,6 +115,8 @@ PROTOTYPES = {
     "defer_k_jpeg_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "defer_k_png_workspace": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "defer_k_png_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    "defer_k_image_workspace": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "defer_k_image_decode": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 _LIB = None

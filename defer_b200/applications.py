@@ -28,6 +28,7 @@ from . import keras_like as K
 from .resize import INTERPOLATIONS, resize_image  # noqa: F401  (Keras load_img's resize, keep_aspect_ratio too, as Pillow)
 from .jpeg import decode_jpeg  # noqa: F401  (Keras load_img's JPEG decode of baseline and progressive files, bit for bit as Pillow)
 from .png import decode_png  # noqa: F401  (Keras load_img's PNG decode of non-interlaced files, bit for bit as Pillow)
+from .image import decode_image  # noqa: F401  (either of the two, told by the file's first bytes as Pillow does)
 from .keras_like import (Activation, Add, BatchNormalization, Conv2D, Dense, Flatten,
                          GlobalAveragePooling2D, Input, MaxPooling2D, Model, ZeroPadding2D)
 

@@ -9,7 +9,7 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = HERE / "lib" / "libdefer_b200.so"
-SOURCES = ["stage.cu", "kernels_simt.cu", "conv_umma.cu", "api_kernels.cu", "jpeg.cu", "png.cu"]
+SOURCES = ["stage.cu", "kernels_simt.cu", "conv_umma.cu", "api_kernels.cu", "jpeg.cu", "png.cu", "image.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC,-fvisibility=hidden", "-DDEFER_BUILD"]
 

@@ -199,20 +199,42 @@ int launch_resize(const uint8_t* x, uint8_t* y, const int32_t* bounds, const int
 // samples reads its size and tables from its int32 block in `tables` (layout: include/defer_b200.h).
 int launch_resize_frames(int pass, const uint8_t* x, uint8_t* y, const int32_t* tables, int n, int H, int W, int H_out,
                          int W_out, int kw_w, int kw_h, cudaStream_t st);
+// Where one decode launch finds sample s: its file at files + s * file, its block at blocks + s * block_ints, its
+// workspace at workspace + s * ws; and which samples it decodes (decode_takes).  The single-format ops pass nullptr and
+// derive them from (H, W); DEFER_OP_IMAGE_DECODE passes the image slot's, and one format per launch.
+struct DecodeStrides {
+  size_t file, ws;
+  int block_ints;
+  int take;   // 0: every sample; DEFER_IMAGE_JPEG: those tagged JPEG; DEFER_IMAGE_PNG: every sample not tagged JPEG
+};
+__device__ __forceinline__ bool decode_takes(const int32_t* blk, int take) {
+  return take == 0 || (blk[DEFER_IMAGE_TAG] == DEFER_IMAGE_JPEG) == (take == DEFER_IMAGE_JPEG);
+}
 // DEFER_OP_JPEG_DECODE (jpeg.cu): n JPEG files in H * W * 3-byte slots, with their blocks -> n U8 (H, W, 3) images, through a
 // workspace of jpeg_workspace_bytes(H, W, n) (256-byte aligned)
 size_t jpeg_workspace_bytes(int H, int W, int n);
+// one sample's workspace bytes (a multiple of 256), and where its coefficients and planes start
+size_t jpeg_ws_stride(int H, int W, size_t* coef_off, size_t* plane_off);
 // the bounds (H, W) the decode takes: H * W * 24 + DEFER_JPEG_SUBSEQ_BITS < 2^31
 bool jpeg_bound_ok(int H, int W);
 int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
-                       cudaStream_t st);
+                       cudaStream_t st, const DecodeStrides* strides = nullptr);
 // DEFER_OP_PNG_DECODE (png.cu): n PNG files in DEFER_PNG_SLOT_BYTES(H, W)-byte slots, with their blocks -> n U8 (H, W, 3)
 // images, through a workspace of png_workspace_bytes(H, W, n) (256-byte aligned)
 size_t png_workspace_bytes(int H, int W, int n);
+// one sample's workspace bytes (a multiple of 256), and where its scanlines start
+size_t png_ws_stride(int H, int W, size_t* raw_off);
 // the bounds (H, W) the decode takes: the slot fits the blocks' int32 offsets
 bool png_bound_ok(int H, int W);
 int launch_png_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
-                      cudaStream_t st);
+                      cudaStream_t st, const DecodeStrides* strides = nullptr);
+// DEFER_OP_IMAGE_DECODE (image.cu): n JPEG or PNG files in DEFER_PNG_SLOT_BYTES(H, W)-byte slots, with their tagged
+// blocks -> n U8 (H, W, 3) images, through a workspace of image_workspace_bytes(H, W, n) (256-byte aligned)
+size_t image_workspace_bytes(int H, int W, int n);
+// the bounds (H, W) both decodes take
+bool image_bound_ok(int H, int W);
+int launch_image_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
+                        cudaStream_t st);
 
 // flag protocol kernels (see stage.cu)
 int launch_wait_flag(const uint32_t* flag, uint32_t* counter, int minus, int* status, unsigned long long timeout_ns,

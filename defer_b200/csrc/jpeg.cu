@@ -183,7 +183,10 @@ struct SegSum {
 struct JpegWs {
   size_t stats, coef, planes, comp, seg_start, seg_total, sub_base, sub, stride;
   int mcu_cap, blocks_cap, subs_cap;
-  size_t slot;
+  size_t slot;      // H * W * 3: the extent clamp of a file, and the image stride
+  size_t file;      // the file slot stride (DecodeStrides)
+  int block_ints;   // the block stride
+  int take;         // which samples (decode_takes)
 };
 enum { SUB_SEG, SUB_EPOS, SUB_EJK, SUB_XPOS, SUB_XJK, SUB_CNT, SUB_PRE, SUB_PPOS, SUB_PJK, SUB_FIELDS };
 
@@ -205,6 +208,9 @@ __host__ __device__ inline JpegWs jpeg_ws(int H, int W) {
   L.sub_base = o;   o += al(((size_t)L.mcu_cap + 1) * 4);
   L.sub = o;        o += al((size_t)L.subs_cap * SUB_FIELDS * 4);
   L.stride = o;
+  L.file = L.slot;
+  L.block_ints = DEFER_JPEG_BLOCK_INTS;
+  L.take = 0;
   return L;
 }
 
@@ -711,7 +717,8 @@ __global__ void __launch_bounds__(JT) jpeg_entropy_kernel(const uint8_t* __restr
   __shared__ int tabs[6 * HUFF];
   __shared__ int sh_int[8];
   const int s = blockIdx.x, tid = threadIdx.x;
-  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
   const Geom g = geom(blk, H, W, L.slot);
   uint8_t* base = ws + (size_t)s * L.stride;
   int32_t* stats = reinterpret_cast<int32_t*>(base + L.stats);
@@ -723,12 +730,12 @@ __global__ void __launch_bounds__(JT) jpeg_entropy_kernel(const uint8_t* __restr
   int32_t* sub = reinterpret_cast<int32_t*>(base + L.sub);
   auto F = [&](int field, int t) -> int32_t& { return sub[(size_t)field * L.subs_cap + t]; };
   if (blk[10] != 0) {
-    progressive_decode(files + (size_t)s * L.slot, blk, g, L, base, tabs, tmp.i, tmp.p, sh_int);
+    progressive_decode(files + (size_t)s * L.file, blk, g, L, base, tabs, tmp.i, tmp.p, sh_int);
     return;
   }
   for (int i = tid; i < 6 * HUFF; i += JT) tabs[i] = blk[T_OFF + i];
   int T, R, nsubs;
-  unstuff_intervals(files + (size_t)s * L.slot + g.off, g.len, g.nseg, comp, seg_start, seg_total, sub_base, L.subs_cap,
+  unstuff_intervals(files + (size_t)s * L.file + g.off, g.len, g.nseg, comp, seg_start, seg_total, sub_base, L.subs_cap,
                     tmp.i, T, R, nsubs);
   // ---- 3. every subsequence decodes from the default state at its first bit
   for (int t = tid; t < nsubs; t += JT) {
@@ -930,7 +937,8 @@ __global__ void __launch_bounds__(IDCT_BLOCKS * 8) jpeg_idct_kernel(const int32_
                                                                     int H, int W, JpegWs L) {
   __shared__ int wsp[IDCT_BLOCKS][64];
   const int s = blockIdx.y, lb = threadIdx.x >> 3, r = threadIdx.x & 7;
-  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
   const Geom g = geom(blk, H, W, L.slot);
   const int b = blockIdx.x * IDCT_BLOCKS + lb;
   if (b >= g.blocks) return;               // the 8 threads of a block leave together
@@ -986,7 +994,8 @@ __device__ __forceinline__ int upsample(const uint8_t* __restrict__ p, int rs, i
 __global__ void __launch_bounds__(256) jpeg_color_kernel(const int32_t* __restrict__ blocks, const uint8_t* __restrict__ ws,
                                                          uint8_t* __restrict__ y_out, int H, int W, JpegWs L) {
   const int s = blockIdx.y;
-  const int32_t* blk = blocks + (size_t)s * DEFER_JPEG_BLOCK_INTS;
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
   const Geom g = geom(blk, H, W, L.slot);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= g.h * g.w) return;
@@ -1014,12 +1023,25 @@ __global__ void __launch_bounds__(256) jpeg_color_kernel(const int32_t* __restri
 
 size_t jpeg_workspace_bytes(int H, int W, int n) { return jpeg_ws(H, W).stride * (size_t)n; }
 
+size_t jpeg_ws_stride(int H, int W, size_t* coef_off, size_t* plane_off) {
+  const JpegWs L = jpeg_ws(H, W);
+  if (coef_off) *coef_off = L.coef;
+  if (plane_off) *plane_off = L.planes;
+  return L.stride;
+}
+
 // Bit positions in the entropy kernel are ints: the last subsequence's end, up to slot * 8 + S_BITS, must fit in one
 bool jpeg_bound_ok(int H, int W) { return (uint64_t)H * W * 3 * 8 + S_BITS < (1ull << 31); }
 
 int launch_jpeg_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
-                       cudaStream_t st) {
-  const JpegWs L = jpeg_ws(H, W);
+                       cudaStream_t st, const DecodeStrides* strides) {
+  JpegWs L = jpeg_ws(H, W);
+  if (strides) {
+    L.file = strides->file;
+    L.stride = strides->ws;
+    L.block_ints = strides->block_ints;
+    L.take = strides->take;
+  }
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   prefer_max_smem(jpeg_entropy_kernel);
   jpeg_entropy_kernel<<<n, JT, 0, st>>>(files, blocks, ws, H, W, L);

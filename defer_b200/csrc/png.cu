@@ -21,7 +21,10 @@ namespace defer {
 
 // Per-sample workspace layout (byte offsets from the sample's base); host and device compute it the same way.
 struct PngWs {
-  size_t slot, stats, stream, raw, stride;
+  size_t slot, stats, stream, raw, stride;   // slot: the extent clamp of a file
+  size_t file;                               // the file slot stride (DecodeStrides)
+  int block_ints;                            // the block stride
+  int take;                                  // which samples (decode_takes)
 };
 
 __host__ __device__ inline PngWs png_ws(int H, int W) {
@@ -33,6 +36,9 @@ __host__ __device__ inline PngWs png_ws(int H, int W) {
   L.stream = o;  o += al(L.slot + 64);                      // the gathered zlib stream, zero past its end
   L.raw = o;     o += al((size_t)H * (1 + 8 * (size_t)W));  // the scanlines, unfiltered in place
   L.stride = o;
+  L.file = L.slot;
+  L.block_ints = DEFER_PNG_BLOCK_INTS;
+  L.take = 0;
   return L;
 }
 
@@ -331,9 +337,10 @@ __global__ void __launch_bounds__(IT) png_inflate_kernel(const uint8_t* __restri
                                                          uint8_t* ws, int H, int W, PngWs L) {
   __shared__ Tables t;
   const int s = blockIdx.x;
-  const int32_t* blk = blocks + (size_t)s * DEFER_PNG_BLOCK_INTS;
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
   const PGeom g = pgeom(blk, H, W);
-  const uint8_t* file = files + (size_t)s * L.slot;
+  const uint8_t* file = files + (size_t)s * L.file;
   uint8_t* base = ws + (size_t)s * L.stride;
   uint8_t* st = base + L.stream;
   // gather the IDAT payloads, each range clamped into the file slot and the total into the stream's room (the slot)
@@ -367,7 +374,9 @@ __device__ __forceinline__ int paeth(int a, int b, int c) {
 // Unfilter in place: bytes at or past `produced` read as zero (the scanlines the stream did not produce)
 __global__ void __launch_bounds__(UT) png_unfilter_kernel(const int32_t* __restrict__ blocks, uint8_t* ws, int H, int W, PngWs L) {
   const int s = blockIdx.x;
-  const PGeom g = pgeom(blocks + (size_t)s * DEFER_PNG_BLOCK_INTS, H, W);
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
+  const PGeom g = pgeom(blk, H, W);
   uint8_t* base = ws + (size_t)s * L.stride;
   uint8_t* raw = base + L.raw;
   int32_t* stats = reinterpret_cast<int32_t*>(base + L.stats);
@@ -416,7 +425,8 @@ __device__ __forceinline__ int low_sample(const uint8_t* row, int x, int d) {
 __global__ void __launch_bounds__(256) png_expand_kernel(const int32_t* __restrict__ blocks, const uint8_t* __restrict__ ws,
                                                          uint8_t* __restrict__ y_out, int H, int W, PngWs L) {
   const int s = blockIdx.y;
-  const int32_t* blk = blocks + (size_t)s * DEFER_PNG_BLOCK_INTS;
+  const int32_t* blk = blocks + (size_t)s * L.block_ints;
+  if (!decode_takes(blk, L.take)) return;
   const PGeom g = pgeom(blk, H, W);
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= g.h * g.w) return;
@@ -452,12 +462,24 @@ __global__ void __launch_bounds__(256) png_expand_kernel(const int32_t* __restri
 
 size_t png_workspace_bytes(int H, int W, int n) { return png_ws(H, W).stride * (size_t)n; }
 
+size_t png_ws_stride(int H, int W, size_t* raw_off) {
+  const PngWs L = png_ws(H, W);
+  if (raw_off) *raw_off = L.raw;
+  return L.stride;
+}
+
 // IDAT offsets and lengths in the block are int32: the slot must fit
 bool png_bound_ok(int H, int W) { return H >= 1 && W >= 1 && DEFER_PNG_SLOT_BYTES((uint64_t)H, (uint64_t)W) < (1ull << 31); }
 
 int launch_png_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace, uint8_t* y,
-                      cudaStream_t st) {
-  const PngWs L = png_ws(H, W);
+                      cudaStream_t st, const DecodeStrides* strides) {
+  PngWs L = png_ws(H, W);
+  if (strides) {
+    L.file = strides->file;
+    L.stride = strides->ws;
+    L.block_ints = strides->block_ints;
+    L.take = strides->take;
+  }
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   png_inflate_kernel<<<n, IT, 0, st>>>(files, blocks, ws, H, W, L);
   png_unfilter_kernel<<<n, UT, 0, st>>>(blocks, ws, H, W, L);

@@ -119,7 +119,7 @@ struct Lane {
   bool timed = false;
   void* peer_out = nullptr;   // HOP_COPY: this lane's input slot on the consumer GPU (destination of the hop copy)
   int32_t* tables = nullptr;  // DEFER_RESIZE_SAMPLE_*: `batch` table blocks, next to the lane's input slot in the arena
-  int32_t* dec_blocks = nullptr;   // DEFER_OP_JPEG_DECODE / _PNG_DECODE: `batch` JPEG or PNG blocks, after the table blocks
+  int32_t* dec_blocks = nullptr;   // DEFER_OP_JPEG_DECODE / _PNG_DECODE / _IMAGE_DECODE: `batch` blocks, after the table blocks
   void* dec_ws = nullptr;          // ... and its decode workspace
   // the microbatch the lane ran last (last stage: the one out_host is filled with); result() refuses any other
   bool stepped = false;
@@ -183,12 +183,12 @@ struct defer_stage_s {
     size_t block_ints = 0;        // int32 values per sample block
     size_t tables_off = 0;        // offset of a lane's blocks from its input slot
   } frames;
-  // JPEG or PNG files at ingress: the DEFER_OP_JPEG_DECODE or _PNG_DECODE op (-1 = none) in front of the per-sample
-  // resize pair
+  // JPEG or PNG files at ingress: the DEFER_OP_JPEG_DECODE, _PNG_DECODE or _IMAGE_DECODE op (-1 = none) in front of the
+  // per-sample resize pair
   struct Decode {
     int op = -1;
     int kind = 0;                 // its op kind
-    size_t block_ints = 0;        // DEFER_JPEG_BLOCK_INTS or DEFER_PNG_BLOCK_INTS
+    size_t block_ints = 0;        // DEFER_JPEG_BLOCK_INTS, DEFER_PNG_BLOCK_INTS or DEFER_IMAGE_BLOCK_INTS
     size_t blocks_off = 0;        // offset of a lane's blocks from its input slot
     size_t ws_bytes = 0;          // decode workspace per lane
   } dec;
@@ -203,13 +203,15 @@ struct defer_stage_s {
 namespace defer {
 
 static size_t elem_bytes(int elem, int fmt) {
-  return elem == DEFER_BUF_U8 || elem == DEFER_BUF_JPEG || elem == DEFER_BUF_PNG ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
+  const bool bytes = elem == DEFER_BUF_U8 || elem == DEFER_BUF_JPEG || elem == DEFER_BUF_PNG || elem == DEFER_BUF_IMAGE;
+  return bytes ? 1 : elem == DEFER_BUF_F32 ? 4 : fmt_bytes_per_elem(fmt);
 }
 
 static size_t buf_bytes(const Buf& b, int fmt) { return b.elems * elem_bytes(b.elem, fmt); }
 
-// the files a stage with a decode op takes, for messages: "JPEG" / "jpeg" or "PNG" / "png"
+// the files a stage with a decode op takes, for messages: "JPEG" / "jpeg", "PNG" / "png" or "JPEG or PNG" / "image"
 static const char* dec_name(const defer_stage_s* s, bool upper) {
+  if (s->dec.kind == DEFER_OP_IMAGE_DECODE) return upper ? "JPEG or PNG" : "image";
   return s->dec.kind == DEFER_OP_PNG_DECODE ? (upper ? "PNG" : "png") : (upper ? "JPEG" : "jpeg");
 }
 
@@ -301,6 +303,8 @@ static int launch_op(defer_stage_s* s, int lane_id, int oi, cudaStream_t st) {
       return launch_jpeg_decode((const uint8_t*)x, L.dec_blocks, nb, bi.h, bi.w, L.dec_ws, (uint8_t*)y, st);
     case DEFER_OP_PNG_DECODE:
       return launch_png_decode((const uint8_t*)x, L.dec_blocks, nb, bi.h, bi.w, L.dec_ws, (uint8_t*)y, st);
+    case DEFER_OP_IMAGE_DECODE:
+      return launch_image_decode((const uint8_t*)x, L.dec_blocks, nb, bi.h, bi.w, L.dec_ws, (uint8_t*)y, st);
     case DEFER_OP_RESIZE:
       if (d.mode == DEFER_RESIZE_SAMPLE_W || d.mode == DEFER_RESIZE_SAMPLE_H) {
         const auto& f = s->frames;
@@ -409,6 +413,12 @@ static void op_costs(defer_stage_s* s, OpRt& op) {
       op.alg_bytes = 3.0 * (double)bi.bytes + 3.0 * nb * bi.h * (1.0 + 8.0 * bi.w) + out_b;
       op.alg_flops = 0;
       break;
+    case DEFER_OP_IMAGE_DECODE: {   // an upper bound: every sample as the larger of a JPEG and a PNG of the slot's size
+      const double blocks_cap = 3.0 * ((bi.h + 15) / 16 * 2) * ((bi.w + 15) / 16 * 2);
+      op.alg_bytes = 3.0 * (double)bi.bytes + nb * std::max(blocks_cap * (128.0 + 64.0), 3.0 * bi.h * (1.0 + 8.0 * bi.w)) + out_b;
+      op.alg_flops = 0;
+      break;
+    }
     default:
       op.alg_bytes = in_b + out_b;
       op.alg_flops = 0;
@@ -488,7 +498,7 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     b.h = bufs[i].h; b.w = bufs[i].w; b.c = bufs[i].c; b.elem = bufs[i].elem;
     if (b.h < 1 || b.w < 1 || b.c < 1 ||
         (b.elem != DEFER_BUF_ACT && b.elem != DEFER_BUF_F32 && b.elem != DEFER_BUF_U8 && b.elem != DEFER_BUF_JPEG &&
-         b.elem != DEFER_BUF_PNG)) {
+         b.elem != DEFER_BUF_PNG && b.elem != DEFER_BUF_IMAGE)) {
       set_error("buffer %d: bad descriptor (%d,%d,%d,elem %d)", i, b.h, b.w, b.c, b.elem);
       return fail(DEFER_ERR_INVALID);
     }
@@ -496,10 +506,10 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
       bool resized = false;
       for (int j = 0; j < n_ops; ++j)
         resized |= ops[j].out == i && (ops[j].kind == DEFER_OP_RESIZE || ops[j].kind == DEFER_OP_JPEG_DECODE ||
-                                       ops[j].kind == DEFER_OP_PNG_DECODE);
+                                       ops[j].kind == DEFER_OP_PNG_DECODE || ops[j].kind == DEFER_OP_IMAGE_DECODE);
       if (!cfg->is_first || (i != cfg->input_buf && !resized)) {
         set_error("buffer %d: a U8 buffer is legal only as the first stage's input buffer or the output of a RESIZE, "
-                  "JPEG_DECODE or PNG_DECODE op", i);
+                  "JPEG_DECODE, PNG_DECODE or IMAGE_DECODE op", i);
         return fail(DEFER_ERR_INVALID);
       }
     }
@@ -514,9 +524,15 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
                 "DEFER_PNG_SLOT_BYTES(H, W) < 2^31", i);
       return fail(DEFER_ERR_INVALID);
     }
+    if (b.elem == DEFER_BUF_IMAGE && (!cfg->is_first || i != cfg->input_buf || b.c != 3 || !image_bound_ok(b.h, b.w))) {
+      set_error("buffer %d: an image buffer is legal only as the first stage's input buffer, (H, W, 3) with "
+                "H * W * 24 + %d < 2^31 and DEFER_PNG_SLOT_BYTES(H, W) < 2^31", i, DEFER_JPEG_SUBSEQ_BITS);
+      return fail(DEFER_ERR_INVALID);
+    }
     b.elems = (size_t)cfg->batch * b.h * b.w * b.c;
-    b.bytes = b.elem == DEFER_BUF_PNG ? (size_t)cfg->batch * DEFER_PNG_SLOT_BYTES((size_t)b.h, (size_t)b.w)
-                                      : buf_bytes(b, cfg->fmt);
+    b.bytes = b.elem == DEFER_BUF_PNG || b.elem == DEFER_BUF_IMAGE
+                  ? (size_t)cfg->batch * DEFER_PNG_SLOT_BYTES((size_t)b.h, (size_t)b.w)
+                  : buf_bytes(b, cfg->fmt);
     s->bufs.push_back(b);
   }
   if (cfg->is_first && s->bufs[cfg->input_buf].elem == DEFER_BUF_ACT) {
@@ -589,6 +605,11 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     }
     if ((bi.elem == DEFER_BUF_PNG) != (d.kind == DEFER_OP_PNG_DECODE) || (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_PNG)) {
       set_error("op %d: a PNG buffer is read only by a PNG_DECODE op (as in0), which reads nothing else", i);
+      return fail(DEFER_ERR_INVALID);
+    }
+    if ((bi.elem == DEFER_BUF_IMAGE) != (d.kind == DEFER_OP_IMAGE_DECODE) ||
+        (d.in1 >= 0 && s->bufs[d.in1].elem == DEFER_BUF_IMAGE)) {
+      set_error("op %d: an image buffer is read only by an IMAGE_DECODE op (as in0), which reads nothing else", i);
       return fail(DEFER_ERR_INVALID);
     }
     if (d.kind != DEFER_OP_PREPROCESS && d.kind != DEFER_OP_RESIZE && d.mode != 0) {
@@ -803,6 +824,20 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
         s->dec.kind = d.kind;
         s->dec.block_ints = DEFER_PNG_BLOCK_INTS;
         break;
+      case DEFER_OP_IMAGE_DECODE:
+        op.kname = "jpeg_entropy_kernel+jpeg_idct_kernel+jpeg_color_kernel+png_inflate_kernel+png_unfilter_kernel+"
+                   "png_expand_kernel";
+        op.n_kernels = 6;
+        if (d.in0 != cfg->input_buf || bo.elem != DEFER_BUF_U8 || bo.h != bi.h || bo.w != bi.w || bo.c != 3 || d.in1 >= 0 ||
+            d.flags || d.mode || d.w_kernel >= 0 || d.w_scale >= 0 || d.w_shift >= 0 || s->dec.op >= 0) {
+          set_error("op %d (image decode): maps the stage's image input (H, W, 3) to a U8 (H, W, 3) buffer, once, with no "
+                    "weights, in1, flags or mode (and no other decode op)", i);
+          return fail(DEFER_ERR_INVALID);
+        }
+        s->dec.op = i;
+        s->dec.kind = d.kind;
+        s->dec.block_ints = DEFER_IMAGE_BLOCK_INTS;
+        break;
       default:
         set_error("op %d: unknown kind %d", i, d.kind);
         return fail(DEFER_ERR_INVALID);
@@ -824,8 +859,8 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     f.block_ints = 2 + (size_t)f.W_out * (2 + f.kw_w) + (size_t)f.H_out * (2 + f.kw_h);
   }
   if (s->dec.op >= 0 && (s->frames.op_w < 0 || ops[s->frames.op_w].in0 != ops[s->dec.op].out)) {
-    set_error("the %s_DECODE op (op %d) feeds the per-sample resize pair: its output is SAMPLE_W's input", dec_name(s, true),
-              s->dec.op);
+    set_error("the %s_DECODE op (op %d) feeds the per-sample resize pair: its output is SAMPLE_W's input",
+              s->dec.kind == DEFER_OP_IMAGE_DECODE ? "IMAGE" : dec_name(s, true), s->dec.op);
     return fail(DEFER_ERR_INVALID);
   }
   for (int i = 0; i < n_ops; ++i)
@@ -876,8 +911,9 @@ int defer_stage_create(const defer_stage_config* cfg, const defer_buf_desc* bufs
     const Buf& bi = s->bufs[cfg->input_buf];
     s->dec.blocks_off = s->slot_stride;
     s->slot_stride += ((size_t)cfg->batch * s->dec.block_ints * 4 + 1023) / 1024 * 1024;
-    s->dec.ws_bytes = s->dec.kind == DEFER_OP_PNG_DECODE ? png_workspace_bytes(bi.h, bi.w, cfg->batch)
-                                                         : jpeg_workspace_bytes(bi.h, bi.w, cfg->batch);
+    s->dec.ws_bytes = s->dec.kind == DEFER_OP_PNG_DECODE     ? png_workspace_bytes(bi.h, bi.w, cfg->batch)
+                      : s->dec.kind == DEFER_OP_IMAGE_DECODE ? image_workspace_bytes(bi.h, bi.w, cfg->batch)
+                                                             : jpeg_workspace_bytes(bi.h, bi.w, cfg->batch);
   }
   s->arena_bytes = CTRL_BYTES + s->slot_stride * cfg->depth;
   if (cudaMalloc((void**)&s->arena, s->arena_bytes) != cudaSuccess) {
@@ -1441,6 +1477,82 @@ int defer_stage_submit_frames(defer_stage_t s, uint64_t seq, int first_index, in
   return DEFER_OK;
 }
 
+}  // extern "C"
+
+namespace defer {
+
+// The checks of one JPEG file of a submit call (`who` names it in the messages): its size within 4..slot, its block's
+// size within the bound and equal to its resize block's, and its entropy data inside the file.
+static int check_jpeg_file(const char* who, const defer_stage_s* s, int i, uint64_t nbytes, uint64_t slot, const int32_t* rb,
+                           const int32_t* jb) {
+  const auto& f = s->frames;
+  DEFER_CHECK(nbytes >= 4 && nbytes <= slot, "%s: file %d has %llu bytes, the slot takes 4..%llu", who, i,
+              (unsigned long long)nbytes, (unsigned long long)slot);
+  DEFER_CHECK(jb[0] >= 1 && jb[0] <= f.H && jb[1] >= 1 && jb[1] <= f.W, "%s: file %d is %dx%d, the slot takes 1..%d x "
+              "1..%d", who, i, jb[0], jb[1], f.H, f.W);
+  DEFER_CHECK(rb[0] == jb[0] && rb[1] == jb[1], "%s: resize block %d is for %dx%d, JPEG block %d for %dx%d", who, i, rb[0],
+              rb[1], i, jb[0], jb[1]);
+  DEFER_CHECK(jb[6] >= 0 && jb[7] >= 0 && (uint64_t)jb[6] + (uint64_t)jb[7] <= nbytes,
+              "%s: file %d: entropy data [%d, %d + %d) outside its %llu bytes", who, i, jb[6], jb[6], jb[7],
+              (unsigned long long)nbytes);
+  DEFER_CHECK(jb[10] >= 0 && jb[10] <= DEFER_JPEG_MAX_SCANS && jb[11] >= 0 && jb[11] <= DEFER_JPEG_MAX_TABLES,
+              "%s: file %d: %d scans and %d Huffman tables, at most %d and %d", who, i, jb[10], jb[11],
+              DEFER_JPEG_MAX_SCANS, DEFER_JPEG_MAX_TABLES);
+  for (int k = 0; k < jb[10]; ++k) {
+    const int32_t* sc = jb + DEFER_JPEG_SCAN_OFF + k * DEFER_JPEG_SCAN_INTS;
+    DEFER_CHECK(sc[9] >= 0 && sc[10] >= 0 && (uint64_t)sc[9] + (uint64_t)sc[10] <= nbytes,
+                "%s: file %d: scan %d's entropy data [%d, %d + %d) outside its %llu bytes", who, i, k, sc[9], sc[9],
+                sc[10], (unsigned long long)nbytes);
+  }
+  return DEFER_OK;
+}
+
+// the prefix of a checked JPEG block that its file uses: a baseline file's DEFER_JPEG_BASE_INTS, a progressive one's pool
+static size_t jpeg_used_ints(const int32_t* jb) {
+  return jb[10] ? (size_t)DEFER_JPEG_POOL_OFF + (size_t)jb[11] * DEFER_JPEG_HUFF_INTS : (size_t)DEFER_JPEG_BASE_INTS;
+}
+
+// The checks of one PNG file of a submit call: its size within 8..slot, its block's size within the bound and equal to
+// its resize block's, its row length and filter unit those of its size, colour type and depth, and its IDAT chunks
+// inside the file and summing to its stream length.
+static int check_png_file(const char* who, const defer_stage_s* s, int i, uint64_t nbytes, uint64_t slot, const int32_t* rb,
+                          const int32_t* pb) {
+  const auto& f = s->frames;
+  DEFER_CHECK(nbytes >= 8 && nbytes <= slot, "%s: file %d has %llu bytes, the slot takes 8..%llu", who, i,
+              (unsigned long long)nbytes, (unsigned long long)slot);
+  DEFER_CHECK(pb[0] >= 1 && pb[0] <= f.H && pb[1] >= 1 && pb[1] <= f.W, "%s: file %d is %dx%d, the slot takes 1..%d x "
+              "1..%d", who, i, pb[0], pb[1], f.H, f.W);
+  DEFER_CHECK(rb[0] == pb[0] && rb[1] == pb[1], "%s: resize block %d is for %dx%d, PNG block %d for %dx%d", who, i, rb[0],
+              rb[1], i, pb[0], pb[1]);
+  const int ct = pb[2], d = pb[3];
+  const int ch = ct == 0 ? 1 : ct == 2 ? 3 : ct == 3 ? 1 : ct == 4 ? 2 : ct == 6 ? 4 : 0;
+  const bool depth_ok = d == 8 || (d == 16 && ct != 3) || ((d == 1 || d == 2 || d == 4) && (ct == 0 || ct == 3));
+  DEFER_CHECK(ch && depth_ok && pb[4] == (int)(((int64_t)pb[1] * ch * d + 7) / 8) && pb[5] == std::max(1, ch * d / 8),
+              "%s: file %d: colour type %d, depth %d, %d bytes per row and filter unit %d do not match", who, i, ct, d,
+              pb[4], pb[5]);
+  DEFER_CHECK(pb[6] >= 1 && pb[6] <= DEFER_PNG_MAX_IDAT && pb[8] >= 0 && pb[8] <= 256,
+              "%s: file %d: %d IDAT chunks (1..%d) and %d palette entries (0..256)", who, i, pb[6], DEFER_PNG_MAX_IDAT,
+              pb[8]);
+  int64_t total = 0;
+  for (int k = 0; k < pb[6]; ++k) {
+    const int32_t off = pb[DEFER_PNG_IDAT_OFF + 2 * k], len = pb[DEFER_PNG_IDAT_OFF + 2 * k + 1];
+    DEFER_CHECK(off >= 0 && len >= 0 && (uint64_t)off + (uint64_t)len <= nbytes,
+                "%s: file %d: IDAT chunk %d [%d, %d + %d) outside its %llu bytes", who, i, k, off, off, len,
+                (unsigned long long)nbytes);
+    total += len;
+  }
+  DEFER_CHECK(total == pb[7], "%s: file %d: its IDAT chunks hold %lld bytes, its block says %d", who, i, (long long)total,
+              pb[7]);
+  return DEFER_OK;
+}
+
+// the prefix of a checked PNG block that its file uses: header, palette and its IDAT ranges
+static size_t png_used_ints(const int32_t* pb) { return (size_t)DEFER_PNG_IDAT_OFF + 2 * (size_t)pb[6]; }
+
+}  // namespace defer
+
+extern "C" {
+
 int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes) {
   DEFER_CHECK(s && data && nbytes && blocks && n >= 1, "submit_jpegs: bad arguments");
@@ -1455,26 +1567,8 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
   const uint64_t slot = (uint64_t)f.H * f.W * 3;
   for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
     const int32_t* rb = blocks + (size_t)i * per;
-    const int32_t* jb = rb + f.block_ints;
     DEFER_CHECK(data[i], "submit_jpegs: file %d is null", i);
-    DEFER_CHECK(nbytes[i] >= 4 && nbytes[i] <= slot, "submit_jpegs: file %d has %llu bytes, the slot takes 4..%llu", i,
-                (unsigned long long)nbytes[i], (unsigned long long)slot);
-    DEFER_CHECK(jb[0] >= 1 && jb[0] <= f.H && jb[1] >= 1 && jb[1] <= f.W, "submit_jpegs: file %d is %dx%d, the slot takes 1..%d x "
-                "1..%d", i, jb[0], jb[1], f.H, f.W);
-    DEFER_CHECK(rb[0] == jb[0] && rb[1] == jb[1], "submit_jpegs: resize block %d is for %dx%d, JPEG block %d for %dx%d", i, rb[0],
-                rb[1], i, jb[0], jb[1]);
-    DEFER_CHECK(jb[6] >= 0 && jb[7] >= 0 && (uint64_t)jb[6] + (uint64_t)jb[7] <= nbytes[i],
-                "submit_jpegs: file %d: entropy data [%d, %d + %d) outside its %llu bytes", i, jb[6], jb[6], jb[7],
-                (unsigned long long)nbytes[i]);
-    DEFER_CHECK(jb[10] >= 0 && jb[10] <= DEFER_JPEG_MAX_SCANS && jb[11] >= 0 && jb[11] <= DEFER_JPEG_MAX_TABLES,
-                "submit_jpegs: file %d: %d scans and %d Huffman tables, at most %d and %d", i, jb[10], jb[11],
-                DEFER_JPEG_MAX_SCANS, DEFER_JPEG_MAX_TABLES);
-    for (int k = 0; k < jb[10]; ++k) {
-      const int32_t* sc = jb + DEFER_JPEG_SCAN_OFF + k * DEFER_JPEG_SCAN_INTS;
-      DEFER_CHECK(sc[9] >= 0 && sc[10] >= 0 && (uint64_t)sc[9] + (uint64_t)sc[10] <= nbytes[i],
-                  "submit_jpegs: file %d: scan %d's entropy data [%d, %d + %d) outside its %llu bytes", i, k, sc[9], sc[9],
-                  sc[10], (unsigned long long)nbytes[i]);
-    }
+    DEFER_TRY(check_jpeg_file("submit_jpegs", s, i, nbytes[i], slot, rb, rb + f.block_ints));
   }
   DEFER_TRY(set_device(s));
   Lane& L = s->lanes[seq % s->cfg.depth];
@@ -1484,10 +1578,7 @@ int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_index, int
   DEFER_CUDA(cudaMemcpy2DAsync(L.tables + (size_t)first_index * f.block_ints, f.block_ints * 4, blocks, per * 4,
                                f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
   // each JPEG block's prefix that its file uses (a baseline file: DEFER_JPEG_BASE_INTS), in one copy when all are baseline
-  auto used = [&](int i) {
-    const int32_t* jb = blocks + (size_t)i * per + f.block_ints;
-    return jb[10] ? (size_t)DEFER_JPEG_POOL_OFF + (size_t)jb[11] * DEFER_JPEG_HUFF_INTS : (size_t)DEFER_JPEG_BASE_INTS;
-  };
+  auto used = [&](int i) { return jpeg_used_ints(blocks + (size_t)i * per + f.block_ints); };
   bool all_base = true;
   for (int i = 0; i < n; ++i) all_base &= used(i) == DEFER_JPEG_BASE_INTS;
   if (all_base) {
@@ -1516,33 +1607,8 @@ int defer_stage_submit_pngs(defer_stage_t s, uint64_t seq, int first_index, int 
   const uint64_t slot = DEFER_PNG_SLOT_BYTES((uint64_t)f.H, (uint64_t)f.W);
   for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
     const int32_t* rb = blocks + (size_t)i * per;
-    const int32_t* pb = rb + f.block_ints;
     DEFER_CHECK(data[i], "submit_pngs: file %d is null", i);
-    DEFER_CHECK(nbytes[i] >= 8 && nbytes[i] <= slot, "submit_pngs: file %d has %llu bytes, the slot takes 8..%llu", i,
-                (unsigned long long)nbytes[i], (unsigned long long)slot);
-    DEFER_CHECK(pb[0] >= 1 && pb[0] <= f.H && pb[1] >= 1 && pb[1] <= f.W, "submit_pngs: file %d is %dx%d, the slot takes 1..%d x "
-                "1..%d", i, pb[0], pb[1], f.H, f.W);
-    DEFER_CHECK(rb[0] == pb[0] && rb[1] == pb[1], "submit_pngs: resize block %d is for %dx%d, PNG block %d for %dx%d", i, rb[0],
-                rb[1], i, pb[0], pb[1]);
-    const int ct = pb[2], d = pb[3];
-    const int ch = ct == 0 ? 1 : ct == 2 ? 3 : ct == 3 ? 1 : ct == 4 ? 2 : ct == 6 ? 4 : 0;
-    const bool depth_ok = d == 8 || (d == 16 && ct != 3) || ((d == 1 || d == 2 || d == 4) && (ct == 0 || ct == 3));
-    DEFER_CHECK(ch && depth_ok && pb[4] == (int)(((int64_t)pb[1] * ch * d + 7) / 8) && pb[5] == std::max(1, ch * d / 8),
-                "submit_pngs: file %d: colour type %d, depth %d, %d bytes per row and filter unit %d do not match", i, ct, d,
-                pb[4], pb[5]);
-    DEFER_CHECK(pb[6] >= 1 && pb[6] <= DEFER_PNG_MAX_IDAT && pb[8] >= 0 && pb[8] <= 256,
-                "submit_pngs: file %d: %d IDAT chunks (1..%d) and %d palette entries (0..256)", i, pb[6], DEFER_PNG_MAX_IDAT,
-                pb[8]);
-    int64_t total = 0;
-    for (int k = 0; k < pb[6]; ++k) {
-      const int32_t off = pb[DEFER_PNG_IDAT_OFF + 2 * k], len = pb[DEFER_PNG_IDAT_OFF + 2 * k + 1];
-      DEFER_CHECK(off >= 0 && len >= 0 && (uint64_t)off + (uint64_t)len <= nbytes[i],
-                  "submit_pngs: file %d: IDAT chunk %d [%d, %d + %d) outside its %llu bytes", i, k, off, off, len,
-                  (unsigned long long)nbytes[i]);
-      total += len;
-    }
-    DEFER_CHECK(total == pb[7], "submit_pngs: file %d: its IDAT chunks hold %lld bytes, its block says %d", i, (long long)total,
-                pb[7]);
+    DEFER_TRY(check_png_file("submit_pngs", s, i, nbytes[i], slot, rb, rb + f.block_ints));
   }
   DEFER_TRY(set_device(s));
   Lane& L = s->lanes[seq % s->cfg.depth];
@@ -1553,8 +1619,49 @@ int defer_stage_submit_pngs(defer_stage_t s, uint64_t seq, int first_index, int 
                                f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
   for (int i = 0; i < n; ++i) {   // each PNG block's prefix that its file uses: header, palette and its IDAT ranges
     const int32_t* pb = blocks + (size_t)i * per + f.block_ints;
-    DEFER_CUDA(cudaMemcpyAsync(L.dec_blocks + (size_t)(first_index + i) * DEFER_PNG_BLOCK_INTS, pb,
-                               ((size_t)DEFER_PNG_IDAT_OFF + 2 * (size_t)pb[6]) * 4, cudaMemcpyHostToDevice, L.stream));
+    DEFER_CUDA(cudaMemcpyAsync(L.dec_blocks + (size_t)(first_index + i) * DEFER_PNG_BLOCK_INTS, pb, png_used_ints(pb) * 4,
+                               cudaMemcpyHostToDevice, L.stream));
+  }
+  return DEFER_OK;
+}
+
+int defer_stage_submit_images(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes) {
+  DEFER_CHECK(s && data && nbytes && blocks && n >= 1, "submit_images: bad arguments");
+  DEFER_CHECK(s->cfg.is_first, "submit_images: only the first stage takes host input");
+  DEFER_CHECK(s->dec.kind == DEFER_OP_IMAGE_DECODE, "submit_images: the stage has no DEFER_OP_IMAGE_DECODE op");
+  const auto& f = s->frames;
+  DEFER_CHECK(first_index >= 0 && first_index <= s->cfg.batch - n, "submit_images: samples [%d, %d) outside the microbatch of %d",
+              first_index, first_index + n, s->cfg.batch);
+  const size_t per = f.block_ints + DEFER_IMAGE_BLOCK_INTS;    // one file's resize block, then its tagged block
+  DEFER_CHECK(block_bytes == (uint64_t)n * per * 4, "submit_images: got %llu block bytes, %d files take %zu",
+              (unsigned long long)block_bytes, n, (size_t)n * per * 4);
+  const uint64_t slot = DEFER_PNG_SLOT_BYTES((uint64_t)f.H, (uint64_t)f.W);
+  const uint64_t jpeg_slot = (uint64_t)f.H * f.W * 3;          // a JPEG's bit positions are ints (jpeg_bound_ok)
+  for (int i = 0; i < n; ++i) {   // all checks first: a refused call copies nothing
+    const int32_t* rb = blocks + (size_t)i * per;
+    const int32_t* b = rb + f.block_ints;
+    DEFER_CHECK(data[i], "submit_images: file %d is null", i);
+    DEFER_CHECK(b[DEFER_IMAGE_TAG] == DEFER_IMAGE_JPEG || b[DEFER_IMAGE_TAG] == DEFER_IMAGE_PNG,
+                "submit_images: file %d: block tag %d, neither DEFER_IMAGE_JPEG (%d) nor DEFER_IMAGE_PNG (%d)", i,
+                b[DEFER_IMAGE_TAG], DEFER_IMAGE_JPEG, DEFER_IMAGE_PNG);
+    if (b[DEFER_IMAGE_TAG] == DEFER_IMAGE_JPEG)
+      DEFER_TRY(check_jpeg_file("submit_images", s, i, nbytes[i], jpeg_slot, rb, b));
+    else
+      DEFER_TRY(check_png_file("submit_images", s, i, nbytes[i], slot, rb, b));
+  }
+  DEFER_TRY(set_device(s));
+  Lane& L = s->lanes[seq % s->cfg.depth];
+  uint8_t* dst = (uint8_t*)L.buf[s->cfg.input_buf];
+  for (int i = 0; i < n; ++i)   // the file's own bytes only, at the start of its sample slot
+    DEFER_CUDA(cudaMemcpyAsync(dst + (size_t)(first_index + i) * slot, data[i], nbytes[i], cudaMemcpyHostToDevice, L.stream));
+  DEFER_CUDA(cudaMemcpy2DAsync(L.tables + (size_t)first_index * f.block_ints, f.block_ints * 4, blocks, per * 4,
+                               f.block_ints * 4, n, cudaMemcpyHostToDevice, L.stream));
+  for (int i = 0; i < n; ++i) {   // each block's prefix that its file uses, in its format's layout (the tag is in both)
+    const int32_t* b = blocks + (size_t)i * per + f.block_ints;
+    const size_t used = b[DEFER_IMAGE_TAG] == DEFER_IMAGE_JPEG ? jpeg_used_ints(b) : png_used_ints(b);
+    DEFER_CUDA(cudaMemcpyAsync(L.dec_blocks + (size_t)(first_index + i) * DEFER_IMAGE_BLOCK_INTS, b, used * 4,
+                               cudaMemcpyHostToDevice, L.stream));
   }
   return DEFER_OK;
 }
@@ -1732,7 +1839,7 @@ int defer_stage_read_buffer(defer_stage_t s, int lane, int buf_id, float* host_o
                 op.aff_op, buf_id);
   }
   DEFER_CUDA(cudaStreamSynchronize(s->lanes[lane].stream));
-  if (b.elem == DEFER_BUF_PNG) {   // the first h * w * 3 bytes of each sample's slot
+  if (b.elem == DEFER_BUF_PNG || b.elem == DEFER_BUF_IMAGE) {   // the first h * w * 3 bytes of each sample's slot
     const size_t per = (size_t)b.h * b.w * b.c, slot = b.bytes / s->cfg.batch;
     std::vector<uint8_t> raw(b.elems);
     DEFER_CUDA(cudaMemcpy2D(raw.data(), per, src, slot, per, s->cfg.batch, cudaMemcpyDeviceToHost));

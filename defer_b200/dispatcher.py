@@ -35,7 +35,9 @@ share a microbatch, and each gives exactly what ``image_size=(h, w)`` would.  On
 With ``decode="jpeg"`` as well, each queue item is a baseline JPEG file (``open(path, "rb").read()``); the first GPU
 decodes it exactly as ``load_img`` does with Pillow (``jpeg.decode_jpeg``), so only the compressed file crosses PCIe
 and the host only parses its markers.  ``decode="png"`` does the same for non-interlaced PNG files (``png.decode_png``);
-the host only walks their chunk headers.  A pipeline decodes one of the two formats.  ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``, and with
+the host only walks their chunk headers.  ``decode="image"`` takes both in one pipeline: each item's format is told
+from its first bytes, as ``PIL.Image.open`` does, never from a file name, and JPEG and PNG files share a microbatch
+(``image.decode_image``).  ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``, and with
 ``decode="jpeg"``) resizes each image's centred crop with the model input's aspect ratio instead of squashing the whole
 image, as ``load_img(..., keep_aspect_ratio=True)`` does: ``applications.resize_image(item, (H, W), interpolation,
 keep_aspect_ratio=True)``.
@@ -59,7 +61,8 @@ import numpy as np
 from . import keras_like as K
 from .applications import check_model_preprocess, check_preprocess
 from .jpeg import check_decode, check_jpeg
-from .png import DECODES, check_png
+from .image import DECODES, check_image
+from .png import check_png
 from .resize import check_frame, check_interpolation, check_keep_aspect_ratio, check_size
 from .dag_util import construct_model
 from .node import DTYPE_TO_FMT, StageRunner, parse_device
@@ -74,7 +77,8 @@ class DEFER:
                  keep_aspect_ratio: bool = False) -> None:
         check_decode(decode, preprocess, image_size, max_image_size, DECODES)
         if decode is not None and batch not in (None, 1):
-            raise ValueError(f"decode={decode!r}: a queue item is one {decode.upper()} file, so batch must be 1, got {batch}")
+            what = "JPEG or PNG" if decode == "image" else decode.upper()
+            raise ValueError(f"decode={decode!r}: a queue item is one {what} file, so batch must be 1, got {batch}")
         if preprocess is not None:
             check_preprocess(preprocess)
         check_interpolation(interpolation)
@@ -98,7 +102,7 @@ class DEFER:
         self.interpolation = interpolation
         self.keep_aspect_ratio = keep_aspect_ratio  # resize Keras' centred crop of each image (load_img keep_aspect_ratio)
         self.max_image_size = max_image_size  # None | (H, W): uint8 queue items of any size up to it, resized on stage 0
-        self.decode = decode                # None | "jpeg" | "png": queue items are JPEG / PNG files, decoded on stage 0
+        self.decode = decode                # None | "jpeg" | "png" | "image": JPEG / PNG / either files, decoded on stage 0
         self.dispatchIP = "localhost"       # reference: socket.gethostbyname(...) (dispatcher.py:23); no sockets here
         self.chunk_size = 512 * 1000        # kept for interface parity (dispatcher.py:24)
         self.dtype = dtype
@@ -205,8 +209,11 @@ class DEFER:
             def submit_items(seq, group):
                 first.submit_frames(seq, 0, group)
         files = self.decode is not None      # JPEG or PNG files
-        check_file = check_png if self.decode == "png" else check_jpeg
-        if files:                            # the files, parsed here, decoded on the GPU
+        check_file = {"jpeg": check_jpeg, "png": check_png, "image": check_image}.get(self.decode)
+        if files and self.decode == "image":  # each file sniffed and parsed here, either format in one group
+            def submit_items(seq, group):
+                first.submit_images(seq, 0, [d for d, _, _ in group], group)
+        elif files:                          # the files, parsed here, decoded on the GPU
             submit_files = first.submit_pngs if self.decode == "png" else first.submit_jpegs
 
             def submit_items(seq, group):
@@ -227,7 +234,7 @@ class DEFER:
                 in_shape = None
                 while True:
                     x = model_input
-                    if files:                        # (file bytes, header): refused files raise here, as bad items do
+                    if files:                        # (file bytes[, kind], header): refused files raise here, as bad items do
                         x = check_file(x, bound)
                     elif bound is not None:          # any size up to the bound: no same-shape rule within a group
                         x = check_frame(x, bound)

@@ -520,18 +520,19 @@ def pack_block(info: JpegInfo, out: Optional[np.ndarray] = None) -> np.ndarray:
     return b
 
 
-DECODES = ("jpeg",)               # the format this module parses; png.DECODES: every format a pipeline decodes
+DECODES = ("jpeg",)               # the format this module parses; image.DECODES: every format a pipeline decodes
 
 
 def check_decode(decode, preprocess, image_size, max_image_size, decodes=DECODES) -> None:
     """``decode=`` of ``DEFER`` / ``plan_stage``: None, or one of ``decodes`` together with ``preprocess`` and
-    ``max_image_size``.  The pipelines pass ``png.DECODES``, which adds "png"."""
+    ``max_image_size``.  The pipelines pass ``image.DECODES``, which adds "png" and "image" (either, told per file)."""
     if decode is None:
         return
     if decode not in decodes:
         raise ValueError(f"decode={decode!r}: the GPU decodes {', '.join(map(repr, decodes))} files")
     if image_size is not None:
-        raise ValueError(f"decode={decode!r} and image_size={image_size}: each {decode.upper()} carries its own size; give "
+        what = "image file" if decode == "image" else decode.upper()
+        raise ValueError(f"decode={decode!r} and image_size={image_size}: each {what} carries its own size; give "
                          "max_image_size=(H, W), the largest image the pipeline takes")
     if preprocess is None or max_image_size is None:
         raise ValueError(f"decode={decode!r} needs preprocess= and max_image_size=: the decoded images are resized and "

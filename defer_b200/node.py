@@ -24,7 +24,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .node_state import NodeState
 from .planner import Plan, plan_stage
-from . import png
+from . import image, png
 from .jpeg import BLOCK_INTS, check_jpeg, pack_block
 from .resize import check_frame, pack_frame_tables
 
@@ -86,7 +86,8 @@ class StageRunner:
         self.resizes = any(o.kind == A.OP_RESIZE for o in plan.ops)
         # planned with max_image_size=: images of mixed sizes, fed by submit_frames with their table blocks
         self.frames = plan.frames
-        self.decode = plan.decode                    # "jpeg" / "png": fed by submit_jpegs / submit_pngs, files with blocks
+        # "jpeg" / "png" / "image": fed by submit_jpegs / submit_pngs / submit_images, files with their blocks
+        self.decode = plan.decode
         self._tables: Dict[int, tuple] = {}          # per lane: blocks, sizes and images of its latest microbatch (kept alive)
         self.in_shape = (self.batch,) + tuple(plan.input_shape)
         self.out_shape = (self.batch,) + tuple(plan.output_shape)
@@ -128,7 +129,8 @@ class StageRunner:
         ``decode="jpeg"`` (with ``preprocess`` and ``max_image_size``): inputs are baseline JPEG files of images up to
         ``(H, W)``, decoded on the GPU as Keras' ``load_img`` does (``jpeg.decode_jpeg``); feed them with
         ``submit_jpegs`` / ``predict_jpegs``.  ``decode="png"``: the same for non-interlaced PNG files (``png.decode_png``),
-        fed with ``submit_pngs`` / ``predict_pngs``.
+        fed with ``submit_pngs`` / ``predict_pngs``.  ``decode="image"``: either format, told apart per file by its first
+        bytes as Pillow does (``image.decode_image``), in one microbatch; fed with ``submit_images`` / ``predict_images``.
         ``keep_aspect_ratio=True`` (with ``image_size`` or ``max_image_size``): each image's centred crop with the model
         input's aspect ratio is resized, as ``load_img(..., keep_aspect_ratio=True)`` does (``resize.keras_crop_box``)."""
         plan = plan_stage(model, is_first=is_first, is_last=is_last, preprocess=preprocess, image_size=image_size,
@@ -235,7 +237,8 @@ class StageRunner:
         if self.frames is None:
             raise ValueError(f"{self.name}: submit_frames needs a stage planned with max_image_size=")
         if self.decode is not None:
-            raise ValueError(f"{self.name}: this stage takes {self.decode.upper()} files; feed them with "
+            what = "JPEG and PNG" if self.decode == "image" else self.decode.upper()
+            raise ValueError(f"{self.name}: this stage takes {what} files; feed them with "
                              f"submit_{self.decode}s / predict_{self.decode}s")
         bound = self.frames["max_image_size"]
         images = []
@@ -268,6 +271,7 @@ class StageRunner:
         parsed here (``jpeg.check_jpeg``: a refused file raises a ValueError and nothing is copied); one C call copies each
         file's own bytes and then the blocks.  ``infos``: the items' ``jpeg.check_jpeg`` headers when the caller has
         already checked them (the items are then ``bytes``).  Same lifetime rule as ``submit``."""
+        self._refuse_images("submit_jpegs")
         if self.decode != "jpeg":
             raise ValueError(f"{self.name}: submit_jpegs needs a stage planned with decode='jpeg'")
         bound = self.frames["max_image_size"]
@@ -301,6 +305,7 @@ class StageRunner:
         """Ingress of a ``decode="png"`` stage, as ``submit_jpegs``: ``items`` are PNG files, their chunks are walked here
         (``png.check_png``: a refused file raises a ValueError and nothing is copied), and one C call copies each file's
         own bytes and then its resize block and the part of its PNG block it uses."""
+        self._refuse_images("submit_pngs")
         if self.decode != "png":
             raise ValueError(f"{self.name}: submit_pngs needs a stage planned with decode='png'")
         bound = self.frames["max_image_size"]
@@ -327,6 +332,47 @@ class StageRunner:
     def predict_pngs(self, items) -> np.ndarray:
         """Single-stage ``model.predict`` of a ``decode="png"`` stage: the outputs of the PNG files ``items``, in order."""
         self.submit_pngs(0, 0, items)
+        self.step(0)
+        return self.result(0)[:len(items)]
+
+    def _refuse_images(self, call: str) -> None:
+        if self.decode == "image":
+            raise ValueError(f"{self.name}: {call} needs a single-format stage; this stage takes JPEG and PNG files told "
+                             "apart per file: feed them with submit_images / predict_images")
+
+    def submit_images(self, seq: int, index: int, items, checked=None) -> None:
+        """Ingress of a ``decode="image"`` stage, as ``submit_jpegs``: each of ``items`` is a JPEG or a PNG file, told
+        apart by its first bytes and checked here (``image.check_image``: a refused file raises a ValueError and nothing
+        is copied).  One C call copies each file's own bytes and then its resize block and the part of its tagged block
+        that it uses.  ``checked``: the items' ``image.check_image`` results when the caller has already checked them
+        ((bytes, kind, header) each).  Same lifetime rule as ``submit``."""
+        if self.decode != "image":
+            raise ValueError(f"{self.name}: submit_images needs a stage planned with decode='image'")
+        bound = self.frames["max_image_size"]
+        if checked is None:
+            checked = [image.check_image(x, bound) for x in items]
+        n = len(checked)
+        if not 1 <= n <= self.batch - index or index < 0:
+            raise ValueError(f"{self.name}: {n} files from sample {index} do not fit the microbatch of {self.batch}")
+        files = [d for d, _, _ in checked]
+        hw = np.array([(i.h, i.w) for _, _, i in checked], np.int32).reshape(n, 2)
+        tables = pack_frame_tables(hw, self.frames["target"], self.frames["kw"], self.frames["interpolation"],
+                                   self.frames.get("keep_aspect_ratio", False))
+        nr = tables.shape[1]
+        blocks = np.zeros((n, nr + image.BLOCK_INTS), np.int32)  # only the prefix each file uses is written and copied
+        blocks[:, :nr] = tables
+        for k, (_, kind, i) in enumerate(checked):
+            image.pack_block(kind, i, blocks[k, nr:])
+        sizes = np.array([len(f) for f in files], np.uint64)
+        self._tables[seq % self.depth] = (blocks, sizes, files)
+        ptrs = (C.c_void_p * n)(*[C.cast(C.c_char_p(f), C.c_void_p).value for f in files])
+        A.check(self.lib.defer_stage_submit_images(self.handle, seq, index, n, ptrs, sizes.ctypes.data,
+                                                   blocks.ctypes.data, blocks.nbytes))
+
+    def predict_images(self, items) -> np.ndarray:
+        """Single-stage ``model.predict`` of a ``decode="image"`` stage: the outputs of the JPEG or PNG files ``items``, in
+        order."""
+        self.submit_images(0, 0, items)
         self.step(0)
         return self.result(0)[:len(items)]
 

@@ -25,7 +25,9 @@ With ``max_image_size=(H, W)`` instead, the stage input is a uint8 slot of that 
 (``resize.pack_frame_tables``); the plan records what the feeder needs to pack them in ``Plan.frames``.  With
 ``decode="jpeg"`` as well, the stage input is a byte slot of ``H * W * 3`` per sample holding one JPEG file, and a
 ``JPEG_DECODE`` op in front of the resize pair decodes it into the uint8 slot (``jpeg.pack_block``); with ``decode="png"``
-the slot holds one PNG file (``png.slot_bytes(H, W)`` bytes) and a ``PNG_DECODE`` op takes that place (``png.pack_block``).
+the slot holds one PNG file (``png.slot_bytes(H, W)`` bytes) and a ``PNG_DECODE`` op takes that place (``png.pack_block``);
+with ``decode="image"`` the slot of that size holds one JPEG or PNG file and an ``IMAGE_DECODE`` op decodes each sample
+in its own format, told by the tag of its block (``image.pack_block``).
 ``keep_aspect_ratio=True`` resizes Keras' centred crop of each image instead (``resize.keras_crop_box``): with
 ``image_size`` the two ``RESIZE`` ops carry box tables, and an axis that keeps its length under a partial box is
 resampled by an op whose ``mode`` names its axis (``RESIZE_W`` / ``_H``); with ``max_image_size`` the feeder packs each
@@ -42,7 +44,7 @@ from . import _cabi as A
 from . import keras_like as K
 from .applications import caffe_shift, check_model_preprocess, check_preprocess
 from .jpeg import check_decode
-from .png import DECODES
+from .image import DECODES
 from .resize import check_interpolation, check_keep_aspect_ratio, check_size, crop_boxes, kcap, resize_tables
 
 
@@ -233,10 +235,10 @@ def plan_stage(model: K.Model, is_first: bool, is_last: bool, preprocess: Option
         h, w = image_size or max_image_size or (H, W)
         input_shape = (h, w, 3)
         files, op_decode = {None: (A.BUF_U8, None), "jpeg": (A.BUF_JPEG, A.OP_JPEG_DECODE),
-                            "png": (A.BUF_PNG, A.OP_PNG_DECODE)}[decode]
+                            "png": (A.BUF_PNG, A.OP_PNG_DECODE), "image": (A.BUF_IMAGE, A.OP_IMAGE_DECODE)}[decode]
         input_buf = img = new_buf((None,) + input_shape, files)
         if decode is not None:
-            # the files decode into the image slot the per-sample resize reads (jpeg.pack_block / png.pack_block per file)
+            # the files decode into the image slot the per-sample resize reads (jpeg / png / image.pack_block per file)
             img = emit(PlanOp(op_decode, img, new_buf((None,) + input_shape, A.BUF_U8),
                               layers=[f"load_img(decode {decode} <={h}x{w})"])).out
         if max_image_size is not None:

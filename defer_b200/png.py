@@ -88,7 +88,7 @@ STATUS_BAD_HEADER = 4             # a dynamic block header zlib refuses
 STATUS_BAD_SYMBOL = 5             # no code of its table, or a literal/length symbol 286-287 or distance 30-31
 STATUS_BAD_DISTANCE = 6           # a distance past the bytes produced
 
-#: the formats ``DEFER(decode=...)`` / ``plan_stage`` take (``jpeg.check_decode(..., decodes=DECODES)``)
+#: the single-format decodes (``image.DECODES`` adds "image", what ``DEFER(decode=...)`` / ``plan_stage`` take)
 DECODES = ("jpeg", "png")
 
 SIGNATURE = b"\x89PNG\r\n\x1a\n"

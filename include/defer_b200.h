@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DEFER_ABI_VERSION 1
+#define DEFER_ABI_VERSION 2
 
 #if defined(DEFER_BUILD)
 #define DEFER_API __attribute__((visibility("default")))
@@ -79,8 +79,10 @@ typedef enum defer_op_kind {
   DEFER_OP_JPEG_DECODE = 13, /* baseline JPEG files -> images (below): in0 = the stage input, a DEFER_BUF_JPEG (H, W, 3)   */
                          /*   slot per sample; out = U8 (H, W, 3), each image packed (h, w, 3) at the start of its sample;  */
                          /*   read by the DEFER_RESIZE_SAMPLE_W op.  No weights, mode 0.                                     */
-  DEFER_OP_PNG_DECODE = 14 /* non-interlaced PNG files -> images (below): as DEFER_OP_JPEG_DECODE, from a DEFER_BUF_PNG  */
+  DEFER_OP_PNG_DECODE = 14, /* non-interlaced PNG files -> images (below): as DEFER_OP_JPEG_DECODE, from a DEFER_BUF_PNG */
                          /*   (H, W, 3) input of DEFER_PNG_SLOT_BYTES(H, W) bytes per sample                                 */
+  DEFER_OP_IMAGE_DECODE = 15 /* JPEG or PNG files, each sample its own (below): as DEFER_OP_PNG_DECODE, from a           */
+                         /*   DEFER_BUF_IMAGE (H, W, 3) input of DEFER_PNG_SLOT_BYTES(H, W) bytes per sample                 */
 } defer_op_kind;
 
 /* defer_op_desc.mode of a DEFER_OP_RESIZE op.  0: the fixed-size resize above (one image size per stage).
@@ -181,6 +183,21 @@ typedef enum defer_op_kind {
  * chunk headers, and 64 KiB for the other chunks */
 #define DEFER_PNG_SLOT_BYTES(H, W) ((H) * (1 + 8 * (W)) + (H) * (1 + 8 * (W)) / 64 + 65536)
 
+/* DEFER_OP_IMAGE_DECODE decodes a microbatch whose samples are JPEG or PNG files, each told by its block's tag, bit for
+ * bit as the two single-format ops do (defer_b200/image.py).  It is planned where DEFER_OP_JPEG_DECODE is.  The sample's
+ * file sits at the start of its DEFER_PNG_SLOT_BYTES(H, W)-byte slot (the larger of the two slots; a JPEG file is still
+ * at most H * W * 3 bytes, as jpeg_bound_ok needs); its int32 block of DEFER_IMAGE_BLOCK_INTS values is the file's
+ * JPEG or PNG block in that format's layout, with the tag in [DEFER_IMAGE_TAG] (both layouts leave it zero, and the
+ * single-format ops never read it).  The op runs the three JPEG kernels on the samples tagged DEFER_IMAGE_JPEG, then the
+ * three PNG kernels on every other sample: a never-written (zeroed) sample decodes as in a PNG stage, to a 1x1 black
+ * image.  The CTAs of the other format's samples exit after reading the tag.  Each sample's workspace is the larger of
+ * the two formats' strides, and holds the layout (stats included) of the format that decoded it. */
+#define DEFER_IMAGE_TAG 15
+#define DEFER_IMAGE_JPEG 1
+#define DEFER_IMAGE_PNG 2
+#define DEFER_IMAGE_BLOCK_INTS \
+  (DEFER_JPEG_BLOCK_INTS > DEFER_PNG_BLOCK_INTS ? DEFER_JPEG_BLOCK_INTS : DEFER_PNG_BLOCK_INTS)
+
 /* defer_op_desc.mode of a DEFER_OP_PREPROCESS op (every other op kind: 0). */
 #define DEFER_PRE_CAFFE 0   /* keras_applications imagenet_utils mode='caffe' (ResNet50/101/152, VGG16) */
 #define DEFER_PRE_TF    1   /* mode='tf' (ResNet50V2/101V2/152V2): fl32(fl32(x / 127.5) - 1), bit for bit */
@@ -193,16 +210,20 @@ typedef enum defer_op_kind {
 #define DEFER_BUF_F32 1   /* plain fp32 regardless of the stage format (image in, probabilities out) */
 #define DEFER_BUF_U8  2   /* uint8 NHWC, 1 B/elem, first stage only: its input buffer or the output of a DEFER_OP_RESIZE; */
                           /* read only by DEFER_OP_RESIZE and DEFER_OP_PREPROCESS                                          */
-                          /* (or of a DEFER_OP_JPEG_DECODE)                                                                */
+                          /* (or of a DEFER_OP_JPEG_DECODE, _PNG_DECODE or _IMAGE_DECODE)                                  */
 #define DEFER_BUF_JPEG 3  /* bytes of one JPEG file per sample, h * w * c of them: the first stage's input buffer only,   */
                           /* read only by DEFER_OP_JPEG_DECODE                                                             */
 #define DEFER_BUF_PNG 4   /* bytes of one PNG file per sample, DEFER_PNG_SLOT_BYTES(h, w) of them (c = 3): the first      */
                           /* stage's input buffer only, read only by DEFER_OP_PNG_DECODE                                   */
+#define DEFER_BUF_IMAGE 5 /* bytes of one JPEG or PNG file per sample, DEFER_PNG_SLOT_BYTES(h, w) of them (c = 3): the    */
+                          /* first stage's input buffer only, (h, w) within both formats' bounds; read only by             */
+                          /* DEFER_OP_IMAGE_DECODE                                                                         */
 
 /* One logical tensor of the plan.  Shapes are per sample, NHWC; vectors use h = w = 1. */
 typedef struct defer_buf_desc {
   int32_t h, w, c;
-  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 | DEFER_BUF_JPEG | DEFER_BUF_PNG */
+  int32_t elem;            /* DEFER_BUF_ACT | DEFER_BUF_F32 | DEFER_BUF_U8 | DEFER_BUF_JPEG | DEFER_BUF_PNG |
+                              DEFER_BUF_IMAGE */
 } defer_buf_desc;
 
 /* One fused op of the plan.  Buffer ids index the defer_buf_desc array; weight ids index the
@@ -311,6 +332,13 @@ DEFER_API int defer_stage_submit_jpegs(defer_stage_t s, uint64_t seq, int first_
  * such a stage. */
 DEFER_API int defer_stage_submit_pngs(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes);
+/* First stage with a DEFER_OP_IMAGE_DECODE op: the same contract, with JPEG or PNG files and DEFER_IMAGE_BLOCK_INTS-value
+ * blocks, each tagged DEFER_IMAGE_JPEG or DEFER_IMAGE_PNG in [DEFER_IMAGE_TAG].  Each file meets the checks of
+ * defer_stage_submit_jpegs or _pngs for its tag; a JPEG file is at most H * W * 3 bytes, a PNG file at most
+ * DEFER_PNG_SLOT_BYTES(H, W).  Only the block prefix a file uses is copied.  Every other submit call refuses such a
+ * stage. */
+DEFER_API int defer_stage_submit_images(defer_stage_t s, uint64_t seq, int first_index, int n, const void* const* data,
+                              const uint64_t* nbytes, const int32_t* blocks, uint64_t block_bytes);
 /* Enqueue microbatch `seq` on lane seq % depth: wait-input -> kernel chain -> hop -> flags. Async. */
 DEFER_API int defer_stage_step(defer_stage_t s, uint64_t seq);
 /* Last stage only: block until microbatch `seq` is complete and copy its fp32 output to host.  A lane keeps only the output
@@ -416,6 +444,16 @@ DEFER_API int defer_k_jpeg_decode(const uint8_t* files, const int32_t* blocks, i
 DEFER_API int defer_k_png_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* raw_off);
 DEFER_API int defer_k_png_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace,
                                  uint8_t* y, void* stream);
+
+/* The whole DEFER_OP_IMAGE_DECODE of n samples: files = n slots of DEFER_PNG_SLOT_BYTES(H, W) bytes, blocks = n tagged
+ * blocks of DEFER_IMAGE_BLOCK_INTS values (4-byte aligned), y = n U8 (H, W, 3) images; workspace of
+ * defer_k_image_workspace bytes, 256-byte aligned, caller-owned.  Per sample (sample_stride apart) the workspace holds
+ * the layout of the format that decoded it: a JPEG sample's stats, coefficients from coef_off and planes from plane_off
+ * as defer_k_jpeg_decode writes them; a PNG sample's stats and scanlines from raw_off as defer_k_png_decode does. */
+DEFER_API int defer_k_image_workspace(int H, int W, int n, uint64_t* bytes, uint64_t* sample_stride, uint64_t* coef_off,
+                                      uint64_t* plane_off, uint64_t* raw_off);
+DEFER_API int defer_k_image_decode(const uint8_t* files, const int32_t* blocks, int n, int H, int W, void* workspace,
+                                   uint8_t* y, void* stream);
 
 #ifdef __cplusplus
 }
